@@ -14,7 +14,8 @@ every rank renders its block with no further communication, and ONE NCCL gather 
 mask to rank 0.  `--scaling weak` renders a whole frame on every rank (N frames per step) instead; at
 N > 1 the strong line carries the weak measurement as `weak_scaling`.  At N = 1 both are the same job.
 
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  `--dump-outputs DIR` also writes rgb / depth / mask of the last timed step
+(float32 .npy; the inputs are seeded, so two builds can be compared output for output).
 """
 
 import argparse
@@ -25,6 +26,7 @@ import sys
 import threading
 import time
 
+sys.dont_write_bytecode = True  # the tree may be read-only: no __pycache__ next to the sources
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -33,9 +35,6 @@ import torch  # noqa: E402
 
 KERNEL_CLASSES = ["view_static", "view_dynamic", "motion", "point1", "point2", "rgbhead", "attention",
                   "gather"]
-# DRAM bytes per (point, view) row of the static per-view kernel from the committed ncu capture
-# (dram__bytes_read.sum + dram__bytes_write.sum per launch / rows); see profiles/
-NCU_DRAM_BYTES_PER_ROW = {"view_static": 298.0}  # profiles/r02_view_twin_ncu.md (156.2 MB / 524 288 rows)
 
 WORKLOAD = dict(H=288, W=512, V_dy=8, V_st=8, N_samples=64, N_importance=64, chunk=8192, seed=0)
 METRIC = "rays/sec (64+64 samples x 8 src views)"
@@ -59,7 +58,15 @@ def parse():
                        "of memory', config.py:168; results do not depend on it)")
   ap.add_argument("--view-kernel", default="default", choices=["default", "twin", "quad", "pipe"],
                   help="per-view stage kernel: library default, twin-warp, quad schedule, or sub-round pipelined twin")
-  return ap.parse_args()
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="write rgb / depth / mask of the pixels the last timed step delivers to rank 0 (the gathered "
+                       "frame with several GPUs) as float32 .npy files into DIR")
+  a = ap.parse_args()
+  if a.steps < 1:
+    ap.error("--steps must be >= 1")
+  if a.dump_outputs and a.impl == "reference":
+    ap.error("--dump-outputs writes the outputs of this repository's path (--impl ours)")
+  return a
 
 
 def peaks():
@@ -68,7 +75,8 @@ def peaks():
     d = json.load(open(p))
     return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"],
                 source="measured (MEASURED_PEAKS.json)")
-  return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+  # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- not a measured rate
+  return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
@@ -135,7 +143,7 @@ def cpu_threads():
 
 def make_cpu_runner():
   """The reference's CPU implementation of the path on the same synthetic frame: the UNMODIFIED reference
-  (oracle/_ref, byte-compiled from /root/reference by oracle/build_ref.py) when it has been built,
+  (oracle/_ref, byte-compiled from a reference checkout by oracle/build_ref.py) when it has been built,
   else the oracle port (oracle/dynibar_oracle.py).  Returns (kind, fn(n_rays) -> None)."""
   torch.set_num_threads(cpu_threads())
   w = WORKLOAD
@@ -227,6 +235,15 @@ def train_step_line(dev, precision, rays=1024, steps=3):
           "loss_first": float(l0), "loss_last": float(l1)}
 
 
+def dump_outputs(path, px):
+  """rgb [rays,3], depth [rays], mask [rays] (float32) of the pixels px [rays,5]."""
+  import numpy as np
+  os.makedirs(path, exist_ok=True)
+  px = px.detach().float().cpu().numpy()
+  for name, arr in (("rgb", px[:, 0:3]), ("depth", px[:, 3]), ("mask", px[:, 4])):
+    np.save(os.path.join(path, name + ".npy"), np.ascontiguousarray(arr, dtype=np.float32))
+
+
 def main():
   a = parse()
   rank = int(os.environ.get("RANK", "0"))
@@ -238,7 +255,7 @@ def main():
                         "render_rays_mv, det=True, inv_uniform=True, chunk %d" % a.chunk,
             "rays_per_frame": a.rays, "precision": a.precision,
             "l2": "per-step working set (source maps 66 MB + GBs of per-chunk intermediates) exceeds the "
-                  "126 MB L2; plus an explicit 256 MB flush between steps"}
+                  "50 MB L2; plus an explicit 256 MB flush between steps"}
 
   if a.impl == "reference":
     if rank != 0:
@@ -321,12 +338,12 @@ def main():
                               self.args, inv_uniform=True, N_importance=w["N_importance"], det=True,
                               is_train=False)["outputs_fine_ref"]
         outs.append(torch.cat([r["rgb"], r["depth"][:, None], r["mask"][:, None].float()], 1))
-      px = torch.cat(outs, 0)
-      if world > 1:  # the path's one exchange step: rendered pixels -> rank 0 over NVLink
+      px = self.delivered = torch.cat(outs, 0)
+      if world > 1:  # the path's one exchange step: rendered pixels -> rank 0 over NVLink (None elsewhere)
         if self.mode == "strong":
-          dd.gather_pixels(px, self.n_total)
+          self.delivered = dd.gather_pixels(px, self.n_total)
         else:
-          dd.gather_pixels(px, px.shape[0] * world)
+          self.delivered = dd.gather_pixels(px, px.shape[0] * world)
       return px
 
     def step_resident(self):
@@ -385,6 +402,8 @@ def main():
   ms = timed(fr.step_resident, a.steps)
   launches = int(_lib.lib.dyn_launch_count(0))
   clocks = sampler.finish()
+  if a.dump_outputs and rank == 0:
+    dump_outputs(a.dump_outputs, fr.delivered)
   # ---- end to end: pinned host buffers in, pinned host pixels out, every step ----
   fr.step_e2e()
   ms_e2e = timed(fr.step_e2e, a.steps)
@@ -488,11 +507,11 @@ def main():
         "clocks": clocks, "gpu_launches": launches,
         "e2e": {"value": e2e_val, "unit": "rays/s", "h2d_bytes_per_step": int(h2d.item()),
                 "d2h_bytes_per_step": int(d2h.item()), "ms_per_step": ms_e2e / a.steps},
-        "roofline_step": {"bound": "tensor", "achieved": achieved, "peak": pk["tf_sustained"],
-                          "unit": "TFLOP/s", "frac": achieved / pk["tf_sustained"],
+        "roofline_step": {"bound": "not profiled (tensor peak as reference)", "achieved": achieved,
+                          "peak": pk["tf_sustained"], "unit": "TFLOP/s", "frac": achieved / pk["tf_sustained"],
                           "flop_per_ray": fpr, "flop_per_ray_essential": fpr - 2 * (S_tot * (
                               w["V_dy"] * (21 * 256 + 256 * 35) + w["V_st"] * 66 * 35)),
-                          "peak_source": pk["source"] + ", sustained bf16",
+                          "peak_source": pk["source"] + ", dense bf16",
                           "scope": "whole step (all kernels of render_rays_mv), per GPU"},
         "kernels": kernels,
         "kernels_how": "separate pass of %d step(s) after the headline run with dyn_profile_enable(1): CUDA events "
@@ -501,16 +520,13 @@ def main():
     line.update(extras)
     if dom is not None:
       kd = kernels[dom]
-      rows_step = {"view_static": n_loc * S_tot * w["V_st"]}.get(dom)
       line["roofline"] = {
-          "kernel": dom, "bound": "tensor", "achieved": kd["tflops"], "peak": pk["tf_sustained"],
-          "unit": "TFLOP/s", "frac": kd["tflops"] / pk["tf_sustained"],
+          "kernel": dom, "bound": "not profiled (tensor peak as reference)", "achieved": kd["tflops"],
+          "peak": pk["tf_sustained"], "unit": "TFLOP/s", "frac": kd["tflops"] / pk["tf_sustained"],
           "achieved_essential": kd.get("tflops_essential"),
-          "traffic": (NCU_DRAM_BYTES_PER_ROW[dom] * rows_step / kd["launches_per_step"]
-                      if dom in NCU_DRAM_BYTES_PER_ROW and rows_step else None),
           "algorithmic_flop_per_launch": macs[dom] * 2 / kd["launches_per_step"],
           "avg_launch_ms": kd["ms_per_step"] / kd["launches_per_step"],
-          "peak_source": pk["source"] + ", sustained bf16 (kernel timed inside a long step)",
+          "peak_source": pk["source"] + ", dense bf16 (kernel timed inside a long step)",
           "how": "CUDA events recorded by the library on the launching stream around every launch of "
                  "this kernel (dyn_profile_*), in a separate pass right after the timed region"}
     if world == 1 and not a.no_cpu_baseline:

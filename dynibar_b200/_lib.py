@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libdynibar_b200.so")
 if not os.path.exists(LIB_PATH):
   raise ImportError(
       "dynibar_b200: %s is missing. Build it with `python __graft_entry__.py` "
-      "(nvcc, sm_100a). There is no CPU/PyTorch fallback for the hot path." % LIB_PATH)
+      "(nvcc, sm_90a). There is no CPU/PyTorch fallback for the hot path." % LIB_PATH)
 
 lib = C.CDLL(LIB_PATH)
 

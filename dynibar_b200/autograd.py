@@ -157,7 +157,7 @@ def _prec_code(precision):
 
 def motion_mlp(module, xyzt, precision=None):
   """Differentiable MotionMLP.forward on [...,4] rows; honours `sf_mag_div` like render_ray.motion_mlp_forward.
-  precision "bf16": the products run on tcgen05 (bf16 operands, fp32 accumulation / master weights)."""
+  precision "bf16": the products run on the tensor cores (bf16 operands, fp32 accumulation / master weights)."""
   from dynibar_b200 import weights
   m = weights.de_parallel(module)
   out = _MotionMLP.apply(xyzt, module, _prec_code(precision), *m.parameters())
@@ -219,7 +219,7 @@ class _NetDynamic(torch.autograd.Function):
 
 def net_dynamic(module, pts, rgb_feat, ray_dir, mask, time, precision=None):
   """Differentiable DynibarDynamic.forward -> raw [R,S,4].  precision "fp32": SIMT products; "bf16": the large
-  products on tcgen05 (bf16 operands, fp32 accumulation, master weights and gradients); glue always fp32."""
+  products on the tensor cores (bf16 operands, fp32 accumulation, master weights and gradients); glue always fp32."""
   from dynibar_b200 import weights
   m = weights.de_parallel(module)
   t = float(time.reshape(-1)[0]) if torch.is_tensor(time) else float(time)

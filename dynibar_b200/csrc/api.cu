@@ -7,6 +7,7 @@
 #include "linear_tc.cuh"
 #include "nets.cuh"
 #include "nets_fused.cuh"
+#include "tc.cuh"
 
 namespace dyn {
 
@@ -45,6 +46,32 @@ int fail(int code, const char* fmt, ...) {
   vsnprintf(err_buf(), 512, fmt, ap);
   va_end(ap);
   return code;
+}
+
+// accumulator memory of the fused tensor-core kernels that keep it in global memory (tc.cuh): a slot for each of
+// two resident CTAs per SM
+tc::AccPool acc_pool() {
+  static tc::AccPool pool[64] = {};
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ||
+      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+    fail(DYN_E_CUDA, "acc_pool: no current CUDA device");
+    return tc::AccPool{};
+  }
+  if (pool[dev].mem == nullptr) {
+    const int slots = 2 * sms;
+    const size_t bytes = (size_t)slots * tc::kAccCtaFloats * sizeof(float);
+    void* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, bytes + slots * sizeof(int));
+    if (e == cudaSuccess) e = cudaMemset((char*)p + bytes, 0, slots * sizeof(int));
+    if (e != cudaSuccess) {
+      if (p) cudaFree(p);
+      fail(DYN_E_CUDA, "acc_pool: %s", cudaGetErrorString(e));
+      return tc::AccPool{};
+    }
+    pool[dev] = tc::AccPool{(float*)p, (int*)((char*)p + bytes), slots};
+  }
+  return pool[dev];
 }
 
 }  // namespace dyn

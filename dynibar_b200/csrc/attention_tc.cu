@@ -1,15 +1,17 @@
-// Ray-transformer attention on tcgen05 (a11: ibrnet/mlp_network.py:13-31, :84-98).
+// Ray-transformer attention on the tensor cores (a11: ibrnet/mlp_network.py:13-31, :84-98).
 //
 // One CTA = one 128-row tile = 128/S whole rays (S | 128).  Q, K, V arrive as bf16 tile
 // images (fused_engine.cuh; written by point1_fused_kernel) and are landed in shared memory
 // by bulk copies (K, V: 32 KB each per tile; Q: one 8 KB head slice at a time);
-// per head h:  logits = Q_h K_h^T  (UMMA 128x128x32, fp32 in TMEM columns [0,128))
+// per head h:  logits = Q_h K_h^T  (128x128x32, fp32 in TMEM columns [0,128))
 //              softmax over the keys of the row's own ray, in registers
 //              (query rows with <= 1 valid view attend uniformly: the reference
 //               masks QUERY rows, mlp_network.py:23-24, :91-94)
-//              O_h = P V_h        (UMMA 128x32x128; P is written back to smem as the
+//              O_h = P V_h        (128x32x128; P is written back to smem as the
 //               A operand, V_h is read in place as an MN-major B operand)
 // O (fp32, TMEM columns [128,256)) is written to global at the end, again as a bf16 tile image.
+// The products run on wgmma, issued by warpgroup 0 (wg_mma); TMEM is the accumulator memory of tc.cuh
+// (a per-CTA slice of the device pool).
 #include "nets.cuh"
 #include "tc.cuh"
 #include <cstdlib>
@@ -27,9 +29,33 @@ constexpr int kQSlice = 128 * 32 * 2;  // Q_h: [128 x 32] = 8 KB
 // + barriers (256 B) + per-row partial softmax sums [2 twins][128][4 heads] + partial maxima [2][128]
 constexpr int kSmemAttn = 3 * kTile + kQSlice + 256 + 2 * 128 * 4 * 4 + 2 * 128 * 4;
 
-// idesc with B in MN-major layout (bit 16)
-__host__ __device__ constexpr uint32_t idesc_bf16_f32_bmn(int M, int N) {
-  return idesc_bf16_f32(M, N) | (1u << 16);
+// D[128 x N] = sum over k-steps ks of A_ks B_ks, by the 128 threads of warpgroup 0 in registers (N-blocks of at most
+// 64 columns), stored to TMEM columns col .. col + N - 1; then every thread arrives on `bar` (128 arrivals).
+// A: 128 K-major rows at a0 + ks * a_step (LBO 2048); B at b0 + ks * b_step (+ 16 B per column of the N-block),
+// K-major (TB = 0) or MN-major (TB = 1) with the given LBO / SBO.
+template <int N, int TB>
+__device__ __forceinline__ void wg_mma(uint32_t col, uint32_t a0, uint32_t a_step, uint32_t b0, uint32_t b_step,
+                                       uint32_t b_lbo, uint32_t b_sbo, int ksteps, uint32_t bar) {
+  constexpr int NB = N > 64 ? 64 : N;
+#pragma unroll
+  for (int nb = 0; nb < N / NB; ++nb) {
+    float acc[2][NB / 2];
+    fence_regs<NB / 2>(acc[0]);
+    fence_regs<NB / 2>(acc[1]);
+    wgmma_fence();
+    for (int ks = 0; ks < ksteps; ++ks)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        Wgmma<NB, 0, TB>::mma(acc[h], smem_desc(a0 + ks * a_step + h * 1024u, 2048u, 128u),
+                              smem_desc(b0 + ks * b_step + nb * NB * 16u, b_lbo, b_sbo), ks ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<NB / 2>(acc[0]);
+    fence_regs<NB / 2>(acc[1]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) acc_store_frag<NB>(acc[h], 64 * h, (int)col + nb * NB);
+  }
+  mbar_arrive(bar);
 }
 
 // TW: two threads per row in twin warps w, w+4 (same TMEM lane quadrant): each twin owns half of the
@@ -51,7 +77,7 @@ attention_tc_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __
   const uint32_t bar_s = smem_u32(bars), bar_o = smem_u32(bars + 1);
   const uint32_t bar_kv = smem_u32(bars + 2), bar_q = smem_u32(bars + 3);
   if (tid == 0) {
-    mbar_init(bar_s, 1); mbar_init(bar_o, 1); mbar_init(bar_kv, 1); mbar_init(bar_q, 1);
+    mbar_init(bar_s, 128); mbar_init(bar_o, 128); mbar_init(bar_kv, 1); mbar_init(bar_q, 1);
     mbar_fence_init();
   }
   if (warp == 0) tmem_alloc(smem_u32(tmem_slot), 256);
@@ -65,8 +91,8 @@ attention_tc_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __
   const int rw = warp & 3;  // row warp: rows 32 rw .. 32 rw + 31
   const size_t roff = (size_t)(r >> 3) * 128 + (r & 7) * 16;
   const int ray_lo = (r / S) * S;  // first key row (inside the tile) of this row's ray
-  // this THREAD's keys [k_lo, k_hi) and the key range touched by ANY row of this warp (tcgen05.ld is
-  // warp-collective: the column blocks a warp skips must be the same for all its lanes)
+  // this THREAD's keys [k_lo, k_hi) and the key range touched by ANY row of this warp (the column blocks a
+  // warp skips are the same for all its lanes: no divergence around the TMEM loads)
   const int k_lo = TW ? ray_lo + tw * (S >> 1) : ray_lo;
   const int k_hi = TW ? k_lo + (S >> 1) : ray_lo + S;
   const int warp_lo = TW ? k_lo : ((rw * 32) / S) * S;
@@ -79,19 +105,11 @@ attention_tc_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __
   const uint8_t* kimg = reinterpret_cast<const uint8_t*>(K);
   const uint8_t* vimg = reinterpret_cast<const uint8_t*>(V);
 
-  // thread 0 issues every bulk copy; the MMAs are issued by an elected lane of warp 0 with the
-  // whole warp converged (descriptors then stay in uniform registers)
-  auto issue_qk = [&](int h) {  // all lanes of warp 0: logits_h = Q_h K_h^T (waits for the Q_h slice)
+  // thread 0 issues every bulk copy; the MMAs are issued by warpgroup 0 (warps 0-3)
+  auto issue_qk = [&](int h) {  // all threads of warpgroup 0: logits_h = Q_h K_h^T (waits for the Q_h slice)
     mbar_wait(bar_q, ph_q & 1); ++ph_q;
     tc_fence_after_sync();
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16_f32(128, 128);
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks)
-        mma_bf16_ss(tmem_base, smem_desc(smem_u32(qt) + (2 * ks) * 2048u, 2048u, 128u),
-                    smem_desc(smem_u32(kt) + (4 * h + 2 * ks) * 2048u, 2048u, 128u), idesc, ks ? 1u : 0u);
-      mma_commit(bar_s);
-    }
+    wg_mma<128, 0>(tmem_base, smem_u32(qt), 4096u, smem_u32(kt) + (4 * h) * 2048u, 4096u, 2048u, 128u, 2, bar_s);
     __syncwarp();
   };
   auto load_q = [&](long long tile, int h) {  // head slice: k-groups 4h..4h+3 are contiguous in the image
@@ -111,7 +129,7 @@ attention_tc_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __
     }
     const bool q_valid = ok && nvalid[row] > 1.f;
     mbar_wait(bar_kv, ph_kv & 1); ++ph_kv;
-    if (warp == 0) issue_qk(0);
+    if (warp < 4) issue_qk(0);
     for (int h = 0; h < 4; ++h) {
       mbar_wait(bar_s, ph_s & 1);
       ++ph_s;
@@ -171,19 +189,12 @@ attention_tc_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* __
       fence_proxy_async_smem();
       tc_fence_before_sync();
       __syncthreads();  // P complete; every thread is done reading logits_h
-      if (warp == 0) {
+      if (warp < 4) {
         tc_fence_after_sync();
-        if (elect_one()) {
-          const uint32_t idesc = idesc_bf16_f32_bmn(128, 32);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            mma_bf16_ss(tmem_base + 128 + 32 * h, smem_desc(smem_u32(pt) + ks * 4096u, 2048u, 128u),
-                        // V_h as MN-major B: n = d in [32h, 32h+32) -> n-groups at stride 2048 (SBO),
-                        // k = key -> k-groups at stride 128 (LBO); this k-step covers keys [16ks, 16ks+16)
-                        smem_desc(smem_u32(vt) + (4 * h) * 2048u + ks * 256u, 128u, 2048u), idesc,
-                        ks ? 1u : 0u);
-          mma_commit(bar_o);
-        }
+        // V_h as MN-major B: n = d in [32h, 32h+32) -> n-groups at stride 2048 (SBO),
+        // k = key -> k-groups at stride 128 (LBO); k-step ks covers keys [16ks, 16ks+16)
+        wg_mma<32, 1>(tmem_base + 128 + 32 * h, smem_u32(pt), 4096u, smem_u32(vt) + (4 * h) * 2048u, 256u, 128u,
+                      2048u, 8, bar_o);
         __syncwarp();
         if (h < 3) issue_qk(h + 1);  // queued behind P V_h; overlaps the next softmax's wait
       }
@@ -246,7 +257,7 @@ attention_twin_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* 
   const uint32_t bar_s = smem_u32(bars), bar_o = smem_u32(bars + 1);
   const uint32_t bar_k = smem_u32(bars + 2), bar_q = smem_u32(bars + 3), bar_v = smem_u32(bars + 5);
   if (tid == 0) {
-    mbar_init(bar_s, 1); mbar_init(bar_o, 1); mbar_init(bar_k, 1); mbar_init(bar_q, 1); mbar_init(bar_v, 1);
+    mbar_init(bar_s, 128); mbar_init(bar_o, 128); mbar_init(bar_k, 1); mbar_init(bar_q, 1); mbar_init(bar_v, 1);
     mbar_fence_init();
   }
   if (warp == 0) tmem_alloc(smem_u32(tmem_slot), 256);
@@ -277,14 +288,7 @@ attention_twin_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* 
   auto issue_qk = [&](int h) {
     mbar_wait(bar_q, ph_q & 1); ++ph_q;
     tc_fence_after_sync();
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16_f32(128, 128);
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks)
-        mma_bf16_ss(tmem_base, smem_desc(smem_u32(qt) + (2 * ks) * 2048u, 2048u, 128u),
-                    smem_desc(smem_u32(kt) + (4 * h + 2 * ks) * 2048u, 2048u, 128u), idesc, ks ? 1u : 0u);
-      mma_commit(bar_s);
-    }
+    wg_mma<128, 0>(tmem_base, smem_u32(qt), 4096u, smem_u32(kt) + (4 * h) * 2048u, 4096u, 2048u, 128u, 2, bar_s);
     __syncwarp();
   };
   auto load_q = [&](long long tile, int h) {
@@ -313,7 +317,7 @@ attention_twin_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* 
     const bool q_valid = ok && nvalid[row] > 1.f;
     // exp(l / sqrt(32) - max) = 2^(l sc - max sc); a query row without two valid views attends uniformly
     const float sc = q_valid ? 0.17677669529663687f * 1.4426950408889634f : 0.f;
-    if (warp == 0) {
+    if (warp < 4) {
       mbar_wait(bar_k, ph_k & 1); ++ph_k;
       issue_qk(0);
     }
@@ -363,18 +367,11 @@ attention_twin_kernel(const __nv_bfloat16* __restrict__ Q, const __nv_bfloat16* 
       fence_proxy_async_smem();
       tc_fence_before_sync();
       __syncthreads();  // P complete; every thread is done reading logits_h
-      if (warp == 0) {
+      if (warp < 4) {
         if (h == 0) { mbar_wait(bar_v, ph_v & 1); ++ph_v; }
         tc_fence_after_sync();
-        if (elect_one()) {
-          const uint32_t idesc = idesc_bf16_f32_bmn(128, 32);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            mma_bf16_ss(tmem_base + 128 + 32 * h, smem_desc(smem_u32(pt) + ks * 4096u, 2048u, 128u),
-                        smem_desc(smem_u32(vt) + (4 * h) * 2048u + ks * 256u, 128u, 2048u), idesc,
-                        ks ? 1u : 0u);
-          mma_commit(bar_o);
-        }
+        wg_mma<32, 1>(tmem_base + 128 + 32 * h, smem_u32(pt), 4096u, smem_u32(vt) + (4 * h) * 2048u, 256u, 128u,
+                      2048u, 8, bar_o);
         __syncwarp();
         if (h < 3) issue_qk(h + 1);
       }
@@ -416,12 +413,14 @@ bool attention_tc_supported(int S) { return S >= 1 && S <= 128 && (128 % S) == 0
 int launch_attention_tc(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __nv_bfloat16* V,
                         const float* nvalid, long long P, int S, __nv_bfloat16* O, cudaStream_t st) {
   if (P == 0) return DYN_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DYN_CUDA(cudaGetDevice(&dev));
   DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long n_tiles = (P + 127) / 128;
   const int grid = (int)(n_tiles < 2 * sms ? n_tiles : 2 * sms);
   const int smem = kSmemAttn;
+  const int rc = bind_acc_pool();
+  if (rc) return rc;
   ProfScope prof(PROF_ATTENTION, st);
   static const bool generic = getenv("DYN_ATTENTION") && !strcmp(getenv("DYN_ATTENTION"), "generic");
   static bool attr_done = false;  // one device per process (torch.distributed: one rank per GPU)

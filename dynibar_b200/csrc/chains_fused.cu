@@ -1,4 +1,4 @@
-// Fused tcgen05 MLP chains that are row-local (no cross-row reduction inside the
+// Fused tensor-core MLP chains that are row-local (no cross-row reduction inside the
 // chain), built on fused_engine.cuh:
 //
 //   motion_fused_kernel : MotionMLP, PE(xyzt) -> 8 x (256, ReLU) with skip -> 18 coeffs
@@ -10,8 +10,8 @@
 //   rgbhead_fused_kernel: static per-view colour-blending head + masked softmax over views
 //                         (mlp_network.py:508-526)
 //
-// All use 256 rows per iteration (two M=128 UMMA tiles), one row per thread in
-// warps 0-7, the MMA issuer in warp 8 and the weight producer in warp 9.
+// All use 256 rows per iteration (two 128-row tiles), one row per thread in
+// warps 0-7, the MMA warpgroup in warps 8-11 and the weight producer in warp 12.
 #include "fused_engine.cuh"
 #include "nets.cuh"
 
@@ -22,7 +22,10 @@ using namespace fe;
 
 namespace {
 
-// common prologue: barriers + TMEM; returns the TMEM base address
+constexpr int kChainThreads = 13 * 32;
+constexpr int kProducerWarp = 12;
+
+// common prologue: barriers + accumulator memory (device pool); returns its base address
 __device__ __forceinline__ uint32_t fused_prologue(uint64_t* bars, uint32_t* tmem_slot, bool pp) {
   const int tid = threadIdx.x, warp = tid >> 5;
   const uint32_t bar0 = smem_u32(bars);
@@ -104,8 +107,8 @@ __device__ __forceinline__ void motion_operand(uint8_t* arow, const float* x4, b
   store8(arow, 136, z);
 }
 
-__global__ void __launch_bounds__(320, 1) motion_fused_kernel(const __grid_constant__ MotionFusedArgs a) {
-  constexpr bool kPP = false;  // MMA-bound ReLU chain: share every weight chunk between the tiles
+__global__ void __launch_bounds__(kChainThreads, 1) motion_fused_kernel(const __grid_constant__ MotionFusedArgs a) {
+  constexpr bool kPP = true;  // ping-pong: the MMA warpgroup holds the accumulators of one tile at a time
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem + 2 * kATileBytes;
   float* cst = reinterpret_cast<float*>(ring + kRing * kStageBytes);  // 8 x 256 biases + 32
@@ -120,9 +123,9 @@ __global__ void __launch_bounds__(320, 1) motion_fused_kernel(const __grid_const
   const uint32_t tmem_base = fused_prologue(bars, tmem_slot, kPP);
   const int n_iter = (int)((a.N + 255) / 256);
 
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers) producer_loop<kPP>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<kPP>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base);
   } else {
     const int tile = tid >> 7, r = tid & 127;
@@ -177,7 +180,7 @@ __global__ void __launch_bounds__(320, 1) motion_fused_kernel(const __grid_const
 // ---------------------------------------------------------------------------
 // per-point stage 1: G -> geometry_fc -> (+ posenc) -> g2, Q, K, V
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(320, 1) point1_fused_kernel(const __grid_constant__ Point1Args a) {
+__global__ void __launch_bounds__(kChainThreads, 1) point1_fused_kernel(const __grid_constant__ Point1Args a) {
   constexpr bool kPP = true;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem + 2 * kATileBytes;
@@ -194,9 +197,9 @@ __global__ void __launch_bounds__(320, 1) point1_fused_kernel(const __grid_const
   const uint32_t tmem_base = fused_prologue(bars, tmem_slot, kPP);
   const int n_iter = (int)((a.P + 255) / 256);
 
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers) producer_loop<kPP>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<kPP>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base);
   } else {
     const int tile = tid >> 7, r = tid & 127;
@@ -300,7 +303,7 @@ __global__ void __launch_bounds__(320, 1) point1_fused_kernel(const __grid_const
 //            [1024,1088) b_rgb2  [1088,1280) w_rgb4 (3 x 64)  [1280..] misc: b_outgeo2, b_rgb4[3]
 // ---------------------------------------------------------------------------
 template <bool DYNAMIC>
-__global__ void __launch_bounds__(320, 1) point2_fused_kernel(const __grid_constant__ Point2Args a) {
+__global__ void __launch_bounds__(kChainThreads, 1) point2_fused_kernel(const __grid_constant__ Point2Args a) {
   constexpr bool kPP = true;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem + 2 * kATileBytes;
@@ -334,9 +337,9 @@ __global__ void __launch_bounds__(320, 1) point2_fused_kernel(const __grid_const
   const uint32_t tmem_base = fused_prologue(bars, tmem_slot, kPP);
   const int n_iter = (int)((a.P + 255) / 256);
 
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers) producer_loop<kPP>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<kPP>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base);
   } else {
     const int tile = tid >> 7, r = tid & 127;
@@ -486,7 +489,7 @@ __global__ void __launch_bounds__(320, 1) point2_fused_kernel(const __grid_const
 // constants: [0,128) unused  [128,192) b_rgb2  [192,256) w_rgb4  [256] b_rgb4
 // ---------------------------------------------------------------------------
 template <int VP>
-__global__ void __launch_bounds__(320, 1) rgbhead_fused_kernel(const __grid_constant__ RgbHeadArgs a) {
+__global__ void __launch_bounds__(kChainThreads, 1) rgbhead_fused_kernel(const __grid_constant__ RgbHeadArgs a) {
   constexpr bool kPP = true;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem + 2 * kATileBytes;
@@ -509,9 +512,9 @@ __global__ void __launch_bounds__(320, 1) rgbhead_fused_kernel(const __grid_cons
   const uint32_t tmem_base = fused_prologue(bars, tmem_slot, kPP);
   const int n_iter = (int)((a.P * VP + 255) / 256);
 
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers) producer_loop<kPP>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<kPP>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base);
   } else {
     const int tile = tid >> 7, r = tid & 127;
@@ -603,14 +606,16 @@ constexpr int kSmemChain = 2 * kATileBytes + kRing * kStageBytes + 2304 * 4 + 25
 
 template <class K, class A>
 int launch_chain(K kernel, const A& args, long long rows, cudaStream_t st) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DYN_CUDA(cudaGetDevice(&dev));
   DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long n_iter = (rows + 255) / 256;
   const int grid = (int)(n_iter < sms ? n_iter : sms);
   if (grid == 0) return DYN_OK;
+  const int rc = bind_acc_pool();
+  if (rc) return rc;
   DYN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemChain));
-  kernel<<<grid, 320, kSmemChain, st>>>(args);
+  kernel<<<grid, kChainThreads, kSmemChain, st>>>(args);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }

@@ -1,9 +1,8 @@
-// Row-local fused tcgen05 chains in the twin-warp structure of view_twin.cu: TWO independent CTAs per SM,
-// each with ONE 128-row tile whose rows are served by TWO threads (warps w and w + 4 share the TMEM lane
-// quadrant w & 3 and split every layer's output columns), plus the MMA issuer (warp 8) and the weight
-// producer (warp 9).  The round-1 versions of these kernels (chains_fused.cu: one 320-thread CTA per SM,
-// two tiles, one thread per row) leave only 8 row warps on an SM; here 16 row warps share it and the two
-// CTAs desynchronise, which is what the latency-bound epilogues need (profiles/r02_chain_kernels.md).
+// Row-local fused tensor-core chains in the twin-warp structure of view_twin.cu: CTAs with ONE 128-row tile
+// whose rows are served by TWO threads (warps w and w + 4 read the same accumulator lanes 32 (w & 3) ..
+// + 31 and split every layer's output columns), plus the MMA warpgroup (warps 8-11) and the weight producer
+// (warp 12).  The other versions of these kernels (chains_fused.cu: two tiles per CTA, one thread per row)
+// give each row a single thread; here two threads share the latency-bound epilogues.
 //
 //   rgbhead_twin_kernel : static per-view colour-blending head + masked softmax over views
 //                         (mlp_network.py:508-526)
@@ -25,8 +24,11 @@ using namespace fe;
 
 namespace {
 
-constexpr int kTStage = 16384;
+constexpr int kTStage = 8192;  // two 8 KB weight stages leave room for the accumulator memory in shared memory
 constexpr int kTRing = 2;
+constexpr int kTwinThreads = 13 * 32;  // row warps 0-7, MMA warpgroup 8-11, weight producer 12
+constexpr int kProducerWarp = 12;
+constexpr int kRhChunks = 16, kP1Chunks = 48, kP2Chunks = 48;  // chunk-table capacity of each kernel
 constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
 
 __device__ __forceinline__ void pair_sync_tw(int pair) {
@@ -40,7 +42,8 @@ struct TwinCta {
   uint32_t bar0, tmem_base;
 };
 
-// common prologue of the twin chains: chunk table, barriers, TMEM (256 columns); `a_bytes` = operand tile size
+// common prologue of the twin chains: chunk table, barriers, TMEM (256 columns, in shared memory after the
+// barriers); `a_bytes` = operand tile size
 template <int kConstFloats>
 __device__ __forceinline__ TwinCta twin_prologue(uint8_t* smem, int a_bytes, FusedChunk* s_tab,
                                                  const FusedChunk* chunks, int nchunks, int extra_bars) {
@@ -57,7 +60,7 @@ __device__ __forceinline__ TwinCta twin_prologue(uint8_t* smem, int a_bytes, Fus
     for (int i = 0; i < extra_bars; ++i) mbar_init(c.bar0 + 8u * (12 + i), 1);
     mbar_fence_init();
   }
-  if ((threadIdx.x >> 5) == 8) tmem_alloc(smem_u32(tmem_slot), 256);
+  if ((threadIdx.x >> 5) == 8) tmem_alloc_smem(smem_u32(tmem_slot), reinterpret_cast<uint8_t*>(bars) + 256);
   tc_fence_before_sync();
   __syncthreads();
   tc_fence_after_sync();
@@ -89,12 +92,12 @@ __device__ __forceinline__ void t_wait(uint32_t bar0, uint32_t& acc_cnt) {
 // ---------------------------------------------------------------------------
 constexpr int kRhATile = 36 * 2048;
 constexpr int kRhConst = 384;
-constexpr int kRhSmem = kRhATile + kTRing * kTStage + kRhConst * 4 + 256;
+constexpr int kRhSmem = kRhATile + kTRing * kTStage + kRhConst * 4 + 256 + kAccSmemBytes;
 
 template <int VP>
-__global__ void __launch_bounds__(320, 2) rgbhead_twin_kernel(const __grid_constant__ RgbHeadArgs a) {
+__global__ void __launch_bounds__(kTwinThreads, 1) rgbhead_twin_kernel(const __grid_constant__ RgbHeadArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(16) FusedChunk s_tab[16];
+  __shared__ __align__(16) FusedChunk s_tab[kRhChunks];
   const TwinCta c = twin_prologue<kRhConst>(smem, kRhATile, s_tab, a.chunks, a.nchunks, 1);
   float* cst = c.cst;
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -103,10 +106,10 @@ __global__ void __launch_bounds__(320, 2) rgbhead_twin_kernel(const __grid_const
   __syncthreads();
   const int n_iter = (int)((a.P * VP + 127) / 128);
 
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers)
       producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<false, 1, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kRhATile);
   } else {
     const int tw = tid >> 7, r = tid & 127;
@@ -257,18 +260,18 @@ __device__ __forceinline__ void t_store_image_blocks(uint32_t tacc, int col0, vo
 // ---------------------------------------------------------------------------
 constexpr int kP1ATile = 34 * 2048;
 constexpr int kP1Const = 16;
-constexpr int kP1Smem = kP1ATile + kTRing * kTStage + kP1Const * 4 + 256;
+constexpr int kP1Smem = kP1ATile + kTRing * kTStage + kP1Const * 4 + 256 + kAccSmemBytes;
 
-__global__ void __launch_bounds__(320, 2) point1_twin_kernel(const __grid_constant__ Point1Args a) {
+__global__ void __launch_bounds__(kTwinThreads, 1) point1_twin_kernel(const __grid_constant__ Point1Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(16) FusedChunk s_tab[32];
+  __shared__ __align__(16) FusedChunk s_tab[kP1Chunks];
   const TwinCta c = twin_prologue<kP1Const>(smem, kP1ATile, s_tab, a.chunks, a.nchunks, 1);
   const int tid = threadIdx.x, warp = tid >> 5;
   const int n_iter = (int)((a.P + 127) / 128);
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers)
       producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<false, 1, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kP1ATile);
   } else {
     const int tw = tid >> 7, r = tid & 127;
@@ -346,12 +349,13 @@ __global__ void __launch_bounds__(320, 2) point1_twin_kernel(const __grid_consta
 constexpr int kP2ATile = 34 * 2048;
 constexpr int kP2X = 640;
 constexpr int kP2Const = kP2X + 6 * 256;
-constexpr int kP2Smem = kP2ATile + kTRing * kTStage + kP2Const * 4 + 256;
+constexpr int kP2Smem = kP2ATile + kTRing * kTStage + kP2Const * 4 + 256 + kAccSmemBytes;
+static_assert(2 * kRhSmem > 227 * 1024 && 2 * kP1Smem > 227 * 1024 && 2 * kP2Smem > 227 * 1024, "one CTA per SM");
 
 template <bool DYNAMIC>
-__global__ void __launch_bounds__(320, 2) point2_twin_kernel(const __grid_constant__ Point2Args a) {
+__global__ void __launch_bounds__(kTwinThreads, 1) point2_twin_kernel(const __grid_constant__ Point2Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(16) FusedChunk s_tab[32];
+  __shared__ __align__(16) FusedChunk s_tab[kP2Chunks];
   const TwinCta c = twin_prologue<kP2Const>(smem, kP2ATile, s_tab, a.chunks, a.nchunks, 1);
   float* cst = c.cst;
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -369,10 +373,10 @@ __global__ void __launch_bounds__(320, 2) point2_twin_kernel(const __grid_consta
   }
   __syncthreads();
   const int n_iter = (int)((a.P + 127) / 128);
-  if (warp == 9) {
+  if (warp == kProducerWarp) {
     if ((tid & 31) < a.producers)
       producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0, tid & 31, a.producers);
-  } else if (warp == 8) {
+  } else if (warp >= 8) {
     issuer_loop<false, 1, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kP2ATile);
   } else {
     const int tw = tid >> 7, r = tid & 127;
@@ -573,9 +577,9 @@ int launch_twin(K kernel, const A& args, long long rows, int smem_bytes, cudaStr
     DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   }
   const long long n_iter = (rows + 127) / 128;
-  const int grid = (int)(n_iter < 2LL * sms ? n_iter : 2LL * sms);
+  const int grid = (int)(n_iter < sms ? n_iter : sms);  // one CTA per SM: the accumulators fill shared memory
   if (grid == 0) return DYN_OK;
-  kernel<<<grid, 320, smem_bytes, st>>>(args);
+  kernel<<<grid, kTwinThreads, smem_bytes, st>>>(args);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }
@@ -588,7 +592,8 @@ int launch_twin(K kernel, const A& args, long long rows, int smem_bytes, cudaStr
 size_t twin_chain_bytes(int kind) { return kind == DYN_NET_MOTION ? 0 : (size_t)(768 * 1024); }
 
 static int upload_twin(std::vector<uint8_t>& img, std::vector<FusedChunk>& tab, char*& cursor, size_t& left,
-                       ChainImage* out, cudaStream_t st) {
+                       ChainImage* out, cudaStream_t st, size_t max_chunks) {
+  if (tab.size() > max_chunks) return fail(DYN_E_INVALID, "twin chain table has %zu chunks, kernel holds %zu", tab.size(), max_chunks);
   const size_t img_bytes = (img.size() + 255) & ~(size_t)255;
   const size_t need = img_bytes + ((tab.size() * sizeof(FusedChunk) + 255) & ~(size_t)255);
   if (need > left) return fail(DYN_E_INVALID, "twin chain images need %zu bytes, have %zu", need, left);
@@ -644,7 +649,7 @@ int twin_chain_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes
       append_layer(L, img, tab, 0, 0, 9, true, kTStage);
     }
     add(wv, 128, 128, 128, identity_map(128, 128), 1.f, false, -1.f, 0);
-    int rc = upload_twin(img, tab, cur, left, &n->chain_tw[0], st);
+    int rc = upload_twin(img, tab, cur, left, &n->chain_tw[0], st, kP1Chunks);
     if (rc) return rc;
     // ---- point stage 2
     add(fc, 128, 128, 128, identity_map(128, 128), 1.f, false, -1.f, 0);
@@ -671,7 +676,7 @@ int twin_chain_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes
       add2(og0, 128, 144, with_bias(128, 144, 128), kLog2e, kLog2e, {}, 0, 9, false);
       add2(n->sl.rgb0, 128, 144, with_bias(128, 144, 128), 1.f, 1.f, {}, 128, 8, true);
     }
-    rc = upload_twin(img, tab, cur, left, &n->chain_tw[1], st);
+    rc = upload_twin(img, tab, cur, left, &n->chain_tw[1], st, kP2Chunks);
     if (rc) return rc;
   }
   if (n->kind == DYN_NET_STATIC) {
@@ -683,7 +688,7 @@ int twin_chain_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes
     std::vector<int> m2 = identity_map(128, 144);
     m2[128] = kBiasHi; m2[129] = kBiasLo;
     add(n->sl.rgb2, 64, 64, 144, m2, 1.f, true, kLog2e, 18);
-    int rc = upload_twin(img, tab, cur, left, &n->chain_tw[2], st);
+    int rc = upload_twin(img, tab, cur, left, &n->chain_tw[2], st, kRhChunks);
     if (rc) return rc;
   }
   return DYN_OK;

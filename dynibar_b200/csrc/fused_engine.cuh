@@ -1,7 +1,7 @@
-// Shared machinery of the fused tcgen05 kernels (nets_fused.cu, chains_fused.cu):
-// smem budget constants, fast activations, A-tile stores, view-group shuffles,
-// the table-driven weight producer and MMA issuer, and the host-side packing of
-// weight chunks into UMMA images.
+// Shared machinery of the fused tensor-core kernels (nets_fused.cu, chains_fused.cu, chains_twin.cu,
+// view_*.cu): smem budget constants, fast activations, A-tile stores, view-group shuffles, the
+// table-driven weight producer and MMA warpgroup, and the host-side packing of weight chunks into
+// wgmma B-operand images.
 #pragma once
 #include <vector>
 
@@ -17,6 +17,7 @@ constexpr int kRing = 4;
 constexpr int kStageBytes = 16384;
 constexpr int kATileBytes = 69632;  // 128 rows x 272 cols bf16 (34 k-groups: geometry_fc.0 has K = 257)
 constexpr int kConstFloats = 2048;
+constexpr int kNB = 64;              // widest N-block of a chunk (accumulator registers of the MMA warpgroup)
 constexpr int kSmemFused = 2 * kATileBytes + kRing * kStageBytes + kConstFloats * 4 + 256;
 // barrier slots inside the fused kernels: [0..3] w_full, [4..7] w_empty, [8] a_ready, [9] acc_full
 
@@ -44,26 +45,14 @@ __device__ __forceinline__ float sigmoid_fast(float x) {
   return __frcp_rn(1.f + ex2f(-x * 1.4426950408889634f));
 }
 
-// tcgen05.wait::ld that carries a data dependency on the 16 destination registers of the load it waits for (so no
-// use of them can be scheduled above it)
-__device__ __forceinline__ void tmem_wait_ld_dep16(float* v) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]),
-                 "+f"(v[8]), "+f"(v[9]), "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15])
-               :
-               : "memory");
-}
-
-// Software-pipelined accumulator read-out: NH half-blocks of 16 TMEM columns; the load of half h + 1 is in flight
-// while fn(h, values) processes half h (TMEM reads run at 64 B/clk: a 32-column load of one warp occupies the port
-// for 64 cycles, and eight row warps per CTA queue on it).  colf(h) = TMEM column of half h.
+// Software-pipelined accumulator read-out: NH half-blocks of 16 columns; the load of half h + 1 is issued
+// before fn(h, values) processes half h.  colf(h) = accumulator column of half h.
 template <int NH, class ColFn, class Fn>
 __device__ __forceinline__ void tmem_pipe16(uint32_t tacc, ColFn colf, Fn fn) {
   float buf[2][16];
   tmem_ld16(tacc + colf(0), buf[0]);
 #pragma unroll
   for (int h = 0; h < NH; ++h) {
-    tmem_wait_ld_dep16(buf[h & 1]);
     if (h + 1 < NH) tmem_ld16(tacc + colf(h + 1), buf[(h + 1) & 1]);
     fn(h, buf[h & 1]);
   }
@@ -141,7 +130,7 @@ __device__ __forceinline__ void rs_step(const float* in, float* out, bool upper,
 
 
 // "Tile image": how bf16 activations travel between fused kernels through HBM.  Rows are grouped in
-// tiles of 128 and stored exactly as the consumer's UMMA A operand sits in shared memory (K-major
+// tiles of 128 and stored exactly as the consumer's wgmma A operand sits in shared memory (K-major
 // 8x8 core matrices): element (row r, column k) of a tile with KG 8-column groups lives at byte
 //   tile * KG * 2048 + (k / 8) * 2048 + (r % 128) * 16 + (k % 8) * 2.
 // The producer's per-row 16-byte stores are therefore warp-coalesced (32 rows x 16 B = 512 B), and
@@ -172,7 +161,7 @@ __device__ __forceinline__ void stage_chunks(FusedChunk* s, const FusedChunk* __
   for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 }
 
-// ---- control warps (one elected lane each) -------------------------------------
+// ---- control warps: the weight producer and the MMA warpgroup --------------------
 // barrier slots: [0..3] w_full, [4..7] w_empty, [8] a_ready(tile0), [9] acc_full(tile0),
 //                [10] a_ready(tile1), [11] acc_full(tile1)
 // Two schedules:
@@ -185,13 +174,17 @@ __device__ __forceinline__ void stage_chunks(FusedChunk* s, const FusedChunk* __
 __device__ __forceinline__ uint32_t bar_aready(uint32_t bar0, int tile, int ring = kRing) { return bar0 + 8u * (2 * ring + 2 * tile); }
 __device__ __forceinline__ uint32_t bar_acc(uint32_t bar0, int tile, int ring = kRing) { return bar0 + 8u * (2 * ring + 1 + 2 * tile); }
 
+// The MMA warpgroup: 4 warps, warp-index aligned (wgmma is issued by a whole warpgroup).  w_empty completes
+// when each of its warps has retired the wgmmas that read the slot (one arrival per warp), acc_full when
+// all of its threads have stored their accumulator fragments (one arrival per thread).
+constexpr int kIssuerWarps = 4;
 // `arrivals` = row threads per 128-row tile (128, or 256 in the twin-warp kernels)
 __device__ __forceinline__ void init_barriers(uint32_t bar0, bool pp, int arrivals = 128, int ring = kRing) {
-  for (int i = 0; i < ring; ++i) { mbar_init(bar0 + 8u * i, 1); mbar_init(bar0 + 8u * (ring + i), 1); }
+  for (int i = 0; i < ring; ++i) { mbar_init(bar0 + 8u * i, 1); mbar_init(bar0 + 8u * (ring + i), kIssuerWarps); }
   mbar_init(bar_aready(bar0, 0, ring), pp ? arrivals : 2 * arrivals);
-  mbar_init(bar_acc(bar0, 0, ring), 1);
+  mbar_init(bar_acc(bar0, 0, ring), 32 * kIssuerWarps);
   mbar_init(bar_aready(bar0, 1, ring), arrivals);
-  mbar_init(bar_acc(bar0, 1, ring), 1);
+  mbar_init(bar_acc(bar0, 1, ring), 32 * kIssuerWarps);
   mbar_fence_init();
 }
 
@@ -201,11 +194,8 @@ __device__ __forceinline__ int round_end(const FusedChunk* __restrict__ chunks, 
   return c + 1 < nchunks ? c + 1 : nchunks;
 }
 
-// One thread sustains ~40 B/clk of cp.async.bulk traffic however many copies it keeps in flight, two
-// threads ~79 B/clk, three ~100 B/clk (profiles/scripts/tma_rate.cu, profiles/r02_view_kernels.md), while
-// a layer at the full MMA rate consumes 64 B/clk of weights: `nlanes` lanes of the producer warp share
-// the chunk stream round-robin (lane p issues the chunks with cnt % nlanes == p; RING % nlanes == 0, so
-// a lane always refills the same ring slots).
+// `nlanes` lanes of the producer warp share the chunk stream round-robin (lane p issues the chunks with
+// cnt % nlanes == p; RING % nlanes == 0, so a lane always refills the same ring slots).
 template <bool PP, int RING = kRing, int STAGE = kStageBytes>
 __device__ __forceinline__ void producer_loop(const FusedChunk* __restrict__ chunks, int nchunks,
                                               const void* wimg, int n_iter, uint8_t* ring, uint32_t bar0,
@@ -230,10 +220,58 @@ __device__ __forceinline__ void producer_loop(const FusedChunk* __restrict__ chu
   }
 }
 
-// Called by ALL 32 lanes of the issuer warp (converged).
+// One N-block of a chunk for the accumulator sets of the tiles this chunk serves: 2 x 64-row wgmmas per k-step.
+template <int NB, int NA>
+__device__ __forceinline__ void mma_chunk(float (&acc)[NA][2][kNB / 2], const uint32_t* a_addr, int t0,
+                                          const FusedChunk& ch, uint32_t w_addr) {
+  const uint32_t lbo_b = (uint32_t)NB * 16u;
+#pragma unroll
+  for (int t = 0; t < NA; ++t) {
+    const uint32_t aa = a_addr[t0 + t] + (uint32_t)ch.a_kgroup * 2048u;
+    for (int ks = 0; ks < ch.ksteps; ++ks) {
+      const uint64_t bd = smem_desc(w_addr + ks * 2u * lbo_b, lbo_b, 128u);
+      const uint32_t sc = ((ch.flags & 8) && ks == 0) ? 0u : 1u;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        Wgmma<NB, 0, 0>::mma(acc[t][h], smem_desc(aa + ks * 4096u + h * 1024u, 2048u, 128u), bd, sc);
+    }
+  }
+}
+// accumulator sets <-> accumulator memory (tile t at columns col0 + 256 t + d_col)
+template <int NB, int NA>
+__device__ __forceinline__ void acc_chunk_io(float (&acc)[NA][2][kNB / 2], int t0, int col0, bool store) {
+#pragma unroll
+  for (int t = 0; t < NA; ++t)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (store) acc_store_frag<NB>(acc[t][h], 64 * h, col0 + 256 * (t0 + t));
+      else acc_load_frag<NB>(acc[t][h], 64 * h, col0 + 256 * (t0 + t));
+    }
+}
+
+// one chunk start to finish: resume the N-block from accumulator memory if it continues one, multiply,
+// wait for the wgmmas to retire, store the N-block if it ends here
+template <int NB, int NA>
+__device__ __forceinline__ void run_chunk(float (&acc)[NA][2][kNB / 2], const uint32_t* a_addr, int t0,
+                                          const FusedChunk& ch, uint32_t w_addr, uint32_t tmem_base) {
+  const int col0 = (int)(tmem_base & 0xffffu) + ch.d_col;
+  if ((ch.flags & 40) == 32) acc_chunk_io<NB>(acc, t0, col0, false);
+#pragma unroll
+  for (int t = 0; t < NA; ++t) { fence_regs<NB / 2>(acc[t][0]); fence_regs<NB / 2>(acc[t][1]); }
+  wgmma_fence();
+  mma_chunk<NB>(acc, a_addr, t0, ch, w_addr);
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int t = 0; t < NA; ++t) { fence_regs<NB / 2>(acc[t][0]); fence_regs<NB / 2>(acc[t][1]); }
+  if (ch.flags & 16) acc_chunk_io<NB>(acc, t0, col0, true);
+}
+
+// Called by ALL 128 threads of the MMA warpgroup (warps 4k .. 4k + 3 of the CTA).
 // FusedChunk.flags: 1 = wait for a_ready before this chunk, 2 = last chunk of a
-// round (commit acc_full), 4 = wait for the second operand barrier (one-tile kernels: the
-// a_ready slot of tile 1) before this chunk, 8 = first k-step overwrites D (start of a layer);
+// round (signal acc_full), 4 = wait for the second operand barrier (one-tile kernels: the
+// a_ready slot of tile 1) before this chunk, 8 = first k-step overwrites D (start of a layer),
+// 16 / 32 = last / first chunk of an N-block (store it to TMEM / without 8: continue from TMEM);
 // d_col = accumulator column offset inside the tile's 256-column TMEM region.
 // NT = 128-row tiles per CTA (1 or 2), RING = weight-ring slots in use.
 template <bool PP, int NT = 2, int RING = kRing, int STAGE = kStageBytes>
@@ -241,9 +279,11 @@ __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunk
                                             uint8_t* smem, uint8_t* ring, uint32_t bar0,
                                             uint32_t tmem_base, int a_tile_bytes = kATileBytes,
                                             long long* dbg = nullptr) {
-  // Entered by the whole (converged) warp; ONE elected lane then runs the loop alone, so every
-  // address / descriptor stays in uniform registers and no per-chunk warp re-convergence is needed.
-  if (elect_one()) {
+  // wgmma is issued by the whole warpgroup; the accumulators of one N-block (<= kNB columns) of every tile the
+  // chunk serves stay in registers across the N-block's chunks
+  {
+    float acc[PP ? 1 : NT][2][kNB / 2];
+    const bool lead = threadIdx.x % 128 == 0;
     uint32_t cnt = 0, a_cnt[2] = {0, 0}, a2_cnt = 0;
     long long t_a = 0, t_w = 0, t_begin = clock64();
     const uint32_t a_addr[2] = {smem_u32(smem), smem_u32(smem + a_tile_bytes)};
@@ -272,22 +312,19 @@ __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunk
               t_a += t1 - t0;
               t_w += t2 - t1;
             }
-            const uint32_t idesc = idesc_bf16_f32(128, ch.npad);
             const uint32_t w_addr = smem_u32(ring + st * STAGE);
-            const uint32_t lbo_b = (uint32_t)ch.npad * 16u;
-#pragma unroll
-            for (int t = 0; t < NT; ++t) {
-              if (PP && t != rep) continue;
-              const uint32_t aa = a_addr[t] + (uint32_t)ch.a_kgroup * 2048u;
-              for (int ks = 0; ks < ch.ksteps; ++ks) {
-                mma_bf16_ss(tmem_base + t * 256 + ch.d_col, smem_desc(aa + ks * 4096u, 2048u, 128u),
-                            smem_desc(w_addr + ks * 2u * lbo_b, lbo_b, 128u), idesc,
-                            ((ch.flags & 8) && ks == 0) ? 0u : 1u);
-              }
+            const int tile0 = PP ? rep : 0;
+            switch (ch.npad) {
+              case 16: run_chunk<16>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
+              case 32: run_chunk<32>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
+              case 48: run_chunk<48>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
+              case 64: run_chunk<64>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
+              default: __trap();  // the host packer emits N-blocks of 16, 32, 48 or 64 columns only
             }
-            mma_commit(bar0 + 8u * (RING + st));
-            if (ch.flags & 2) mma_commit(bar_acc(bar0, PP ? rep : 0, RING));
-            if (dbg && blockIdx.x == 0 && cnt < 120) {
+            __syncwarp();
+            if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (RING + st));  // this warp's wgmmas have retired
+            if (ch.flags & 2) mbar_arrive(bar_acc(bar0, PP ? rep : 0, RING));
+            if (dbg && blockIdx.x == 0 && lead && cnt < 120) {
               dbg[8 + 4 * cnt + 0] = t0; dbg[8 + 4 * cnt + 1] = t1;
               dbg[8 + 4 * cnt + 2] = t2; dbg[8 + 4 * cnt + 3] = clock64();
             }
@@ -296,7 +333,7 @@ __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunk
         c0 = c1;
       }
     }
-    if (dbg != nullptr && blockIdx.x == 0) {
+    if (dbg != nullptr && blockIdx.x == 0 && lead) {
       dbg[0] = clock64() - t_begin;  // issuer lifetime
       dbg[1] = t_a;                  // waiting for A operands (epilogues)
       dbg[2] = t_w;                  // waiting for weight chunks (ring)
@@ -337,20 +374,33 @@ inline float bf2f(uint16_t h) {
   return f;
 }
 
-inline void append_layer(const HostLayer& L, std::vector<uint8_t>& img, std::vector<FusedChunk>& tab,
-                         int d_col = 0, int a_kgroup0 = 0, int first_flags = 9, bool last = true,
-                         int stage_bytes = kStageBytes) {
+// rows [n0, n0 + nb) of a layer as a layer of its own (an N-block)
+inline HostLayer layer_rows(const HostLayer& L, int n0, int nb) {
+  HostLayer B = L;
+  B.N = L.N - n0 < nb ? (L.N - n0 > 0 ? L.N - n0 : 0) : nb;
+  B.Npad = nb;
+  if (B.N > 0) {
+    B.W = L.W + (size_t)n0 * L.Kw;
+    if (L.bias != nullptr) B.bias = L.bias + n0;
+  }
+  return B;
+}
+
+// One N-block (L.Npad <= kNB outputs), k-steps [k_begin, k_end), cut into chunks of at most one ring stage;
+// `first_flags` go on the first chunk, `last_flags` on the last.
+inline void append_block(const HostLayer& L, std::vector<uint8_t>& img, std::vector<FusedChunk>& tab,
+                         int d_col, int a_kgroup0, int first_flags, int last_flags, int stage_bytes, int k_begin,
+                         int k_end) {
   int steps_per_chunk = stage_bytes / (L.Npad * 32);
   if (steps_per_chunk > 8) steps_per_chunk = 8;
-  const int ksteps_total = L.Kpad / 16;
-  for (int k0 = 0; k0 < ksteps_total; k0 += steps_per_chunk) {
-    const int ks = (ksteps_total - k0) < steps_per_chunk ? (ksteps_total - k0) : steps_per_chunk;
+  for (int k0 = k_begin; k0 < k_end; k0 += steps_per_chunk) {
+    const int ks = (k_end - k0) < steps_per_chunk ? (k_end - k0) : steps_per_chunk;
     FusedChunk ch;
     ch.off = (uint32_t)img.size();
     ch.bytes = (uint32_t)(L.Npad * 32 * ks);
     ch.npad = (uint16_t)L.Npad;
     ch.ksteps = (uint8_t)ks;
-    ch.flags = (uint8_t)((k0 == 0 ? first_flags : 0) | ((last && k0 + ks >= ksteps_total) ? 2 : 0));
+    ch.flags = (uint8_t)((k0 == k_begin ? first_flags : 0) | (k0 + ks >= k_end ? last_flags : 0));
     ch.a_kgroup = (uint16_t)(a_kgroup0 + k0 * 2);
     ch.d_col = (uint16_t)d_col;
     img.resize(img.size() + ch.bytes, 0);
@@ -373,58 +423,39 @@ inline void append_layer(const HostLayer& L, std::vector<uint8_t>& img, std::vec
   }
 }
 
+// A layer as N-blocks of at most kNB output columns, each streamed over all of K before the next one (the
+// MMA warpgroup keeps one N-block's accumulators in registers).  The operand waits of `first_flags` (1, 4) go
+// on the layer's first chunk, its 8 ("overwrite D") on the first chunk of every N-block.
+inline void append_layer(const HostLayer& L, std::vector<uint8_t>& img, std::vector<FusedChunk>& tab,
+                         int d_col = 0, int a_kgroup0 = 0, int first_flags = 9, bool last = true,
+                         int stage_bytes = kStageBytes) {
+  for (int n0 = 0; n0 < L.Npad; n0 += kNB)
+    append_block(layer_rows(L, n0, L.Npad - n0 < kNB ? L.Npad - n0 : kNB), img, tab, d_col + n0, a_kgroup0,
+                 32 | (n0 == 0 ? first_flags & 5 : 0) | (first_flags & 8),
+                 16 | (last && n0 + kNB >= L.Npad ? 2 : 0), stage_bytes, 0, L.Kpad / 16);
+}
+
 // A layer issued in SUB-ROUNDS: `plan[r]` lists the runs (first k-step, number of k-steps) of operand columns
 // that sub-round r consumes; the issuer waits for one operand arrival round per sub-round (chunk flag 1) and
 // signals the epilogue only after the last one (flag 2).  The row warps arrive after every block of operand
 // columns they finish, so the k-steps over finished columns overlap the epilogue of the remaining ones.
+// Every sub-round covers all N-blocks; sub-round 1 continues from the partial sums sub-round 0 stored.
 // Chunk c of a run starting at k-step k0 reads the operand tile at k-group a_kgroup0 + 2 * (k0 + ...).
 using LayerPlan = std::vector<std::vector<std::pair<int, int>>>;
 inline void append_layer_plan(const HostLayer& L, std::vector<uint8_t>& img, std::vector<FusedChunk>& tab,
                               int d_col, int a_kgroup0, const LayerPlan& plan, int stage_bytes = kStageBytes) {
-  int steps_per_chunk = stage_bytes / (L.Npad * 32);
-  if (steps_per_chunk > 8) steps_per_chunk = 8;
-  bool first_chunk = true;
-  for (size_t r = 0; r < plan.size() && r < 2; ++r) {  // at most two sub-rounds (two operand barriers)
-    bool first_of_round = true;
-    for (size_t q = 0; q < plan[r].size(); ++q) {
-      const int run0 = plan[r][q].first, run1 = run0 + plan[r][q].second;
-      for (int k0 = run0; k0 < run1; k0 += steps_per_chunk) {
-        const int ks = (run1 - k0) < steps_per_chunk ? (run1 - k0) : steps_per_chunk;
-        const bool last = r + 1 == plan.size() && q + 1 == plan[r].size() && k0 + ks >= run1;
-        FusedChunk ch;
-        ch.off = (uint32_t)img.size();
-        ch.bytes = (uint32_t)(L.Npad * 32 * ks);
-        ch.npad = (uint16_t)L.Npad;
-        ch.ksteps = (uint8_t)ks;
+  const size_t nr = plan.size() < 2 ? plan.size() : 2;  // at most two sub-rounds (two operand barriers)
+  for (size_t r = 0; r < nr; ++r)
+    for (int n0 = 0; n0 < L.Npad; n0 += kNB)
+      for (size_t q = 0; q < plan[r].size(); ++q) {
         // sub-round 0 waits on the operand barrier (flag 1), sub-round 1 on the SECOND operand barrier (flag 4):
         // a row thread arrives on each of them exactly once per layer -- with a single barrier a fast thread's
         // second arrival could complete the phase that a slow thread has not reached yet
-        ch.flags = (uint8_t)((first_of_round ? (r == 0 ? 1 : 4) : 0) | (first_chunk ? 8 : 0) | (last ? 2 : 0));
-        ch.a_kgroup = (uint16_t)(a_kgroup0 + k0 * 2);
-        ch.d_col = (uint16_t)d_col;
-        img.resize(img.size() + ch.bytes, 0);
-        uint16_t* dst = reinterpret_cast<uint16_t*>(img.data() + ch.off);
-        const float bs = L.bias_scale >= 0.f ? L.bias_scale : L.scale;
-        for (int n = 0; n < L.Npad; ++n)
-          for (int kk = 0; kk < ks * 16; ++kk) {
-            const int col = L.colmap[k0 * 16 + kk];
-            float val = 0.f;
-            if (n < L.N) {
-              if (col >= 0) {
-                val = L.W[(size_t)n * L.Kw + col] * L.scale * (L.colscale.empty() ? 1.f : L.colscale[k0 * 16 + kk]);
-              } else if (L.bias != nullptr && (col == kBiasHi || col == kBiasLo)) {
-                const float b = L.bias[n] * bs, hi = bf2f(f2bf(b));
-                val = col == kBiasHi ? hi : b - hi;
-              }
-            }
-            dst[tile_off((uint32_t)L.Npad, (uint32_t)n, (uint32_t)kk) / 2] = f2bf(val);
-          }
-        tab.push_back(ch);
-        first_of_round = false;
-        first_chunk = false;
+        const int first = q > 0 ? 0 : 32 | (n0 == 0 ? (r == 0 ? 1 : 4) : 0) | (r == 0 ? 8 : 0);
+        const int last = q + 1 < plan[r].size() ? 0 : 16 | (r + 1 == nr && n0 + kNB >= L.Npad ? 2 : 0);
+        append_block(layer_rows(L, n0, L.Npad - n0 < kNB ? L.Npad - n0 : kNB), img, tab, d_col + n0, a_kgroup0,
+                     first, last, stage_bytes, plan[r][q].first, plan[r][q].first + plan[r][q].second);
       }
-    }
-  }
 }
 
 inline std::vector<int> identity_map(int K, int Kpad) {

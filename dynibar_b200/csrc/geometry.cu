@@ -1,7 +1,7 @@
 // Geometry kernels: ray sampling (a2), trajectory displacement (a3 tail),
 // projection + bilinear gather + view-angle difference (a4-a6), Plucker
 // coordinates (a7), optical flow / expected scene flow (a14).
-// All fp32.  Reference file:line citations are relative to /root/reference.
+// All fp32.  Reference file:line citations are relative to the reference checkout's root.
 #include <cuda_bf16.h>
 
 #include "common.cuh"

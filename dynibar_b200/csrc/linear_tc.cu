@@ -1,13 +1,9 @@
 // Generic tensor-core linear layer  Y = act(concat(segments) * W^T + b)
-// on tcgen05 (bf16 operands, fp32 accumulation in TMEM).
+// on wgmma (bf16 operands, fp32 accumulation in registers).
 //
-// One CTA computes a 256-row slab (two M=128 UMMA tiles that share every
-// weight chunk) for the full output width N <= 256.
-//   warps 0-7 : A-operand loaders (global fp32 -> bf16 -> canonical smem tile,
-//               one row per thread, K in chunks of 64) and epilogue
-//               (tcgen05.ld -> bias -> activation -> global)
-//   warp 8    : lane 0 streams pre-packed weight chunks with cp.async.bulk
-//               into a 3-stage ring and issues the tcgen05.mma instructions.
+// One CTA computes a 128-row slab for the full output width N <= 256: two warpgroups of 64 rows, K in
+// chunks of 64; per chunk every thread loads its share of the slab (global fp32 -> bf16 -> canonical smem
+// tile, the next chunk's loads in flight during the MMAs) and thread 0 lands the weight chunk by cp.async.bulk.
 // Used for the per-point layers of the aggregation networks and, until the
 // fused per-view kernels take over, for every large layer in DYN_PREC_BF16 mode.
 #include "linear_tc.cuh"
@@ -19,16 +15,10 @@ using namespace tc;
 
 namespace {
 
-constexpr int kKC = 64;           // K per chunk
-constexpr int kWStages = 3;
-constexpr int kTileBytes = 128 * kKC * 2;      // one 128-row A sub-tile of a chunk: 16 KB
-constexpr int kABufBytes = 2 * kTileBytes;     // both tiles: 32 KB
-constexpr int kWStageBytes = 256 * kKC * 2;    // 32 KB (N up to 256)
-constexpr int kSmemBytes = 2 * kABufBytes + kWStages * kWStageBytes + 1024;  // N up to 256: one CTA per SM
-// narrower layers use weight stages of their own size (Npad x 64 bf16) and two of them: two CTAs fit an SM and
-// the load / MMA / store phases of one overlap the other's
-__host__ __device__ constexpr int w_stages(int Npad) { return Npad <= 144 ? 2 : kWStages; }
-__host__ __device__ constexpr int smem_bytes(int Npad) { return 2 * kABufBytes + w_stages(Npad) * Npad * kKC * 2 + 1024; }
+constexpr int kKC = 64;                   // K per chunk
+constexpr int kRows = 128;                // rows per CTA
+constexpr int kATile = kRows * kKC * 2;   // one A chunk: 16 KB
+__host__ __device__ constexpr int smem_bytes(int Npad) { return 2 * kATile + 2 * Npad * kKC * 2 + 64; }
 
 __device__ __forceinline__ float act_f(float v, int act) {
   switch (act) {
@@ -51,183 +41,124 @@ __device__ __forceinline__ float seg_value(const TcLinArgs& a, long long row, in
   return 0.f;
 }
 
-__global__ void __launch_bounds__(288, 2) linear_tc_kernel(const __grid_constant__ TcLinArgs a) {
+// D[64 x w] (+)= A * B for one N-block of w <= 64 columns
+__device__ __forceinline__ void mma_block(float* d, int w, uint64_t ad, uint64_t bd, uint32_t sc) {
+  switch (w) {
+    case 16: Wgmma<16, 0, 0>::mma(d, ad, bd, sc); break;
+    case 32: Wgmma<32, 0, 0>::mma(d, ad, bd, sc); break;
+    case 48: Wgmma<48, 0, 0>::mma(d, ad, bd, sc); break;
+    default: Wgmma<64, 0, 0>::mma(d, ad, bd, sc); break;
+  }
+}
+
+__global__ void __launch_bounds__(256, 1) linear_tc_kernel(const __grid_constant__ TcLinArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int nws = w_stages(a.Npad);                       // weight ring depth
-  const int wsb = a.Npad * kKC * 2;                       // bytes per weight stage
-  uint8_t* a_buf = smem;                                  // 2 x 32 KB
-  uint8_t* w_buf = smem + 2 * kABufBytes;                 // nws x wsb
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * kABufBytes + nws * wsb);
-  // bars: [0,1] a_full, [2,3] a_empty, [4..6] w_full, [7..9] w_empty, [10] acc_full
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const uint32_t bar0 = smem_u32(bars);
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
+  const int wsb = a.Npad * kKC * 2;  // bytes per weight chunk
+  uint8_t* a_buf = smem;             // 2 x 16 KB
+  uint8_t* w_buf = smem + 2 * kATile;
+  const uint32_t bar0 = smem_u32(w_buf + 2 * wsb);  // [0,1]: weight chunk of stage s has landed
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const long long m0 = (long long)blockIdx.x * kRows;
   const int nchunks = a.nchunks;
-  const uint32_t tmem_cols = a.Npad <= 16 ? 32u : (a.Npad <= 32 ? 64u : (a.Npad <= 64 ? 128u : (a.Npad <= 128 ? 256u : 512u)));
-
+  const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.Wp);
   if (tid == 0) {
-    mbar_init(BAR(0), 256); mbar_init(BAR(1), 256);
-    mbar_init(BAR(2), 1); mbar_init(BAR(3), 1);
-    for (int i = 0; i < kWStages; ++i) { mbar_init(BAR(4 + i), 1); mbar_init(BAR(7 + i), 1); }  // nws of them used
-    mbar_init(BAR(10), 1);
+    mbar_init(bar0, 1);
+    mbar_init(bar0 + 8, 1);
     mbar_fence_init();
   }
-  if (warp == 8) tmem_alloc(smem_u32(tmem_slot), tmem_cols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const long long m0 = (long long)blockIdx.x * 256;
-  const uint32_t w_chunk_bytes = (uint32_t)a.Npad * kKC * 2;
-
-  if (warp == 8) {
-    // the whole warp arrives converged; one ELECTED lane runs the loop (uniform-register descriptors,
-    // see fused_engine.cuh: issuer_loop)
-    if (elect_one()) {
-      // ---------------- weight producer + MMA issuer ----------------
-      const uint32_t idesc = idesc_bf16_f32(128, a.Npad);
-      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.Wp);
-      const int ahead = nws - 1;  // chunks requested ahead of the one being multiplied
-      for (int c = 0; c < ahead && c < nchunks; ++c) {
-        mbar_arrive_expect_tx(BAR(4 + c), w_chunk_bytes);
-        bulk_g2s(smem_u32(w_buf + c * wsb), wsrc + (size_t)c * w_chunk_bytes, w_chunk_bytes,
-                 BAR(4 + c));
-      }
-      for (int kc = 0; kc < nchunks; ++kc) {
-        const int c2 = kc + ahead;
-        if (c2 < nchunks) {
-          const int s2 = c2 % nws;
-          if (c2 >= nws) mbar_wait(BAR(7 + s2), ((c2 / nws) - 1) & 1);
-          mbar_arrive_expect_tx(BAR(4 + s2), w_chunk_bytes);
-          bulk_g2s(smem_u32(w_buf + s2 * wsb), wsrc + (size_t)c2 * w_chunk_bytes,
-                   w_chunk_bytes, BAR(4 + s2));
-        }
-        const int ws = kc % nws, ab = kc & 1;
-        mbar_wait(BAR(4 + ws), (kc / nws) & 1);
-        mbar_wait(BAR(0 + ab), (kc >> 1) & 1);
-        tc_fence_after_sync();
-        int ksteps = (a.K - kc * kKC + 15) / 16;
-        if (ksteps > 4) ksteps = 4;
-        const uint32_t a_addr = smem_u32(a_buf + ab * kABufBytes);
-        const uint32_t w_addr = smem_u32(w_buf + ws * wsb);
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t ad = smem_desc(a_addr + t * kTileBytes + ks * 2 * (128 * 16), 128 * 16, 128);
-            const uint64_t bd = smem_desc(w_addr + ks * 2 * (a.Npad * 16), a.Npad * 16, 128);
-            mma_bf16_ss(tmem_base + t * a.Npad, ad, bd, idesc, (kc > 0 || ks > 0) ? 1u : 0u);
-          }
-        }
-        mma_commit(BAR(2 + ab));
-        mma_commit(BAR(7 + ws));
-      }
-      mma_commit(BAR(10));
-    }
-  } else {
-    // ---------------- A loaders ----------------
-    const long long row = m0 + tid;
-    const bool row_ok = row < a.M;
-    const int tile = tid >> 7, r = tid & 127;
-    const float rs = (row_ok && a.row_scale) ? a.row_scale[row] : 1.f;
-    // fast path: one dense, 16-byte aligned fp32 source
-    const bool dense = a.nseg == 1 && a.seg[0].div == 1 && (a.seg[0].ld & 3) == 0 &&
-                       ((reinterpret_cast<uintptr_t>(a.seg[0].p) & 15) == 0);
-    const int lane = tid & 31;
-    for (int kc = 0; kc < nchunks; ++kc) {
-      const int ab = kc & 1;
-      const int kbase = kc * kKC;
-      if (dense && kbase + kKC <= a.K) {
-        // coalesced: one warp instruction pair covers 4 rows x 64 floats (lane -> row l/8, k-group l%8)
-        float4 q0[8], q1[8];
-        float sc[8];
-#pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          const int lr = warp * 32 + rr * 4 + (lane >> 3);
-          const long long grow = m0 + lr;
-          q0[rr] = make_float4(0.f, 0.f, 0.f, 0.f); q1[rr] = q0[rr]; sc[rr] = 1.f;
-          if (grow < a.M) {
-            const float4* src = reinterpret_cast<const float4*>(a.seg[0].p + grow * a.seg[0].ld + kbase + (lane & 7) * 8);
-            q0[rr] = __ldg(src); q1[rr] = __ldg(src + 1);
-            if (a.row_scale) sc[rr] = __ldg(a.row_scale + grow);
-          }
-        }
-        if (kc >= 2) mbar_wait(BAR(2 + ab), ((kc >> 1) - 1) & 1);
-#pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          const int lr = warp * 32 + rr * 4 + (lane >> 3);
-          const int tl = lr >> 7, rl = lr & 127;
-          uint4 q;
-          q.x = pack_bf16x2(q0[rr].x * sc[rr], q0[rr].y * sc[rr]);
-          q.y = pack_bf16x2(q0[rr].z * sc[rr], q0[rr].w * sc[rr]);
-          q.z = pack_bf16x2(q1[rr].x * sc[rr], q1[rr].y * sc[rr]);
-          q.w = pack_bf16x2(q1[rr].z * sc[rr], q1[rr].w * sc[rr]);
-          *reinterpret_cast<uint4*>(a_buf + ab * kABufBytes + tl * kTileBytes + (lane & 7) * 2048 +
-                                    (rl >> 3) * 128 + (rl & 7) * 16) = q;
-        }
-      } else {
-        float v[kKC];
-#pragma unroll
-        for (int j = 0; j < kKC; ++j)
-          v[j] = (row_ok && kbase + j < a.K) ? seg_value(a, row, kbase + j) : 0.f;
-        if (kc >= 2) mbar_wait(BAR(2 + ab), ((kc >> 1) - 1) & 1);
-        uint8_t* dst = a_buf + ab * kABufBytes + tile * kTileBytes + (r >> 3) * 128 + (r & 7) * 16;
-#pragma unroll
-        for (int g = 0; g < kKC / 8; ++g) {
-          uint4 q;
-          q.x = pack_bf16x2(v[8 * g + 0] * rs, v[8 * g + 1] * rs);
-          q.y = pack_bf16x2(v[8 * g + 2] * rs, v[8 * g + 3] * rs);
-          q.z = pack_bf16x2(v[8 * g + 4] * rs, v[8 * g + 5] * rs);
-          q.w = pack_bf16x2(v[8 * g + 6] * rs, v[8 * g + 7] * rs);
-          *reinterpret_cast<uint4*>(dst + g * (128 * 16)) = q;
-        }
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(BAR(0 + ab));
-    }
-    // ---------------- epilogue ----------------
-    mbar_wait(BAR(10), 0);
-    tc_fence_after_sync();
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32);
-    float* stg = reinterpret_cast<float*>(a_buf);  // [256][33] fp32 staging (33 KB of the 64 KB A area)
-    for (int cb = 0; cb < a.Npad; cb += 32) {
-      const int ncol = (a.Npad - cb) < 32 ? (a.Npad - cb) : 32;  // 32 or 16
-      float acc[32];
-      if (ncol == 32) {
-        tmem_ld32(tmem_addr(tmem_base, lane_base, (uint32_t)(tile * a.Npad + cb)), acc);
-      } else {
-        tmem_ld16(tmem_addr(tmem_base, lane_base, (uint32_t)(tile * a.Npad + cb)), acc);
-      }
-      tmem_wait_ld();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int col = cb + i;
-        float y = 0.f;
-        if (i < ncol && col < a.N) y = act_f(acc[i] + (a.b ? __ldg(a.b + col) : 0.f), a.act);
-        stg[tid * 33 + i] = y;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      {
-        const int col = cb + lane;
-        const bool col_ok = lane < ncol && col < a.N;
-#pragma unroll 8
-        for (int rr = 0; rr < 32; ++rr) {
-          const int lr = warp * 32 + rr;
-          const long long grow = m0 + lr;
-          if (col_ok && grow < a.M) a.Y[grow * a.ldy + col] = stg[lr * 33 + lane];
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
-    tc_fence_before_sync();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bar0, (uint32_t)wsb);
+    bulk_g2s(smem_u32(w_buf), wsrc, (uint32_t)wsb, bar0);
   }
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, tmem_cols);
+
+  // operand loads: thread -> k-group kg (8 columns) of slab rows lr0 + 32 i
+  const int kg = tid & 7, lr0 = tid >> 3;
+  const bool dense = a.nseg == 1 && a.seg[0].div == 1 && (a.seg[0].ld & 3) == 0 &&
+                     ((reinterpret_cast<uintptr_t>(a.seg[0].p) & 15) == 0);
+  float v[4][8];
+  auto fetch = [&](int kc) {
+    const int k0 = kc * kKC + 8 * kg;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const long long row = m0 + lr0 + 32 * i;
+      const bool ok = row < a.M;
+      const float rs = (ok && a.row_scale) ? __ldg(a.row_scale + row) : 1.f;
+      if (ok && dense && k0 + 8 <= a.K) {
+        const float4* src = reinterpret_cast<const float4*>(a.seg[0].p + row * a.seg[0].ld + k0);
+        const float4 q0 = __ldg(src), q1 = __ldg(src + 1);
+        v[i][0] = q0.x * rs; v[i][1] = q0.y * rs; v[i][2] = q0.z * rs; v[i][3] = q0.w * rs;
+        v[i][4] = q1.x * rs; v[i][5] = q1.y * rs; v[i][6] = q1.z * rs; v[i][7] = q1.w * rs;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[i][j] = (ok && k0 + j < a.K) ? seg_value(a, row, k0 + j) * rs : 0.f;
+      }
+    }
+  };
+  auto stash = [&](int s) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      uint4 q;
+      q.x = pack_bf16x2(v[i][0], v[i][1]); q.y = pack_bf16x2(v[i][2], v[i][3]);
+      q.z = pack_bf16x2(v[i][4], v[i][5]); q.w = pack_bf16x2(v[i][6], v[i][7]);
+      *reinterpret_cast<uint4*>(a_buf + s * kATile + tile_off(kRows, lr0 + 32 * i, 8 * kg)) = q;
+    }
+  };
+
+  float acc[4][32];
+  fetch(0);
+  for (int kc = 0; kc < nchunks; ++kc) {
+    const int s = kc & 1;
+    stash(s);
+    fence_proxy_async_smem();
+    __syncthreads();  // A chunk kc is complete; every warpgroup has retired its wgmmas of chunk kc - 1
+    if (tid == 0 && kc + 1 < nchunks) {  // stage s ^ 1 held chunk kc - 1
+      mbar_arrive_expect_tx(bar0 + 8u * (s ^ 1), (uint32_t)wsb);
+      bulk_g2s(smem_u32(w_buf + (s ^ 1) * wsb), wsrc + (size_t)(kc + 1) * wsb, (uint32_t)wsb, bar0 + 8u * (s ^ 1));
+    }
+    if (kc + 1 < nchunks) fetch(kc + 1);
+    mbar_wait(bar0 + 8u * s, (kc >> 1) & 1);
+    int ksteps = (a.K - kc * kKC + 15) / 16;
+    if (ksteps > 4) ksteps = 4;
+    const uint32_t a_addr = smem_u32(a_buf + s * kATile) + wg * 1024u;
+    const uint32_t w_addr = smem_u32(w_buf + s * wsb);
+#pragma unroll
+    for (int b = 0; b < 4; ++b) fence_regs<32>(acc[b]);
+    wgmma_fence();
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const uint64_t ad = smem_desc(a_addr + ks * 2 * (kRows * 16), kRows * 16, 128);
+      const uint32_t sc = (kc > 0 || ks > 0) ? 1u : 0u;
+#pragma unroll
+      for (int b = 0; b < 4; ++b)
+        if (64 * b < a.Npad)
+          mma_block(acc[b], min(64, a.Npad - 64 * b),
+                    ad, smem_desc(w_addr + 64 * b * 16 + ks * 2 * (a.Npad * 16), a.Npad * 16, 128), sc);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int b = 0; b < 4; ++b) fence_regs<32>(acc[b]);
+  }
+
+  // ---------------- epilogue: bias, activation, fp32 out ----------------
+  const int w = (tid >> 5) & 3, l = tid & 31;
+#pragma unroll
+  for (int b = 0; b < 4; ++b) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int col0 = 64 * b + 8 * j + 2 * (l & 3);
+      if (64 * b + 8 * j >= a.Npad) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long row = m0 + 64 * wg + 16 * w + (l >> 2) + 8 * h;
+        if (row >= a.M) continue;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + e;
+          if (col < a.N) a.Y[row * a.ldy + col] = act_f(acc[b][4 * j + 2 * h + e] + (a.b ? __ldg(a.b + col) : 0.f), a.act);
+        }
+      }
+    }
   }
 }
 
@@ -281,11 +212,10 @@ int launch_linear_tc(const LinArgs& f, const void* packed_w, cudaStream_t st) {
   a.nchunks = (f.K + kKC - 1) / kKC;
   static bool attr_set = false;
   if (!attr_set) {
-    DYN_CUDA(cudaFuncSetAttribute(linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  kSmemBytes));
+    DYN_CUDA(cudaFuncSetAttribute(linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256)));
     attr_set = true;
   }
-  linear_tc_kernel<<<cdiv(f.M, 256), 288, smem_bytes(a.Npad), st>>>(a);
+  linear_tc_kernel<<<cdiv(f.M, kRows), 256, smem_bytes(a.Npad), st>>>(a);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }

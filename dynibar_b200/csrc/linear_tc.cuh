@@ -1,4 +1,4 @@
-// tcgen05 linear layer (linear_tc.cu)
+// tensor-core (wgmma) linear layer (linear_tc.cu)
 #pragma once
 #include "linear_f32.cuh"
 

@@ -1,9 +1,9 @@
 // Staged evaluation of the three networks (a3, a8-a11): the reference's op
 // graph as one kernel per layer -- generic linear layers (fp32 SIMT in
-// linear_f32.cu for DYN_PREC_FP32, tcgen05 in linear_tc.cu for DYN_PREC_BF16)
+// linear_f32.cu for DYN_PREC_FP32, wgmma in linear_tc.cu for DYN_PREC_BF16)
 // plus the fused fp32 glue below (positional encodings, view
 // pooling, visibility gating, ray transformer, heads).  This is the parity
-// mode; the throughput mode is the tcgen05 path in nets_tc.cu.
+// mode; the throughput mode is the fused tensor-core path (nets_fused.cu and the chain kernels).
 #include <math.h>
 
 #include "linear_tc.cuh"
@@ -545,8 +545,8 @@ __global__ void zero_last_kernel(float* __restrict__ coeff, int R, int S, int n_
 
 static const float* P_(const dyn_net* n, int off) { return off < 0 ? nullptr : n->params + off; }
 
-// one linear layer in the requested precision: tcgen05 (bf16 operands) when the
-// net carries packed images and the layer is big enough to fill a UMMA tile
+// one linear layer in the requested precision: tensor cores (bf16 operands) when the
+// net carries packed images and the layer is big enough to fill a 128-row tile
 static int run_lin(const dyn_net* n, const LinearP& l, const LinArgs& a, int prec, cudaStream_t st) {
   if (prec == DYN_PREC_BF16 && n->packed != nullptr && a.M >= 128 && l.out >= 16)
     return launch_linear_tc(a, reinterpret_cast<const char*>(n->packed) + l.tc, st);
@@ -764,7 +764,7 @@ int motion_f32(const dyn_net* n, const float* x, int ldx, bool time_is_column, f
                long long N_all, float* coeff, void* ws, size_t ws_bytes, int prec, cudaStream_t st) {
   const MotionLayout& L = n->ml;
   if (prec == DYN_PREC_BF16 && n->chain[0].img != nullptr) {
-    // whole MLP in one tcgen05 kernel (chains_fused.cu); no workspace needed
+    // whole MLP in one tensor-core kernel (chains_fused.cu); no workspace needed
     MotionFusedArgs a;
     memset(&a, 0, sizeof(a));
     a.x = x; a.ldx = ldx; a.time_is_column = time_is_column ? 1 : 0; a.time = time;
@@ -809,7 +809,7 @@ void motion_freqs(float f[16]) {
 }
 
 // ---------------------------------------------------------------------------
-// Fused (DYN_PREC_BF16) evaluation: per-view stage in ONE tcgen05 kernel
+// Fused (DYN_PREC_BF16) evaluation: per-view stage in ONE tensor-core kernel
 // (nets_fused.cu: projection + gather + per-view MLP chain + pooling), then the
 // per-point tail and heads as staged tensor-core layers.
 // ---------------------------------------------------------------------------
@@ -849,7 +849,7 @@ size_t net_fused_workspace(int kind, int R, int S, int V) {
 }
 
 // per-point stage on the fused chains: point1 (geometry_fc, Q|K|V) -> ray-transformer
-// attention (tcgen05 when S divides 128, else the SIMT kernel) -> point2 (fc + LayerNorm + heads);
+// attention (tensor cores when S divides 128, else the SIMT kernel) -> point2 (fc + LayerNorm + heads);
 // G, Q, K, V, O are bf16 tile images, g2 / GW use the fp32 tile layout (fused_engine.cuh)
 static int run_point_fused(const dyn_net* n, const float* G, long long P, int R, int S, bool dynamic,
                            float* posenc_tab, TrunkBufs& t, Point2Args& p2, cudaStream_t st) {

@@ -1,6 +1,6 @@
 // Host-side dispatch of the fused per-(point, view) stage of the two aggregation networks: argument
-// block + choice between the twin-warp kernel (view_twin.cu, default) and the quad-schedule kernel
-// (view_quad.cu, kept for comparison).
+// block + choice between the twin-warp kernel (view_twin.cu, default), the quad-schedule kernel
+// (view_quad.cu) and the sub-round pipelined twin kernel (view_twin3.cu), kept for comparison.
 //
 // Reference semantics: ibrnet/projection.py:103-176, ibrnet/mlp_network.py:236-284
 // (dynamic) and :423-497 (static).
@@ -12,12 +12,13 @@
 
 namespace dyn {
 
-constexpr int kDefaultViewKernel = 3;  // sub-round pipelined twin kernel + software-pipelined TMEM read-out (profiles/r02_kernels.md)
+// the twin-warp kernel: the fastest of them on an H100 (bench.py --view-kernel twin | pipe | quad; DESIGN.md §3.2)
+constexpr int kDefaultViewKernel = 0;
 
-// Three schedules of the same per-tile work: 0 = the twin-warp kernel (view_twin.cu: two independent CTAs per
-// SM), 1 = the quad kernel (view_quad.cu: one CTA per SM alternating between two tiles), 2 = the twin-warp
-// kernel with sub-round pipelined layers (view_twin3.cu).  DYN_VIEW_KERNEL=twin|quad|pipe or
-// dyn_debug_set_view_kernel(); profiles/r02_view_kernels.md has the comparison.
+// Three schedules of the same per-tile work: 0 = the twin-warp kernel (view_twin.cu: one CTA per SM, one
+// tile), 1 = the quad kernel (view_quad.cu: one CTA per SM alternating between two tiles), 2 = the twin-warp
+// kernel with sub-round pipelined layers (view_twin3.cu; 3 = the same with one barrier arrival per warp).
+// DYN_VIEW_KERNEL=twin|quad|pipe or dyn_debug_set_view_kernel().
 static int g_view_kernel = -1;
 void set_view_kernel(int which) { g_view_kernel = (which >= 0 && which <= 3) ? which : -1; }
 static int view_kernel() {
@@ -41,7 +42,7 @@ int producer_lanes() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("DYN_PRODUCERS");
-    v = (e != nullptr && e[0] == '2') ? 2 : 1;  // two lanes of ONE warp do not help (divergence): r02_view_kernels.md
+    v = (e != nullptr && e[0] == '2') ? 2 : 1;
   }
   return v;
 }

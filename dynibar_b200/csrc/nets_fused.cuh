@@ -10,13 +10,15 @@ constexpr int kGStride = 272;  // row stride of the pooled per-point feature G (
 
 struct FusedChunk {
   uint32_t off, bytes;   // weight chunk inside the image
-  uint16_t npad;         // UMMA N of the layer
+  uint16_t npad;         // wgmma N of the chunk (N-block of the layer: 16, 32, 48 or 64)
   uint8_t ksteps;        // K = 16 * ksteps in this chunk
   uint8_t flags;         // 1: wait for the operand (a_ready) before this chunk
                          // 2: last chunk of a round (signal the epilogue)
+                         // 4: wait for the second operand barrier (sub-round 1 of a pipelined layer)
                          // 8: first k-step overwrites D (start of a layer)
+                         // 16 / 32: last / first chunk of an N-block (fused_engine.cuh: issuer_loop)
   uint16_t a_kgroup;     // first 8-column group of the A tile this chunk consumes
-  uint16_t d_col;        // accumulator column offset inside the tile's TMEM region
+  uint16_t d_col;        // accumulator column of the chunk's first output inside the tile's region
 };
 
 struct ViewFusedArgs {
@@ -130,7 +132,7 @@ int launch_point1_fused(const dyn_net* n, Point1Args& a, cudaStream_t st);
 int launch_point2_fused(const dyn_net* n, Point2Args& a, cudaStream_t st);
 int launch_rgbhead_fused(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st);
 
-// twin-warp versions of the row-local chains (chains_twin.cu); DYN_CHAINS=fused selects the round-1 kernels
+// twin-warp versions of the row-local chains (chains_twin.cu, the default); DYN_CHAINS=fused selects chains_fused.cu
 size_t twin_chain_bytes(int kind);
 int twin_chain_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_point1_twin(const dyn_net* n, Point1Args& a, cudaStream_t st);

@@ -518,7 +518,7 @@ struct Prod {
   cudaStream_t st;
   const float* prm;
   float* dprm;
-  bool tc;      // large products on tcgen05 (train_tc.cu)
+  bool tc;      // large products on the tensor cores (train_tc.cu)
   void* img;    // scratch of tc_grad_in
   // dW[out, width] (leading dimension ldw, column offset applied by the caller) += dz^T in;
   // in[(row / bdiv) * ldin + c], optionally scaled per row

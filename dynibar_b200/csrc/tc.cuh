@@ -1,16 +1,25 @@
-// sm_100a tensor-core primitives as inline PTX: mbarrier, bulk async copy
-// (TMA engine, cp.async.bulk), TMEM allocation, tcgen05.mma / commit / ld / st,
-// and the shared-memory matrix / instruction descriptors for bf16 x bf16 -> fp32
-// UMMA with K-major, non-swizzled ("interleave") operand tiles.
+// sm_90a tensor-core primitives as inline PTX: mbarrier, bulk async copy
+// (TMA engine, cp.async.bulk), wgmma.mma_async (warpgroup MMA, bf16 x bf16 -> fp32) and its
+// shared-memory matrix descriptors for K-major / MN-major, non-swizzled ("interleave") operand tiles,
+// and the accumulator memory ("TMEM") of the fused kernels.
 //
 // Operand layout used throughout (both A [M x K] and B [N x K], bf16):
 //   8x8 core matrices of 128 contiguous bytes (8 rows x 16 B);
 //   byte offset of element (r, k) = (k/8)*LBO + (r/8)*SBO + (r%8)*16 + (k%8)*2
 //   with SBO = 128 (row groups packed back to back) and LBO = rows*16.
-// One tcgen05.mma consumes K = 16 (two core matrices along K).
+// One wgmma consumes K = 16 (two core matrices along K) for 64 rows of A.
+//
+// Accumulator memory: a 128-lane x (up to) 512-column fp32 array per CTA, laid out [column / 4][lane][4].
+// The MMA warpgroup stores each finished 128 x N block there from its wgmma registers; the row threads read
+// their row (lane = row of the 128-row tile) in blocks of 8 - 32 columns and may use columns as scratch.
+// One-tile kernels keep it in shared memory (256 columns, 128 KB), the others in their slice of a
+// device buffer (acc_pool, indexed by blockIdx.x), which stays L2-resident.  The writer stores before
+// arriving on an mbarrier and the reader loads after waiting on it (release / acquire at CTA scope).
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
+
+#include "common.cuh"
 
 namespace dyn {
 namespace tc {
@@ -37,10 +46,9 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// try_wait suspends the thread in hardware until the phase completes or a time limit expires; with the
-// default (short) limit the waiting warps of the fused kernels executed 40 % of all issued instructions
-// in this retry loop (ncu source view, profiles/r02_view_kernels.md).  The explicit suspend-time hint
-// keeps a waiting thread asleep for up to ~20 us per attempt; completion of the phase still wakes it at once.
+// try_wait suspends the thread in hardware until the phase completes or a time limit expires; the explicit
+// suspend-time hint keeps a waiting thread asleep for up to ~20 us per attempt instead of spinning in this
+// retry loop; completion of the phase still wakes it at once.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done;
   do {
@@ -55,15 +63,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 // ---- proxies / fences ---------------------------------------------------------
-// generic-proxy smem writes (st.shared) -> visible to the async proxy (UMMA reads)
+// generic-proxy smem writes (st.shared) -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---- bulk async copy global -> shared (UBLKCP), completion on an mbarrier ------
@@ -75,50 +77,95 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
       : "memory");
 }
 
-// ---- TMEM ----------------------------------------------------------------------
-// whole-warp, .sync.aligned; ncols power of two in [32, 512]
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
 // ---- descriptors ---------------------------------------------------------------
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 |
-//   [46,48) version = 1 (Blackwell) | [61,64) layout type = 0 (no swizzle)
+// wgmma shared-memory matrix descriptor: [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 |
+// base offset 0 | [62,64) layout type 0 (interleave, no swizzle).
+//   K-major operand:  LBO = byte stride between core matrices along K, SBO = along M / N.
+//   MN-major operand: LBO = byte stride between 8-row groups along K, SBO = between 8-element groups along M / N.
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes,
                                               uint32_t sbo_bytes) {
   uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = fp32 (bits [4,6) = 1),
-// A = B = bf16 ([7,10) = [10,13) = 1), both K-major (bits 15, 16 = 0),
-// N >> 3 at [17,23), M >> 4 at [24,29).
-__host__ __device__ constexpr uint32_t idesc_bf16_f32(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+
+// ---- warpgroup MMA -------------------------------------------------------------
+// D[64 x N] (+)= A[64 x 16] * B[16 x N] with A, B in shared memory; executed by all 128 threads of a
+// warpgroup.  TA / TB = 1: the operand is MN-major.  Accumulator fragment of thread t (warp w = t / 32 of
+// the warpgroup, lane l): d[i] is row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
+template <int N, int TA, int TB>
+struct Wgmma;
+template <int TA, int TB>
+struct Wgmma<16, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<32, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<48, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23"
+        "}, %24, %25, p, 1, 1, %27, %28;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait
+template <int R>
+__device__ __forceinline__ void fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- MMA -------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void mma_bf16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 // one deterministic leader lane of a fully converged warp (same lane every call)
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -129,59 +176,117 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// arrive on `bar` when every tcgen05 op issued so far by this thread has completed
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
+
+// ---- accumulator memory, addressed TMEM-style ----------------------------------------
+// tmem_alloc binds the CTA's accumulator memory and writes its base address (lane << 16 | column) to a
+// shared-memory slot; loads and stores complete in program order, so tmem_wait_* and tc_fence_* only keep
+// the compiler from moving accumulator accesses across them.  A slot of the device pool belongs to one CTA
+// from its tmem_alloc to its tmem_dealloc, so launches on several streams of a device can share the pool.
+constexpr int kAccCols = 512;
+constexpr size_t kAccCtaFloats = (size_t)kAccCols * 128;
+constexpr int kAccSmemBytes = 256 * 128 * 4;  // a one-tile kernel's accumulator memory in shared memory
+struct AccPool {
+  float* mem;  // slots x kAccCtaFloats
+  int* busy;   // slots flags: 1 = claimed
+  int slots;
+};
+static __device__ AccPool g_acc_pool;  // this translation unit's copy of acc_pool(): set by bind_acc_pool()
+static __shared__ float* s_acc;        // this CTA's accumulator memory (shared or global)
+static __shared__ int s_acc_slot;      // its pool slot, -1 in shared memory
+
+__device__ __forceinline__ void compiler_fence() { asm volatile("" ::: "memory"); }
+__device__ __forceinline__ void tc_fence_before_sync() { compiler_fence(); }
+__device__ __forceinline__ void tc_fence_after_sync() { compiler_fence(); }
+__device__ __forceinline__ void tmem_wait_ld() { compiler_fence(); }
+__device__ __forceinline__ void tmem_wait_st() { compiler_fence(); }
+
+// called by one warp before the CTA's first __syncthreads: base address 0, memory = a free slot of the
+// device pool (ncols <= kAccCols; waits while every slot is held by a running CTA) ...
+__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
+  (void)ncols;
+  if ((threadIdx.x & 31) == 0) {
+    int s = (int)(blockIdx.x % g_acc_pool.slots);
+    while (atomicCAS(g_acc_pool.busy + s, 0, 1) != 0) s = (s + 1) % g_acc_pool.slots;
+    __threadfence();
+    s_acc_slot = s;
+    s_acc = g_acc_pool.mem + (size_t)s * kAccCtaFloats;
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(dst_smem), "r"(0u) : "memory");
+  }
+}
+// ... or kAccSmemBytes of shared memory at `region` (one 128-row tile, 256 columns)
+__device__ __forceinline__ void tmem_alloc_smem(uint32_t dst_smem, void* region) {
+  if ((threadIdx.x & 31) == 0) {
+    s_acc_slot = -1;
+    s_acc = reinterpret_cast<float*>(region);
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(dst_smem), "r"(0u) : "memory");
+  }
+}
+// called by one warp after the CTA's last __syncthreads
+__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
+  (void)taddr; (void)ncols;
+  if ((threadIdx.x & 31) == 0 && s_acc_slot >= 0) {
+    __threadfence();
+    atomicExch(g_acc_pool.busy + s_acc_slot, 0);
+  }
 }
 
-// ---- TMEM <-> registers (warp w may only touch lanes 32*(w%4) .. +31) --------------
+__device__ __forceinline__ float* acc_cta() { return s_acc; }
 __device__ __forceinline__ uint32_t tmem_addr(uint32_t base, uint32_t lane, uint32_t col) {
   return base + (lane << 16) + col;
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// 16 B of (lane, 4 columns); the calling thread's lane is its lane inside the warp plus the address's lane
+__device__ __forceinline__ float4* acc_quad(uint32_t taddr) {
+  const uint32_t lane = (taddr >> 16) + (threadIdx.x & 31), col = taddr & 0xffffu;
+  return reinterpret_cast<float4*>(acc_cta()) + (size_t)(col >> 2) * 128 + lane;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+template <int NC>
+__device__ __forceinline__ void tmem_ld(uint32_t taddr, float* v) {
+  const float4* p = acc_quad(taddr);
+#pragma unroll
+  for (int i = 0; i < NC / 4; ++i) {
+    const float4 q = p[i * 128];
+    v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w;
+  }
 }
+__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) { tmem_ld<16>(taddr, v); }
+__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) { tmem_ld<32>(taddr, v); }
 __device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-        "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-        "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-        "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-        "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
+  float4* p = acc_quad(taddr);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) p[i * 128] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
 }
-__device__ __forceinline__ void tmem_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+// accumulator fragment of a 64-row wgmma (rows row0 .. row0 + 63, columns col0 .. col0 + N - 1) <-> memory
+template <int N>
+__device__ __forceinline__ void acc_store_frag(const float* d, int row0, int col0) {
+  const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  float* base = acc_cta();
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = col0 + 8 * j + 2 * (l & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 16 * w + (l >> 2) + 8 * h;
+      *reinterpret_cast<float2*>(base + ((size_t)(col >> 2) * 128 + row) * 4 + (col & 3)) =
+          make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+    }
+  }
 }
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void acc_load_frag(float* d, int row0, int col0) {
+  const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  const float* base = acc_cta();
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = col0 + 8 * j + 2 * (l & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 16 * w + (l >> 2) + 8 * h;
+      const float2 q = *reinterpret_cast<const float2*>(base + ((size_t)(col >> 2) * 128 + row) * 4 + (col & 3));
+      d[4 * j + 2 * h] = q.x;
+      d[4 * j + 2 * h + 1] = q.y;
+    }
+  }
 }
 
 // ---- bf16 packing ------------------------------------------------------------------
@@ -196,4 +301,24 @@ __host__ __device__ constexpr uint32_t tile_off(uint32_t rows, uint32_t r, uint3
 }
 
 }  // namespace tc
+
+// Host: the accumulator-memory pool of the current device (allocated and zeroed on first use, kept for the life
+// of the process; a first launch inside a stream capture fails: that set-up is not capturable).
+tc::AccPool acc_pool();
+
+// Points this translation unit's g_acc_pool at the current device's pool.
+static inline int bind_acc_pool() {
+  static float* bound[64] = {};  // what this translation unit's symbol holds, per device
+  int dev = 0;
+  DYN_CUDA(cudaGetDevice(&dev));
+  const tc::AccPool p = acc_pool();
+  if (p.mem == nullptr) return DYN_E_CUDA;
+  if (dev < 0 || dev >= 64) return fail(DYN_E_INVALID, "device index %d out of range", dev);
+  if (bound[dev] != p.mem) {
+    DYN_CUDA(cudaMemcpyToSymbol(tc::g_acc_pool, &p, sizeof(p)));
+    bound[dev] = p.mem;
+  }
+  return DYN_OK;
+}
+
 }  // namespace dyn

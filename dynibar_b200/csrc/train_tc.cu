@@ -1,17 +1,17 @@
-// Tensor-core products of the training backward (bf16 operands, fp32 accumulation in TMEM, fp32 master
+// Tensor-core products of the training backward (bf16 operands, fp32 accumulation, fp32 master
 // weights and gradients): the two GEMMs per linear layer that dominate a training step,
 //
 //   dW[out, width] += dZ^T X      (tc_grad_w)   reduction over the ROWS: both operands are read exactly as they lie
 //                                               in HBM (row-major, the reduction index is the slow one) and staged as
-//                                               MN-major UMMA operands -- no transposition anywhere
+//                                               MN-major wgmma operands -- no transposition anywhere
 //   dIn[rows, width] = dZ W[:, c0:c0+width]  (tc_grad_in)  == a forward linear layer whose weight is a transposed
 //                                               slice of W: packed on the fly, then linear_tc.cu's kernel
 //
-// tc_grad_w: one CTA owns a slab of rows.  Warps 0-7 stage 64 rows at a time (fp32 -> bf16, one 16-byte chunk =
+// tc_grad_w: a CTA owns a slab of rows and a 128 x 128 tile of dW; warps 0-7 stage 64 rows at a time (one 16 B chunk =
 // 8 consecutive columns of one row per store; 8 consecutive rows form one 128-byte core matrix whose CONTIGUOUS
 // dimension is M / N, i.e. the canonical MN-major no-swizzle layout: LBO = 128 B between 8-row groups along K,
-// SBO = 64 * 16 B between 8-column groups along M / N); warp 8 issues tcgen05.mma (a_major = b_major = MN) over a
-// 2-stage ring; the accumulators (out x width fp32, up to 2 x 256 TMEM columns) live in TMEM for the whole slab and
+// SBO = 64 * 16 B between 8-column groups along M / N); warpgroup g multiplies rows 64 g .. of the tile with wgmma (both
+// operands MN-major) over a 2-stage ring; its accumulators live in registers for the whole slab and
 // are added to dW with float atomics at the end.
 #include "linear_tc.cuh"
 #include "tc.cuh"
@@ -23,11 +23,10 @@ using namespace tc;
 
 namespace {
 
-constexpr int kRowsStage = 64;                       // K per stage
-// one stage = A image (Mpad columns) + B image (Npad columns) of 64 rows; two stages.  256 x 256: 128 KB (one CTA
-// per SM); 128 x 128: 64 KB (three per SM)
-__host__ __device__ constexpr int gw_stage_bytes(int Mpad, int Npad) { return (Mpad + Npad) * kRowsStage * 2; }
-__host__ __device__ constexpr int gw_smem(int Mpad, int Npad) { return 2 * gw_stage_bytes(Mpad, Npad) + 1024; }
+constexpr int kRowsStage = 64;   // K per stage
+constexpr int kTileM = 128, kTileN = 128;
+constexpr int kStageBytes = (kTileM + kTileN) * kRowsStage * 2;  // 32 KB
+constexpr int kGwSmem = 2 * kStageBytes;
 
 struct GradWArgs {
   const float* dz; long long lddz; int out;
@@ -35,14 +34,8 @@ struct GradWArgs {
   const float* kscale;
   long long rows, rows_per_cta;
   float* dW; long long ldw;
-  int Mpad, Npad;
+  int mtiles, nblocks;
 };
-
-// instruction descriptor: D fp32, A = B = bf16, BOTH MN-major (bits 15, 16), N >> 3 at [17,23), M >> 4 at [24,29)
-__host__ __device__ constexpr uint32_t idesc_bf16_f32_mn(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
 
 // 8 consecutive columns [c, c + 8) of row `row` (zero outside the matrix), scaled, as 8 bf16
 __device__ __forceinline__ uint4 load8_bf16(const float* __restrict__ p, long long ld, long long row, long long rows,
@@ -64,121 +57,104 @@ __device__ __forceinline__ uint4 load8_bf16(const float* __restrict__ p, long lo
   return q;
 }
 
-__global__ void __launch_bounds__(288, 2) grad_w_tc_kernel(const __grid_constant__ GradWArgs a) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int kStageBytes = gw_stage_bytes(a.Mpad, a.Npad);
-  const int kOpBytes = a.Mpad * kRowsStage * 2;  // the A image; the B image follows it
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * kStageBytes);
-  // bars: [0,1] full (256 arrivals), [2,3] empty (tcgen05.commit), [4] done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t bar0 = smem_u32(bars);
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  const int mtiles = a.Mpad >> 7;
-  const int need_cols = mtiles * a.Npad;
-  const uint32_t tmem_cols = need_cols <= 32 ? 32u : (need_cols <= 64 ? 64u : (need_cols <= 128 ? 128u : (need_cols <= 256 ? 256u : 512u)));
-  if (tid == 0) {
-    mbar_init(BAR(0), 256); mbar_init(BAR(1), 256);
-    mbar_init(BAR(2), 1); mbar_init(BAR(3), 1);
-    mbar_init(BAR(4), 1);
-    mbar_fence_init();
+__device__ __forceinline__ void mma_block_mn(float* d, int w, uint64_t ad, uint64_t bd, uint32_t sc) {
+  switch (w) {
+    case 16: Wgmma<16, 1, 1>::mma(d, ad, bd, sc); break;
+    case 32: Wgmma<32, 1, 1>::mma(d, ad, bd, sc); break;
+    case 48: Wgmma<48, 1, 1>::mma(d, ad, bd, sc); break;
+    default: Wgmma<64, 1, 1>::mma(d, ad, bd, sc); break;
   }
-  if (warp == 8) tmem_alloc(smem_u32(tmem_slot), tmem_cols);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+}
 
+// grid: x = slab, y = M tile * nblocks + N block
+__global__ void __launch_bounds__(256, 1) grad_w_tc_kernel(const __grid_constant__ GradWArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+  const int mt = blockIdx.y / a.nblocks, nbk = blockIdx.y % a.nblocks;
+  const int m0 = mt * kTileM, n0 = nbk * kTileN;
+  const int nw = min(kTileN, ((a.width - n0) + 15) / 16 * 16);  // columns of this N block (multiple of 16)
   const long long r_lo = (long long)blockIdx.x * a.rows_per_cta;
   const long long r_hi = r_lo + a.rows_per_cta < a.rows ? r_lo + a.rows_per_cta : a.rows;
   const int nstages = (int)((r_hi - r_lo + kRowsStage - 1) / kRowsStage);
 
-  if (warp == 8) {
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16_f32_mn(128, a.Npad);
-      for (int s = 0; s < nstages; ++s) {
-        const int sb = s & 1;
-        mbar_wait(BAR(0 + sb), (s >> 1) & 1);
-        tc_fence_after_sync();
-        const uint32_t a_addr = smem_u32(smem + sb * kStageBytes);
-        const uint32_t b_addr = a_addr + kOpBytes;
-        for (int mt = 0; mt < mtiles; ++mt) {
+  // loaders: four lanes read 4 x 32 B = one 128-byte line of a row (8 lines per warp instruction instead of 32);
+  // a warp owns 8 rows of the stage.  Groups g < 16 are 8 columns of dZ (M), g >= 16 of X (N).
+  const int srow = warp * 8 + (lane >> 2), gsel = lane & 3;
+  const bool dz_vec = (a.lddz & 3) == 0 && (reinterpret_cast<uintptr_t>(a.dz) & 15) == 0;
+  const bool x_vec = (a.ldx & 3) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0;
+  const int ngroups = 16 + nw / 8;
+  uint4 q[8];
+  auto fetch = [&](int s) {
+    const long long row = r_lo + (long long)s * kRowsStage + srow;
+    const bool row_in = row < r_hi;
+    const long long rows_lim = row_in ? a.rows : 0;  // rows of the next CTA's slab read as zero
+    const float sc = (row_in && a.kscale != nullptr) ? __ldg(a.kscale + row) : 1.f;
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            // 16 rows of the reduction = two 8-row core-matrix groups (LBO = 128 B apart); 16 column groups of the
-            // M tile start at mt * 16 * (64 rows * 16 B)
-            const uint64_t ad = smem_desc(a_addr + mt * 16 * (kRowsStage * 16) + ks * 256, 128, kRowsStage * 16);
-            const uint64_t bd = smem_desc(b_addr + ks * 256, 128, kRowsStage * 16);
-            mma_bf16_ss(tmem_base + mt * a.Npad, ad, bd, idesc, (s > 0 || ks > 0) ? 1u : 0u);
-          }
-        }
-        mma_commit(BAR(2 + sb));
-      }
-      mma_commit(BAR(4));
+    for (int j = 0; j < 8; ++j) {
+      const int g = gsel + 4 * j;
+      if (g < 16) q[j] = load8_bf16(a.dz, a.lddz, row, rows_lim, m0 + 8 * g, a.out, 1.f, dz_vec);
+      else if (g < ngroups) q[j] = load8_bf16(a.x, a.ldx, row, rows_lim, n0 + 8 * (g - 16), a.width, sc, x_vec);
     }
-  } else {
-    // ---------------- loaders: four lanes read 4 x 32 B = one 128-byte line of a row (8 lines per warp
-    //                  instruction instead of 32); a warp owns 8 rows of the stage ----------------
-    const int lane = tid & 31;
-    const int srow = warp * 8 + (lane >> 2), gsel = lane & 3;  // row of the stage, chunk phase
-    const bool dz_vec = (a.lddz & 3) == 0 && (reinterpret_cast<uintptr_t>(a.dz) & 15) == 0;
-    const bool x_vec = (a.ldx & 3) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0;
-    const int ga = a.Mpad >> 3, gb = a.Npad >> 3;
-    for (int s = 0; s < nstages; ++s) {
-      const int sb = s & 1;
-      const long long row = r_lo + (long long)s * kRowsStage + srow;
-      const bool row_in = row < r_hi;
-      const long long rows_lim = row_in ? a.rows : 0;  // rows of the next CTA's slab read as zero
-      const float sc = (row_in && a.kscale != nullptr) ? __ldg(a.kscale + row) : 1.f;
-      if (s >= 2) mbar_wait(BAR(2 + sb), ((s >> 1) - 1) & 1);
-      uint8_t* abase = smem + sb * kStageBytes + srow * 16;
-      uint8_t* bbase = abase + kOpBytes;
-      // batches of four 16-byte chunks: all loads of a batch are in flight before the first store
-      for (int g0 = gsel; g0 < ga; g0 += 16) {
-        uint4 q[4];
+  };
+  auto stash = [&](int sb) {
+    uint8_t* base = smem + sb * kStageBytes + srow * 16;
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (g0 + 4 * j < ga) q[j] = load8_bf16(a.dz, a.lddz, row, rows_lim, (g0 + 4 * j) * 8, a.out, 1.f, dz_vec);
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (g0 + 4 * j < ga) *reinterpret_cast<uint4*>(abase + (g0 + 4 * j) * (kRowsStage * 16)) = q[j];
-      }
-      for (int g0 = gsel; g0 < gb; g0 += 16) {
-        uint4 q[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (g0 + 4 * j < gb) q[j] = load8_bf16(a.x, a.ldx, row, rows_lim, (g0 + 4 * j) * 8, a.width, sc, x_vec);
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (g0 + 4 * j < gb) *reinterpret_cast<uint4*>(bbase + (g0 + 4 * j) * (kRowsStage * 16)) = q[j];
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(BAR(0 + sb));
+    for (int j = 0; j < 8; ++j) {
+      const int g = gsel + 4 * j;
+      if (g < ngroups) *reinterpret_cast<uint4*>(base + g * (kRowsStage * 16)) = q[j];
     }
-    // ---------------- epilogue: warps 0-3 own M tile 0, warps 4-7 M tile 1 ----------------
-    mbar_wait(BAR(4), 0);
-    tc_fence_after_sync();
-    const int mt = warp >> 2;
-    if (mt < mtiles) {
-      const int o = mt * 128 + (warp & 3) * 32 + (tid & 31);
-      const uint32_t lane_base = (uint32_t)((warp & 3) * 32);
-      for (int cb = 0; cb < a.Npad; cb += 16) {
-        float acc[16];
-        tmem_ld16(tmem_addr(tmem_base, lane_base, (uint32_t)(mt * a.Npad + cb)), acc);
-        tmem_wait_ld();
-        if (o < a.out) {
+  };
+
+  float acc[2][32];
+  if (nstages > 0) fetch(0);
+  for (int s = 0; s < nstages; ++s) {
+    const int sb = s & 1;
+    stash(sb);
+    fence_proxy_async_smem();
+    __syncthreads();  // stage s is complete; the wgmmas of stage s - 1 (other buffer) have retired
+    if (s + 1 < nstages) fetch(s + 1);
+    const uint32_t a_addr = smem_u32(smem + sb * kStageBytes) + wg * 8 * (kRowsStage * 16);
+    const uint32_t b_addr = smem_u32(smem + sb * kStageBytes) + 16 * (kRowsStage * 16);
+    fence_regs<32>(acc[0]);
+    fence_regs<32>(acc[1]);
+    wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 16; ++i)
-            if (cb + i < a.width) atomicAdd(a.dW + (long long)o * a.ldw + cb + i, acc[i]);
-        }
-      }
+    for (int ks = 0; ks < 4; ++ks) {
+      // 16 rows of the reduction = two 8-row core-matrix groups (LBO = 128 B apart); 8-column groups along M / N
+      // at SBO = 64 rows * 16 B
+      const uint64_t ad = smem_desc(a_addr + ks * 256, 128, kRowsStage * 16);
+      const uint32_t sc = (s > 0 || ks > 0) ? 1u : 0u;
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+        if (64 * b < nw)
+          mma_block_mn(acc[b], min(64, nw - 64 * b), ad,
+                       smem_desc(b_addr + 64 * b / 8 * (kRowsStage * 16) + ks * 256, 128, kRowsStage * 16), sc);
     }
-    tc_fence_before_sync();
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(acc[0]);
+    fence_regs<32>(acc[1]);
   }
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, tmem_cols);
+  if (nstages == 0) return;
+
+  // ---------------- epilogue: fragment -> dW (float atomics) ----------------
+  const int w = warp & 3;
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (64 * b + 8 * j >= nw) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int o = m0 + 64 * wg + 16 * w + (lane >> 2) + 8 * h;
+        if (o >= a.out) continue;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = n0 + 64 * b + 8 * j + 2 * (lane & 3) + e;
+          if (c < a.width) atomicAdd(a.dW + (long long)o * a.ldw + c, acc[b][4 * j + 2 * h + e]);
+        }
+      }
+    }
   }
 }
 
@@ -211,28 +187,26 @@ int tc_grad_w(const float* dz, long long lddz, int out, long long rows, const fl
   GradWArgs a;
   a.dz = dz; a.lddz = lddz; a.out = out; a.x = x; a.ldx = ldx; a.width = width; a.kscale = kscale;
   a.rows = rows; a.dW = dW; a.ldw = ldw;
-  a.Mpad = out <= 128 ? 128 : 256;
-  a.Npad = (width + 15) / 16 * 16;
-  // slabs: one wave of CTAs (as many as fit the GPU at this tile size), at least 1024 rows each: the epilogue adds
-  // out x width floats per CTA with atomics
-  const int smem = gw_smem(a.Mpad, a.Npad);
-  int per_sm = (227 * 1024) / smem;
-  const int tm = (a.Mpad / 128) * a.Npad;  // TMEM columns (allocated as a power of two >= 32)
-  int tcols = 32;
-  while (tcols < tm) tcols *= 2;
-  if (per_sm > 512 / tcols) per_sm = 512 / tcols;
-  if (per_sm > 2) per_sm = 2;  // launch bounds
-  if (per_sm < 1) per_sm = 1;
-  long long per = (rows + 148LL * per_sm - 1) / (148LL * per_sm);
+  a.mtiles = (out + kTileM - 1) / kTileM;
+  a.nblocks = (width + kTileN - 1) / kTileN;
+  // slabs: one wave of CTAs over all dW tiles, at least 1024 rows each: the epilogue adds a dW tile per CTA with
+  // atomics
+  int dev = 0, sms = 0;
+  DYN_CUDA(cudaGetDevice(&dev));
+  DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int tiles = a.mtiles * a.nblocks;
+  long long slabs = (sms + tiles - 1) / tiles;
+  long long per = (rows + slabs - 1) / slabs;
   per = per < 1024 ? 1024 : per;
   per = (per + kRowsStage - 1) / kRowsStage * kRowsStage;
   a.rows_per_cta = per;
   static bool attr_set = false;
   if (!attr_set) {
-    DYN_CUDA(cudaFuncSetAttribute(grad_w_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gw_smem(256, 256)));
+    DYN_CUDA(cudaFuncSetAttribute(grad_w_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGwSmem));
     attr_set = true;
   }
-  grad_w_tc_kernel<<<(unsigned)((rows + per - 1) / per), 288, smem, st>>>(a);
+  const dim3 grid((unsigned)((rows + per - 1) / per), (unsigned)tiles);
+  grad_w_tc_kernel<<<grid, 256, kGwSmem, st>>>(a);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }

@@ -1,25 +1,23 @@
-// Fused per-(point, view) stage of the two aggregation networks on tcgen05, "quad" schedule
+// Fused per-(point, view) stage of the two aggregation networks on the tensor cores, "quad" schedule
 // (reference: ibrnet/projection.py:103-176, ibrnet/mlp_network.py:236-284 (dynamic) / :423-497 (static)).
 //
 // Same per-tile work as view_twin.cu (projection, masks, view-angle difference, bilinear gather,
 // Plucker / positional encodings, ray_dir_fc, both view poolings, base_fc -> vis_fc -> vis_fc2), but
 // scheduled so that the CUDA cores never wait for the tensor pipe:
 //
-//   * ONE 576-thread CTA per SM owns TWO 128-row tiles (TMEM 2 x 256 columns, two 64 KB operand tiles);
+//   * ONE CTA per SM owns TWO 128-row tiles (TMEM 2 x 256 columns, two 64 KB operand tiles);
 //   * all 16 row warps serve BOTH tiles: every row has four threads (warps w, w+4, w+8, w+12 share the
 //     TMEM lane quadrant w & 3) that split each layer's output columns, the gathered channels and the
 //     pooled channels four ways;
 //   * the row warps ALTERNATE between the tiles phase by phase:  epilogue_k(tile 0) -> arrive ->
-//     epilogue_k(tile 1) -> arrive -> wait(tile 0) ...  While they run tile 1's epilogue the issuer warp
+//     epilogue_k(tile 1) -> arrive -> wait(tile 0) ...  While they run tile 1's epilogue the MMA warpgroup
 //     (fused_engine.cuh: issuer_loop<PP = true>) runs tile 0's next layer on the tensor cores, and vice
-//     versa, so an accumulator is normally complete by the time its epilogue starts.  With two
-//     independent CTAs per SM (view_twin.cu) a tile whose warps wait for an MMA leaves only 8 warps on
-//     the SM; here 16 warps always have work (profiles/r02_view_quad.md).
+//     versa, so an accumulator is normally complete by the time its epilogue starts.
 //   * the bilinear taps of a tile are issued one phase before they are consumed: their L2 latency is
 //     covered by the other tile's phase.
 //
 // warps 0-15 : row warps (quad index q = warp >> 2, TMEM lane quadrant = warp & 3)
-// warp 16    : MMA issuer (one elected lane)      warp 17 : weight producer (cp.async.bulk ring)
+// warps 16-19 : MMA warpgroup (wgmma)             warp 20 : weight producer (cp.async.bulk ring)
 #include <cstdlib>
 #include "fused_engine.cuh"
 #include "geometry.cuh"
@@ -39,19 +37,14 @@ constexpr int kQRing = 4;
 constexpr int Q_B2 = 0, Q_B4 = 48, Q_B5 = 176, Q_B6 = 304, Q_W6V = 432, Q_B7 = 560, Q_W8 = 688,
               Q_MISC = 816, Q_DFEAT = 832, Q_XCH5 = 880, Q_XCH7 = Q_XCH5 + 1024, kQConst = Q_XCH7 + 1024;
 constexpr int kQSmem = 2 * kQATile + kQRing * kQStage + kQConst * 4 + 256;
-constexpr int W_ISSUE = 16, W_PROD = 17;
+constexpr int W_ISSUE = 16, W_PROD = 16 + kIssuerWarps;  // MMA warpgroup, weight producer
+constexpr int kQThreads = 32 * (W_PROD + 1);
 
 __device__ __forceinline__ void quad_sync(int quadrant) {
   asm volatile("bar.sync %0, 128;" ::"r"(quadrant + 1) : "memory");
 }
 
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
+__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) { tmem_ld<8>(taddr, v); }
 
 // 11 values of one PE component: [x, cos(2^k x) k=0..4, sin(2^k x) k=0..4]
 __device__ __forceinline__ void pe_comp11(float x, float* o) {
@@ -503,7 +496,7 @@ struct QuadOps {
 };
 
 template <int VP, bool ST>
-__global__ void __launch_bounds__(576, 1) view_quad_kernel(const __grid_constant__ ViewFusedArgs a) {
+__global__ void __launch_bounds__(kQThreads, 1) view_quad_kernel(const __grid_constant__ ViewFusedArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem + 2 * kQATile;
   float* cst = reinterpret_cast<float*>(ring + kQRing * kQStage);
@@ -545,7 +538,7 @@ __global__ void __launch_bounds__(576, 1) view_quad_kernel(const __grid_constant
   if (warp == W_PROD) {
     if ((tid & 31) < a.producers)
       producer_loop<true, kQRing, kQStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
-  } else if (warp == W_ISSUE) {
+  } else if (warp >= W_ISSUE) {
     issuer_loop<true, 2, kQRing, kQStage>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base, kQATile,
                                           a.dbg ? a.dbg + 256 : nullptr);
   } else {
@@ -744,14 +737,16 @@ int launch_view_quad(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st)
   const long long n_iter = (a.P * VP + 255) / 256;
   const int grid = (int)(n_iter < sms ? n_iter : sms);
   if (grid == 0) return DYN_OK;
+  const int rc = bind_acc_pool();
+  if (rc) return rc;
   const bool st_net = n->kind == DYN_NET_STATIC;
   ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
   if (st_net) {
-    if (VP == 8) view_quad_kernel<8, true><<<grid, 576, kQSmem, st>>>(a);
-    else view_quad_kernel<16, true><<<grid, 576, kQSmem, st>>>(a);
+    if (VP == 8) view_quad_kernel<8, true><<<grid, kQThreads, kQSmem, st>>>(a);
+    else view_quad_kernel<16, true><<<grid, kQThreads, kQSmem, st>>>(a);
   } else {
-    if (VP == 8) view_quad_kernel<8, false><<<grid, 576, kQSmem, st>>>(a);
-    else view_quad_kernel<16, false><<<grid, 576, kQSmem, st>>>(a);
+    if (VP == 8) view_quad_kernel<8, false><<<grid, kQThreads, kQSmem, st>>>(a);
+    else view_quad_kernel<16, false><<<grid, kQThreads, kQSmem, st>>>(a);
   }
   DYN_LAUNCH_CHECK();
   return DYN_OK;

@@ -1,4 +1,4 @@
-// Fused per-(point, view) stage of the two aggregation networks on tcgen05 (reference:
+// Fused per-(point, view) stage of the two aggregation networks on the tensor cores (reference:
 // ibrnet/projection.py:103-176, ibrnet/mlp_network.py:236-284 (dynamic) / :423-497 (static)).
 // Per 128-row tile, without leaving the SM:
 //
@@ -10,19 +10,18 @@
 //   visibility re-weighting and the second mean/var pooling -> G (bf16 tile image) per point
 //
 // Engine: fused_engine.cuh (operand tile in shared memory written by the epilogues, accumulators
-// in TMEM, weights streamed through a cp.async.bulk ring, table-driven MMA issuer).  Every row is
+// in TMEM, weights streamed through a cp.async.bulk ring, table-driven MMA warpgroup).  Every row is
 // served by TWO threads in twin warps w and w + 4*NT (same TMEM lane quadrant), which is what the
 // latency-bound epilogues need; each twin owns half of every layer's output columns and half of the
 // gathered / pooled channels, and the twins exchange only two scalars per row and iteration (the
 // partial visibility logits).
 //
-// TWO independent CTAs per SM, each with one 128-row tile:
-//   warps 0-3 : twin 0 (quadrant = w & 3)      warps 4-7 : twin 1 of the same rows
-//   warp 8    : MMA issuer (one elected lane)  warp 9    : weight producer
-// (the NT = 2 template value -- one 576-thread CTA with two ping-pong tiles -- was measured 5 % slower in
-// round 1 and is no longer instantiated; the alternating two-tile schedule lives in view_quad.cu).
+// One CTA per SM with one 128-row tile:
+//   warps 0-3  : twin 0 (quadrant = w & 3)  warps 4-7 : twin 1 of the same rows
+//   warps 8-11 : MMA warpgroup (wgmma)      warp 12   : weight producer
+// (the alternating two-tile schedule lives in view_quad.cu).
 //
-// Latency hiding inside a CTA (round 2, profiles/r02_view_kernels.md): the source views are read in
+// Latency hiding inside a CTA: the source views are read in
 // their packed per-frame layouts (bf16 channels-last features: 2 x 16-byte loads per tap and twin; RGBA
 // fp32 images: 1 load per tap), the taps are ISSUED right after the projection and consumed after the
 // positional-encoding operand has been built and handed to the tensor cores, the per-ray reference
@@ -40,21 +39,19 @@ using namespace fe;
 
 namespace {
 
-constexpr bool kTwinPP = true;  // ping-pong (measured 8% faster than lock-step, profiles/r01_kernels.md)
+constexpr bool kTwinPP = true;  // ping-pong between the tiles of a two-tile CTA
 constexpr int kTwinATile = 69632;  // K <= 256 (+ one k-step of bias columns): 34 k-groups
 // T_B5 / T_B7 hold log2(e) * bias, T_W6V / T_W8 hold ln(2) * weight (the hidden activations of vis_fc.0 and
 // vis_fc2.0 live on the exp2 scale); the biases of base_fc.2 and vis_fc.2 ride in the MMA
 constexpr int T_B2 = 0, T_B5 = 48, T_W6V = 176, T_B7 = 304, T_W8 = 432, T_MISC = 560, T_DFEAT = 576,
               T_CAMS = 624 /* 16 views x (P 12 + centre 3 + pad) */, T_XCH = T_CAMS + 256;  // + 2 x [2][128] exchange
 constexpr int kTwinConst = T_XCH + 512;
-// NT = 128-row tiles per CTA: 2 -> one 576-thread CTA per SM (ping-pong between its tiles);
-// 1 -> two independent 320-thread CTAs per SM, each with one tile and a 2-slot weight ring, so
-// the tensor pipe is shared by two unsynchronised instruction streams.
-// weight ring: 16 KB stages; 8 KB stages x twice the slots measured 14 % slower (per-chunk barrier and
-// issue overhead outweighs the faster slot turnover, profiles/r01_kernels.md)
-constexpr int kTwinStage = 16384;
+// NT = 128-row tiles per CTA (only NT = 1 is instantiated); 8 KB weight stages leave room for TMEM in shared memory.
+constexpr int kTwinStage = 8192;
 constexpr int twin_ring(int nt) { return nt == 1 ? 2 : 4; }
-constexpr int twin_smem(int nt) { return nt * kTwinATile + twin_ring(nt) * kTwinStage + kTwinConst * 4 + 256; }
+constexpr int twin_threads(int nt) { return nt * 256 + 32 * (kIssuerWarps + 1); }
+// shared memory: operand tile(s) | weight ring | constants | barriers (256 B) | accumulator memory (one tile)
+constexpr int twin_smem(int nt) { return nt * kTwinATile + twin_ring(nt) * kTwinStage + kTwinConst * 4 + 256 + kAccSmemBytes; }
 
 __device__ __forceinline__ void pair_sync(int pair) {
   asm volatile("bar.sync %0, 64;" ::"r"(pair + 1) : "memory");
@@ -104,12 +101,12 @@ __device__ __forceinline__ void elu_block_to_A(uint8_t* arow, uint32_t tacc, int
 }
 
 template <int VP, bool ST, int NT>
-__global__ void __launch_bounds__(NT * 256 + 64, NT == 1 ? 2 : 1)
+__global__ void __launch_bounds__(twin_threads(NT), 1)
     view_twin_kernel(const __grid_constant__ ViewFusedArgs a) {
   constexpr int ROWS = 128 * NT;          // rows per iteration
   constexpr int RING = twin_ring(NT);
   constexpr bool PP = (NT == 2) && kTwinPP;
-  constexpr int W_ISSUE = 8 * NT, W_PROD = 8 * NT + 1;
+  constexpr int W_ISSUE = 8 * NT, W_PROD = 8 * NT + kIssuerWarps;  // MMA warpgroup, weight producer
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem + NT * kTwinATile;
   float* cst = reinterpret_cast<float*>(ring + RING * kTwinStage);
@@ -141,7 +138,8 @@ __global__ void __launch_bounds__(NT * 256 + 64, NT == 1 ? 2 : 1)
       cst[T_MISC + 2] = (ST && a.o_s >= 0) ? fabsf(prm[a.o_s]) : 0.f;
     }
   }
-  if (warp == W_ISSUE) tmem_alloc(smem_u32(tmem_slot), 256 * NT);
+  static_assert(NT == 1, "the accumulator memory in shared memory holds one tile");
+  if (warp == W_ISSUE) tmem_alloc_smem(smem_u32(tmem_slot), smem + twin_smem(NT) - kAccSmemBytes);
   tc_fence_before_sync();
   __syncthreads();
   tc_fence_after_sync();
@@ -153,7 +151,7 @@ __global__ void __launch_bounds__(NT * 256 + 64, NT == 1 ? 2 : 1)
   if (warp == W_PROD) {
     if ((tid & 31) < a.producers)
       producer_loop<PP, RING, kTwinStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
-  } else if (warp == W_ISSUE) {
+  } else if (warp >= W_ISSUE) {
     issuer_loop<PP, NT, RING, kTwinStage>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base, kTwinATile,
                            a.dbg ? a.dbg + 128 : nullptr);
   } else {
@@ -772,17 +770,18 @@ int launch_view_twin(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st)
   a.ablate = ablate;
   const int VP = V <= 8 ? 8 : 16;
   const long long n_iter = (a.P * VP + 127) / 128;
-  const long long slots = 2LL * sms;
+  static_assert(2 * twin_smem(1) > 227 * 1024, "one CTA per SM");  // shared memory holds the accumulators
+  const long long slots = sms;
   const int grid = (int)(n_iter < slots ? n_iter : slots);
   if (grid == 0) return DYN_OK;
   const bool st_net = n->kind == DYN_NET_STATIC;
   ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
   if (st_net) {
-    if (VP == 8) view_twin_kernel<8, true, 1><<<grid, 320, twin_smem(1), st>>>(a);
-    else view_twin_kernel<16, true, 1><<<grid, 320, twin_smem(1), st>>>(a);
+    if (VP == 8) view_twin_kernel<8, true, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
+    else view_twin_kernel<16, true, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
   } else {
-    if (VP == 8) view_twin_kernel<8, false, 1><<<grid, 320, twin_smem(1), st>>>(a);
-    else view_twin_kernel<16, false, 1><<<grid, 320, twin_smem(1), st>>>(a);
+    if (VP == 8) view_twin_kernel<8, false, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
+    else view_twin_kernel<16, false, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
   }
   DYN_LAUNCH_CHECK();
   return DYN_OK;

@@ -29,7 +29,7 @@ from dynibar_b200 import weights as _weights
 from dynibar_b200._lib import lib, ptr, f32c, check, stream, dev_of, Args
 from dynibar_b200.projection import project_gather
 
-# GEMM precision of the network kernels: "bf16" = tcgen05 (bf16 operands / fp32 accumulate and statistics; the
+# GEMM precision of the network kernels: "bf16" = tensor cores (bf16 operands / fp32 accumulate and statistics; the
 # production mode and the default), "fp32" = SIMT everywhere (parity mode).  Three ways to choose, innermost wins:
 # the `precision=` argument of render_rays_mv / render_rays_mono (per call), `precision_scope(name)` (per
 # thread, a context manager), `set_precision(name)` / the DYNIBAR_B200_PRECISION environment variable (process
@@ -290,7 +290,7 @@ def net_static_forward(module, pts, ref_rays, src_rays, rgb_feat, ray_diff, mask
 
 
 # ---------------------------------------------------------------------------
-# fused a4-a11 (DYN_PREC_BF16): gather + per-view MLP chain in one tcgen05 kernel
+# fused a4-a11 (DYN_PREC_BF16): gather + per-view MLP chain in one tensor-core kernel
 # ---------------------------------------------------------------------------
 class _FrameCache(object):
   """Packed per-frame copies of the source views, keyed by the IDENTITY of the source tensor (a weak
@@ -527,7 +527,7 @@ def _render_pass(ray_batch, feat_dy, feat_st, pts, z, s, t, frame_idx, offsets, 
   fused = (_prec() == _lib.PREC_BF16 and USE_FUSED and ray_batch["src_cameras"].shape[1] <= 16
            and ray_batch["static_src_cameras"].shape[1] <= 16)
   if fused:
-    # gather + per-view MLP chain + pooling in one tcgen05 kernel per branch: the
+    # gather + per-view MLP chain + pooling in one tensor-core kernel per branch: the
     # [R,S,V,35] gather output and the per-view activations never reach HBM
     raw_dy, m_dy = net_dynamic_fused(net_dy, pts, seq, ray_dir, cam, ray_batch["src_rgbs"],
                                      ray_batch["src_cameras"], featmaps_channels_last(feat_dy), t)
@@ -602,7 +602,7 @@ def render_rays_mono(frame_idx, time_embedding, time_offset, ray_batch, model, f
   """Coarse-only rendering for monocular video (render_ray.py:870-1277), including the
   cross-time branch (:1099-1270) when is_train=True.  With gradients enabled and parameters / feature
   maps that require grad the differentiable fp32 training path runs (`_render_mono_train`); otherwise
-  the forward-only kernels (fused tcgen05 path in bf16 mode) under no_grad."""
+  the forward-only kernels (fused tensor-core path in bf16 mode) under no_grad."""
   if _wants_grad(model, featmaps):
     with precision_scope(precision):
       return _render_mono_train_chunked(frame_idx, time_embedding, time_offset, ray_batch, model, featmaps,
@@ -717,7 +717,7 @@ def _render_mono_train(frame_idx, time_embedding, time_offset, ray_batch, model,
   the parameters of motion_mlp / net_coarse_dy / net_coarse_st and the feature maps.  torch itself only
   concatenates the time column, zeroes the last samples' coefficients, slices and detaches.  Precision (the
   library-wide setting / `precision=`): "bf16" runs the products of the three networks, forward and backward, on
-  tcgen05 (bf16 operands, fp32 accumulation, fp32 master weights and gradients); "fp32" = SIMT products."""
+  tensor cores (bf16 operands, fp32 accumulation, fp32 master weights and gradients); "fp32" = SIMT products."""
   from dynibar_b200 import autograd as ag
   t = _scalar(time_embedding[0].float())
   rb, hb = _with_host_copies(ray_batch, model, ("trajectory_basis",))

@@ -1,9 +1,9 @@
-/* dynibar_b200 -- C ABI of the B200-native DynIBaR per-ray IBR hot path.
+/* dynibar_b200 -- C ABI of the CUDA-native DynIBaR per-ray IBR hot path (H100, sm_90a).
  *
  * The reference (google/dynibar @ 5412b55) has no FFI layer: its boundary for
  * this path is the Python call surface of ibrnet/render_ray.py,
  * ibrnet/projection.py and ibrnet/mlp_network.py.  Each entry point below
- * names the reference function (file:line under /root/reference) it replaces;
+ * names the reference function (file:line in the reference checkout) it replaces;
  * the Python modules under dynibar_b200/ bind them with ctypes behind the reference's own
  * function / class names (see INTEGRATION.md).
  *
@@ -13,8 +13,12 @@
  *     The tiny per-frame arrays (`*_cam`, `*_cams`, `basis`) may be HOST
  *     pointers as well: host copies are read without synchronising the stream.
  *   - the caller owns every buffer (inputs, outputs, workspace, packed
- *     weights); the library never allocates or frees device memory and keeps
- *     no device pointer after return except inside a `dyn_net_t` handle.
+ *     weights); the library keeps no device pointer after return except inside
+ *     a `dyn_net_t` handle.  Its one allocation: on the first fused tensor-core
+ *     launch on a device it allocates device memory for the accumulators of the
+ *     fused kernels (2 x SMs x 256 KB, kept for the life of the process; a
+ *     CTA holds one slot of it while it runs, so streams can share it).  The
+ *     first fused launches on a device must not be inside a stream capture.
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it,
  *     nothing synchronises.
  *   - return 0 on success, a negative DYN_E_* otherwise; `dyn_last_error()`
@@ -42,7 +46,7 @@ extern "C" {
 #define DYN_NET_MOTION 2  /* MotionMLP,      mlp_network.py:558 */
 
 #define DYN_PREC_FP32 0 /* SIMT fp32 everywhere (parity mode) */
-#define DYN_PREC_BF16 1 /* tcgen05: bf16 operands, fp32 accumulate/statistics */
+#define DYN_PREC_BF16 1 /* tensor cores (wgmma): bf16 operands, fp32 accumulate/statistics */
 
 typedef struct dyn_net* dyn_net_t;
 
@@ -69,7 +73,7 @@ int dyn_profile_read(int cls, float* total_ms, int* launches);
  * names, mlp_network.py:159-214 / :349-403 / :591-603).  `n_params` is checked
  * against the expected count.  `packed` is a caller-owned device buffer of
  * dyn_net_packed_bytes(kind) bytes that receives the tensor-core operand
- * images (bf16, UMMA canonical layout); it may be NULL for DYN_PREC_FP32 use.
+ * images (bf16, wgmma canonical layout); it may be NULL for DYN_PREC_FP32 use.
  * n_samples sizes the sinusoid table of the dynamic net (mlp_network.py:218).
  */
 size_t dyn_net_param_count(int kind);
@@ -238,7 +242,7 @@ int dyn_resample(const float* z_vals, const float* weights, const float* u,
  * (dyn_encoder_train_workspace_bytes); the backward ACCUMULATES d(loss)/d(params) into d_params (n_params floats, the
  * order of dyn_encoder_forward's `params`; the caller zeroes it) from d_coarse / d_fine [N,32,H/4,W/4] (either may be
  * NULL).  The images carry no gradient.  Every convolution is differentiated through its im2col form; `precision`
- * DYN_PREC_BF16 runs the two products per convolution on tcgen05 (bf16 operands, fp32 accumulation). */
+ * DYN_PREC_BF16 runs the two products per convolution on the tensor cores (bf16 operands, fp32 accumulation). */
 size_t dyn_encoder_train_workspace_bytes(int N, int H, int W);
 size_t dyn_encoder_backward_scratch_bytes(int N, int H, int W);
 int dyn_encoder_train_forward(const float* params, size_t n_params, const float* images, int N, int H, int W,
@@ -294,7 +298,7 @@ int dyn_motion_mlp_backward(dyn_net_t motion, const float* xyzt, const float* d_
  * d_rgb_feat [R,S,V,35] (gradient w.r.t. the gathered colours + features; NULL to skip) and, for the dynamic net,
  * d_pts [R,S,3] (through the positional encoding of ref_pts_fc; NULL to skip).  mask / ray_diff / rays / time carry
  * no gradient (the reference detaches them).  `precision`: DYN_PREC_FP32 = SIMT products; DYN_PREC_BF16 = the
- * products of the large layers on tcgen05 (bf16 operands, fp32 accumulation, fp32 master weights / gradients; the
+ * products of the large layers on the tensor cores (bf16 operands, fp32 accumulation, fp32 master weights / gradients; the
  * net must have been created with layer images, dyn_net_create_ex pack_level >= 1); everything else stays fp32.
  * Float atomics (not bit-reproducible between runs). */
 size_t dyn_net_train_workspace_bytes(int kind, int R, int S, int V);
@@ -365,11 +369,13 @@ int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid,
                           void* stream);
 
 /* ---- unit-test hook (HOST only, no GPU needed): pack one nn.Linear [N, Kw] into the bf16
- * UMMA weight image the fused kernels stream (dynibar_b200/csrc/fused_engine.cuh:
+ * wgmma weight image the fused kernels stream (dynibar_b200/csrc/fused_engine.cuh:
  * append_layer).  colmap[Kpad] maps operand column -> weight column, -1 = zero,
  * -2 / -3 = hi / lo bf16 halves of the folded bias; `scale` multiplies weights and
- * bias.  Chunks of `stage_bytes`; element (n, k) of a chunk that starts at k0 sits at
- * byte ((k-k0)/8)*(Npad*16) + (n/8)*128 + (n%8)*16 + ((k-k0)%8)*2 of that chunk.
+ * bias.  The outputs are packed in N-blocks of nb = min(64, Npad - n0) rows, each cut
+ * along K into chunks of at most min(8, stage_bytes / (nb*32)) k-steps of 16;
+ * element (n, k) of a chunk that starts at (n0, k0) sits at byte
+ * ((k-k0)/8)*(nb*16) + ((n-n0)/8)*128 + ((n-n0)%8)*16 + ((k-k0)%8)*2 of that chunk.
  * Writes the image into out_img (out_bytes capacity), its size into *img_bytes and the
  * number of chunks into *nchunks. */
 int dyn_debug_pack_layer(const float* W, const float* bias, int N, int Kw, int Npad,
@@ -380,20 +386,20 @@ int dyn_debug_pack_layer(const float* W, const float* bias, int N, int Kw, int N
  * 128-row tile: the layout activations use between the fused kernels. */
 size_t dyn_debug_tile_image_off(long long row, int kgroup, int kgroups);
 
-/* comparison hook: which kernel runs the fused per-view stage: 0 = twin-warp kernel (csrc/view_twin.cu: two
- * independent CTAs per SM), 1 = quad-schedule kernel (csrc/view_quad.cu: one CTA per SM alternating between
+/* comparison hook: which kernel runs the fused per-view stage: 0 = twin-warp kernel (csrc/view_twin.cu: one
+ * tile per CTA, the default), 1 = quad-schedule kernel (csrc/view_quad.cu: one CTA per SM alternating between
  * two tiles), 2 = twin-warp kernel with sub-round pipelined layers (csrc/view_twin3.cu).  The environment
  * variable DYN_VIEW_KERNEL=twin|quad|pipe sets the initial value. */
 void dyn_debug_set_view_kernel(int which);
 
 /* profiling hook: when set, block 0 of the fused static per-view kernel writes clock64()
- * phase timestamps ([2 twins][64]) into dev_buf (profiles/scripts/prof_phases.py). */
+ * phase timestamps ([2 twins][64]) into dev_buf. */
 void dyn_debug_set_view_timestamps(long long* dev_buf);
 
 /* ---- building block: one nn.Linear on the tensor cores -----------------------
  * Y[M,N] = act(X[M,K] W[N,K]^T + b) with bf16 operands / fp32 accumulation
- * (tcgen05).  act: 0 none, 1 ELU, 2 ReLU, 3 sigmoid.  N <= 256.  packed_ws must
- * hold dyn_linear_tc_packed_bytes(N, K) bytes (bf16 UMMA image of W).  This is
+ * (wgmma).  act: 0 none, 1 ELU, 2 ReLU, 3 sigmoid.  N <= 256.  packed_ws must
+ * hold dyn_linear_tc_packed_bytes(N, K) bytes (bf16 wgmma image of W).  This is
  * the kernel behind every nn.Linear of mlp_network.py in DYN_PREC_BF16 mode;
  * exported for unit testing. */
 size_t dyn_linear_tc_packed_bytes(int N, int K);

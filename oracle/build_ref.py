@@ -17,7 +17,7 @@ import sys
 import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_SRC = "/root/reference/ibrnet"
+REF_SRC = os.path.join(os.environ.get("DYNIBAR_REFERENCE", "/root/reference"), "ibrnet")
 OUT = os.path.join(HERE, "_ref", "ibrnet")
 MODULES = ("render_ray", "projection", "mlp_network", "render_image", "sample_ray", "feature_network")
 

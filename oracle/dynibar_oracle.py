@@ -8,7 +8,7 @@ arm.  The product (`dynibar_b200/`) never imports it and has no CPU fallback.
 Pinning: `tests/golden/make_golden.py` runs the UNMODIFIED reference from
 /root/reference on seeded inputs and commits the tensors under tests/golden/;
 `tests/test_oracle_golden.py` checks this restatement against those fixtures
-(and, when /root/reference is present, against the live reference).
+(and against a further stored run, tests/golden/live_reference.pt).
 
 Everything is functional: network weights arrive as plain `state_dict`s whose
 key names are the reference's (`base_fc.0.weight`, `ray_attention.w_qs.weight`

@@ -22,7 +22,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-REF = "/root/reference"
+REF = os.environ.get("DYNIBAR_REFERENCE", "/root/reference")  # as in oracle/build_ref.py
+# the gather outputs rgb_feat_* [R,S,V,35] dominate a fixture: they are stored for every STAGE_RAY_STEP-th ray
+# only (whole rays: the networks couple the samples of a ray), which keeps each fixture under 1 MB
+STAGE_RAY_STEP = 3
 
 warnings.filterwarnings("ignore")
 
@@ -122,6 +125,15 @@ def stage_tensors(ref, batch, feat, model_ref, args, frame, t, offs, S, num_vv,
               ref_plucker=ref_pl, src_plucker=src_pl)
 
 
+def sample_stage_rays(st):
+  """keep rgb_feat_dy / rgb_feat_st for the rays rgb_feat_rays only"""
+  rays = torch.arange(0, st["rgb_feat_dy"].shape[0], STAGE_RAY_STEP)
+  st["rgb_feat_rays"] = rays
+  for k in ("rgb_feat_dy", "rgb_feat_st"):
+    st[k] = st[k][rays].clone()
+  return st
+
+
 def clean(d):
   if d is None:
     return None
@@ -164,9 +176,9 @@ def main():
                                   N_importance=cfg["N_importance"], det=False,
                                   is_train=False)
       fx["rand_outputs_fine_ref"] = clean(ret["outputs_fine_ref"])
-    fx["stages"] = clean(stage_tensors(ref, batch, feat_c, mref, args, frame, t,
-                                       offs, cfg["N_samples"], cfg["num_vv"],
-                                       cfg["inv_uniform"]))
+    fx["stages"] = sample_stage_rays(clean(stage_tensors(ref, batch, feat_c, mref, args, frame, t,
+                                                         offs, cfg["N_samples"], cfg["num_vv"],
+                                                         cfg["inv_uniform"])))
     path = os.path.join(HERE, name + ".pt")
     torch.save(fx, path)
     print(name, "->", path, "%.1f KB" % (os.path.getsize(path) / 1024))

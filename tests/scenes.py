@@ -1,5 +1,7 @@
 """Seeded scene/model configurations shared by the golden generator and tests."""
 
+import zlib
+
 import torch
 
 from dynibar_b200 import synthetic
@@ -77,3 +79,18 @@ def sampler_data(batch, H, W, seed, n_flow=6):
   data["flows"] = torch.randn(1, n_flow, H, W, 2, generator=g)
   data["masks"] = (torch.rand(1, n_flow, H, W, generator=g) > 0.3).float()
   return data
+
+
+def encoder_weights(m, seed):
+  """Seeded parameters for a 2-D encoder of the reference's ResNet layout (this repository's or the reference's own
+  module): each parameter is drawn from a generator of its own (seed, name), so both get the same values."""
+  with torch.no_grad():
+    for name, p in m.named_parameters():
+      g = torch.Generator().manual_seed(seed * 1000003 + zlib.crc32(name.encode()))
+      if name.endswith("bn1.weight") or name.endswith("bn2.weight") or name.endswith("downsample.1.weight"):
+        p.copy_(torch.rand(p.shape, generator=g) + 0.5)
+      elif name.endswith(".bias"):
+        p.copy_(torch.rand(p.shape, generator=g) * 0.6 - 0.3)
+      else:
+        p.copy_(torch.randn(p.shape, generator=g) * (2.0 / p[0].numel()) ** 0.5)
+  return m.requires_grad_(False)

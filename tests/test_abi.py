@@ -25,13 +25,13 @@ def test_library_exports_every_declared_symbol():
   assert sorted(_lib.SIGNATURES) == names
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
   from dynibar_b200 import _lib
   out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True)
   if out.returncode != 0:
     return  # cuobjdump not on PATH: nothing to check
   archs = set(re.findall(r"sm_(\d+a?)", out.stdout))
-  assert archs == {"100a"}, archs
+  assert archs == {"90a"}, archs
 
 
 def test_version_and_error_string_without_gpu():

@@ -1,12 +1,13 @@
 """2-D feature encoder (row f1) against the reference's own ResNet (ibrnet/feature_network.py:179-311):
-committed fixture (tests/golden/encoder.pt, from make_golden_frame.py-style generation with the unmodified
-reference) and, when oracle/_ref is present, the live reference module on the same weights."""
+committed fixtures of the unmodified reference: tests/golden/encoder.pt (full maps of a small batch) and
+tests/golden/live_reference.pt (make_golden_live.py: a seeded sample of positions at three image sizes)."""
 
 import os
 
 import pytest
 import torch
 
+import scenes
 from dynibar_b200 import feature_network as fn
 
 pytestmark = pytest.mark.gpu
@@ -41,20 +42,17 @@ def test_encoder_matches_reference_fixture():
 
 @pytest.mark.parametrize("N,H,W", [(2, 288, 512), (3, 37, 53), (1, 135 * 4 // 4, 240)])
 def test_encoder_matches_live_reference(N, H, W):
-  from oracle import build_ref
-  if not build_ref.available():
-    pytest.skip("oracle/_ref not built")
-  ref = build_ref.load()
-  m = _model(N * 1000 + H)
-  r = ref.fn.ResNet(coarse_out_ch=32, fine_out_ch=32, coarse_only=False)
-  r.load_state_dict(m.state_dict(), strict=True)
-  x = torch.rand(N, 3, H, W)
-  with torch.no_grad():
-    wc, wf = r.eval()(x)
+  from golden import make_golden_live as ml
+  fx = torch.load(os.path.join(os.path.dirname(GOLD), "live_reference.pt"), weights_only=False)["encoder"][(N, H, W)]
+  m = scenes.encoder_weights(fn.ResNet(), N * 1000 + H)
+  x = ml.encoder_input(N, H, W)
+  assert abs(float(x.double().sum()) - fx["input_sum"]) < 1e-6 * fx["input_sum"]
   c, f = m.to(DEV)(x.to(DEV))
   torch.cuda.synchronize()
-  torch.testing.assert_close(c.cpu(), wc, rtol=2e-4, atol=2e-4)
-  torch.testing.assert_close(f.cpu(), wf, rtol=2e-4, atol=2e-4)
+  assert tuple(c.shape) == fx["shape"] and tuple(f.shape) == fx["shape"]
+  idx = ml.encoder_sample(c.numel(), N, H)
+  torch.testing.assert_close(c.cpu().flatten()[idx], fx["coarse"], rtol=2e-4, atol=2e-4)
+  torch.testing.assert_close(f.cpu().flatten()[idx], fx["fine"], rtol=2e-4, atol=2e-4)
 
 
 def test_encoder_feeds_the_renderer_layout():
@@ -69,7 +67,7 @@ def test_encoder_backward_matches_oracle_autograd(N, H, W, prec):
   """Row f2: gradients of every executed encoder parameter against torch autograd through the oracle's restatement of
   ResNet.forward (pinned to the reference by tests/test_oracle_golden.py).  fp32: 2e-3 relative L2 per tensor
   (InstanceNorm + ReLU network; the ReLU kinks make a few units flip with the summation order); bf16 products
-  (tcgen05): 1e-1."""
+  (tensor cores): 1e-1."""
   from dynibar_b200 import render_ray as rr
   from oracle import dynibar_oracle as orc
   m = _model(N * 100 + H).requires_grad_(True)

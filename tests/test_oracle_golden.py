@@ -2,10 +2,9 @@
 
 1. against the committed golden fixtures (outputs of the unmodified reference,
    tests/golden/make_golden.py) -- runs anywhere;
-2. against the live reference when /root/reference is present (build container).
+2. against reference outputs on a further seeded scene (tests/golden/live_reference.pt,
+   tests/golden/make_golden_live.py).
 """
-
-import os
 
 import pytest
 import torch
@@ -68,8 +67,9 @@ def test_oracle_matches_golden(name, golden):
   st = fx["stages"]
   _cmp("coeff", aux["coeff"], st["coeff"])
   _cmp("seq", aux["seq"], st["seq"])
-  _cmp("rgb_feat_dy", aux["rgb_feat_dy"], st["rgb_feat_dy"])
-  _cmp("rgb_feat_st", aux["rgb_feat_st"], st["rgb_feat_st"])
+  rays = st["rgb_feat_rays"]  # the fixture keeps the gather outputs of these rays (tests/golden/make_golden.py)
+  _cmp("rgb_feat_dy", aux["rgb_feat_dy"][rays], st["rgb_feat_dy"])
+  _cmp("rgb_feat_st", aux["rgb_feat_st"][rays], st["rgb_feat_st"])
   _cmp("ray_diff_st", aux["ray_diff_st"], st["ray_diff_st"])
   _cmp("mask_dy", aux["mask_dy"], st["mask_dy"])
   _cmp("mask_st", aux["mask_st"], st["mask_st"])
@@ -127,25 +127,20 @@ def test_sample_pdf_edge_cases():
   torch.testing.assert_close(s[0], torch.linspace(0, 1, 16), atol=1e-5, rtol=0)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/ibrnet"),
-                    reason="live reference only exists in the build container")
-def test_oracle_matches_live_reference():
-  from golden import make_golden as mg
-  ref = mg.import_reference()
-  cfg = dict(scenes.GOLDEN_CONFIGS["mv_small"], seed=77, rays=16, V_dy=7, V_st=4)
+def test_oracle_matches_live_reference(golden):
+  from golden import make_golden_live as ml
+  fx = golden("live_reference")["mv77"]
+  cfg = dict(scenes.GOLDEN_CONFIGS["mv_small"], **ml.MV77)
   batch, feat_c, feat_f, frame, t, offs, model, args = scenes.build(cfg)
-  mref = mg.reference_model(ref, model, args, False)
+  assert abs(_checksum(batch, [feat_c, feat_f]) - fx["checksum"]) < 1e-6 * fx["checksum"], \
+      "seeded inputs drifted from the ones the fixture was generated with"
   with torch.no_grad():
-    want = ref.rr.render_rays_mv(frame, t, offs, batch, mref, ref.proj.Projector("cpu"),
-                                 feat_c, feat_f, cfg["N_samples"], args,
-                                 inv_uniform=True, N_importance=cfg["N_importance"],
-                                 det=True, is_train=False)
     got = orc.render_rays_mv(frame, t, offs, batch, model, None, feat_c, feat_f,
                              cfg["N_samples"], args, inv_uniform=True,
                              N_importance=cfg["N_importance"], det=True, is_train=False)
   for k in ("outputs_coarse_ref", "outputs_fine_ref", "outputs_fine_ref_dy"):
-    for kk in want[k]:
-      _cmp("%s/%s" % (k, kk), got[k][kk], want[k][kk])
+    for kk in fx[k]:
+      _cmp("%s/%s" % (k, kk), got[k][kk], fx[k][kk])
 
 
 def test_oracle_encoder_matches_reference_fixture(golden):

@@ -73,7 +73,8 @@ def test_stages_against_golden(rr, golden, name):
   f, rd, mk = P.compute_with_motions(pts, _dev(st["seq"]), b["camera"], b["src_rgbs"],
                                      b["src_cameras"], fc[0])
   assert_close_frac("mask_dy", mk, st["mask_dy"], max_bad_frac=1e-3)
-  assert_close_frac("rgb_feat_dy", f, st["rgb_feat_dy"], rtol=1e-4, atol=2e-5, max_bad_frac=1e-3)
+  rays = st["rgb_feat_rays"]  # the fixture keeps the gather outputs of these rays (tests/golden/make_golden.py)
+  assert_close_frac("rgb_feat_dy", f[rays.to(DEV)], st["rgb_feat_dy"], rtol=1e-4, atol=2e-5, max_bad_frac=1e-3)
   _cmp_ray_diff("ray_diff_dy", rd, st["ray_diff_dy"])
   # the public compute_angle (projection.py:61-101), called the way compute_with_motions calls it
   # (static point expanded over the views) and with the un-expanded point
@@ -86,24 +87,26 @@ def test_stages_against_golden(rr, golden, name):
   f, rd, mk = P.compute_with_motions(pts, pts[None].repeat(V_st, 1, 1, 1), b["camera"],
                                      b["static_src_rgbs"], b["static_src_cameras"], fc[2])
   assert_close_frac("mask_st", mk, st["mask_st"], max_bad_frac=1e-3)
-  assert_close_frac("rgb_feat_st", f, st["rgb_feat_st"], rtol=1e-4, atol=2e-5, max_bad_frac=1e-3)
+  assert_close_frac("rgb_feat_st", f[rays.to(DEV)], st["rgb_feat_st"], rtol=1e-4, atol=2e-5, max_bad_frac=1e-3)
   _cmp_ray_diff("ray_diff_st", rd, st["ray_diff_st"])
   assert_close_frac("ref_plucker", rr.compute_ref_plucker_coordinate(b["ray_o"], b["ray_d"]),
                     st["ref_plucker"], rtol=1e-5, atol=1e-6)
   assert_close_frac("src_plucker", rr.compute_src_plucker_coordinate(pts, b["static_src_cameras"]),
                     st["src_plucker"], rtol=1e-5, atol=1e-6)
-  # networks on the reference's inputs; compare where >= 1 view is valid
-  ray_dir = torch.nn.functional.normalize(b["ray_d"], dim=-1)
-  raw_dy = m.net_coarse_dy(pts, _dev(st["rgb_feat_dy"]), ray_dir, None, None, _dev(st["mask_dy"]),
+  # networks on the reference's inputs (the rays whose gather outputs the fixture keeps); compare where >= 1 view
+  # is valid
+  rd = rays.to(DEV)
+  ray_dir = torch.nn.functional.normalize(b["ray_d"], dim=-1)[rd]
+  raw_dy = m.net_coarse_dy(pts[rd], _dev(st["rgb_feat_dy"]), ray_dir, None, None, _dev(st["mask_dy"][rays]),
                            torch.tensor([tt]))
-  raw_st = m.net_coarse_st(pts, _dev(st["ref_plucker"]), _dev(st["src_plucker"]),
-                           _dev(st["rgb_feat_st"]), ray_dir, _dev(st["ray_diff_st"]),
-                           _dev(st["mask_st"]))
+  raw_st = m.net_coarse_st(pts[rd], _dev(st["ref_plucker"][rays]), _dev(st["src_plucker"][rays]),
+                           _dev(st["rgb_feat_st"]), ray_dir, _dev(st["ray_diff_st"][rays]),
+                           _dev(st["mask_st"][rays]))
   for br, raw in (("dy", raw_dy), ("st", raw_st)):
-    valid = (st["mask_" + br].sum(2) > 0).expand(-1, -1, 4)
+    valid = (st["mask_" + br][rays].sum(2) > 0).expand(-1, -1, 4)
     # (a few samples sit on the mask_rgb / in-bounds discontinuities: their blending softmax
     #  differs in the 3rd digit; everything else must meet the tolerance)
-    assert_close_frac("raw_" + br, raw.cpu()[valid], st["raw_" + br][valid], rtol=2e-4, atol=2e-5,
+    assert_close_frac("raw_" + br, raw.cpu()[valid], st["raw_" + br][rays][valid], rtol=2e-4, atol=2e-5,
                       max_bad_frac=5e-3)
     inval = ~valid[..., 3]
     assert (raw.cpu()[..., 3][inval] == -1e9).all()

@@ -1,4 +1,4 @@
-"""tcgen05 path: the tensor-core linear layer against a torch reference with
+"""Tensor-core (wgmma) path: the tensor-core linear layer against a torch reference with
 the same operand rounding, and DYN_PREC_BF16 end-to-end parity.
 
 Tolerances (stated, north_star "within a stated floating-point tolerance"):
@@ -66,7 +66,7 @@ def test_bf16_mode_end_to_end(golden, name):
   from dynibar_b200.projection import Projector
   fx = golden(name)
   cfg = dict(fx["cfg"])
-  cfg["rays"] = 256  # enough rows for the UMMA tiles to be exercised
+  cfg["rays"] = 256  # enough rows for the 128-row tensor-core tiles to be exercised
   batch, feat_c, feat_f, frame, t, offs, model, args = scenes.build(cfg)
   d = lambda x: synthetic.to_device(x, DEV)
   with torch.no_grad():
@@ -156,7 +156,7 @@ def test_bf16_mode_against_oracle_at_benchmark_shapes(name):
 
 @pytest.mark.parametrize("name", ["mv_small", "mv_linear", "mono_small"])
 def test_fused_view_stage_matches_staged(golden, name):
-  """The fused per-view kernel (gather + MLP chain + pooling on tcgen05) against the
+  """The fused per-view kernel (gather + MLP chain + pooling on the tensor cores) against the
   fp32 staged path on the same inputs: raw [R,S,4] of both nets and the projector mask."""
   from dynibar_b200 import render_ray as rr
   from dynibar_b200.projection import Projector

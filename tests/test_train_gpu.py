@@ -5,7 +5,7 @@ differentiable pieces (raw2outputs_vanilla, compute_traj_pts, compute_optical_fl
 
 Bar, precision "fp32": forward values rtol 2e-4; gradients 1e-3 relative in the L2 norm per tensor (fp32 kernels
 with a different summation order than ATen; ELU is C1, so there are no kink flips except the MotionMLP's ReLUs, see
-test_backward_gpu.py).  Precision "bf16" (products on tcgen05 with bf16 operands, everything else fp32): forward
+test_backward_gpu.py).  Precision "bf16" (tensor-core products with bf16 operands, everything else fp32): forward
 2e-2, gradients 5e-2 (matrices) / 1e-1 (vectors) against the same fp32 oracle."""
 
 import pytest
@@ -123,8 +123,8 @@ def test_net_static_backward_matches_oracle_autograd(R, S, V, aa, mrgb, prec):
   (got * d(gen * scale)).sum().backward()
   for k, p in mod.named_parameters():
     # `s` (anti-alias pooling): a small sum of large cancelling terms, (e - min e) / (sum + 1e-8): 1e-2 in fp32; with
-    # bf16 products the 0.5 % noise of d(pooling weights) is amplified by 1 / (sum + 1e-8) past the signal
-    # (profiles/r02_train.md), so only finiteness is checked there
+    # bf16 products the 0.5 % noise of d(pooling weights) is amplified by 1 / (sum + 1e-8) past the signal,
+    # so only finiteness is checked there
     if k == "s":
       if prec == "fp32":
         _close(k, p.grad, w[k].grad, 1e-2)
@@ -256,11 +256,11 @@ def test_render_rays_mono_training_step_matches_oracle_autograd(name, prec):
       if mname == "net_coarse_st" and k == "s":
         # ill-conditioned in fp32 on this rig (far samples: cos ~ 1 for every view, so the pooling weights are
         # (e - min e) / (sum + 1e-8) with sum ~ 1e-6): torch's own fp32 autograd differs from its fp64 autograd by
-        # 300 % here (profiles/r02_train.md); the well-conditioned case is test_net_static_backward_*
+        # 300 % here; the well-conditioned case is test_net_static_backward_*
         assert torch.isfinite(p.grad).all()
         continue
-      # bar: 5e-3 for weight matrices -- torch's own fp32 autograd is 1.5e-3 away from its fp64 autograd on this rig
-      # (profiles/r02_train.md) -- and 2e-2 for bias / LayerNorm vectors: column sums over all rows whose terms cancel
+      # bar: 5e-3 for weight matrices -- torch's own fp32 autograd is 1.5e-3 away from its fp64 autograd on this
+      # rig -- and 2e-2 for bias / LayerNorm vectors: column sums over all rows whose terms cancel
       # to ~1e-3 of their magnitude (e.g. the blending head: sum_v d logit_v = 0 per point), so the summation order
       # shows; a wrong or missing term is an O(1) error
       if prec == "fp32":
@@ -268,7 +268,7 @@ def test_render_rays_mono_training_step_matches_oracle_autograd(name, prec):
       elif mname == "motion_mlp" and k.startswith("pts_linears"):
         # ReLU network with bf16 products: pre-activations within bf16 rounding of 0 (~0.3 % of the units per layer)
         # take the other side of the kink, each flip is an O(1) change of that unit's gradient -> sqrt(0.003) ~ 5 %
-        # in L2 at the last hidden layer, growing to ~11 % at the first (measured: profiles/r02_train.md); the smooth
+        # in L2 at the last hidden layer, growing to ~11 % at the first; the smooth
         # (ELU) aggregation nets stay at 0.2 - 0.5 %
         _close("%s.%s" % (mname, k), p.grad, w[k].grad, 2e-1, floor=1e-5)
       else:  # bf16 operands: 2^-9 per element, averaged over the reductions and chained through ~10 layers
@@ -281,7 +281,7 @@ def test_render_rays_mono_training_step_matches_oracle_autograd(name, prec):
                                                           (4100, 256, 256, 0, False), (3000, 35, 66, 3, True),
                                                           (20000, 64, 128, 1, False)])
 def test_tensorcore_training_products(rows, out, width, ldx_pad, scaled):
-  """csrc/train_tc.cu: dW += dZ^T X (MN-major UMMA operands, reduction over the rows) and dIn = dZ W on tcgen05
+  """csrc/train_tc.cu: dW += dZ^T X (MN-major wgmma operands, reduction over the rows) and dIn = dZ W on the tensor cores
   against fp64 products of the bf16-rounded operands (what the tensor cores multiply), fp32 accumulation."""
   from dynibar_b200._lib import lib, ptr, check, stream
   g = torch.Generator().manual_seed(rows + out)

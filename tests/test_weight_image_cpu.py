@@ -1,5 +1,5 @@
 """Host-side checks (no GPU) of the two memory formats the fused tensor-core kernels rely on:
-the bf16 UMMA weight image (chunked, K-major 8x8 core matrices, folded bias, scale) built by
+the bf16 wgmma weight image (N-blocks, chunked, K-major 8x8 core matrices, folded bias, scale) built by
 `fused_engine.cuh: append_layer`, and the activation tile image (`tile_image_off`)."""
 
 import ctypes
@@ -30,19 +30,28 @@ def _pack(W, bias, Npad, colmap, scale, stage):
   return out[:nbytes.value].view(np.uint16), nch.value
 
 
+def _blocks(Npad, Kpad, stage):
+  """(first output, outputs, first k-step, k-steps) of every chunk, in image order"""
+  out = []
+  for n0 in range(0, Npad, 64):
+    nb = min(64, Npad - n0)
+    steps = min(stage // (nb * 32), 8)
+    for k0 in range(0, Kpad // 16, steps):
+      out.append((n0, nb, k0, min(steps, Kpad // 16 - k0)))
+  return out
+
+
 def _unpack(img16, Npad, Kpad, stage):
   """image -> dense [Npad, Kpad] fp32, following the layout documented in include/dynibar_b200.h"""
-  steps = min(stage // (Npad * 32), 8)
   dense = np.zeros((Npad, Kpad), dtype=np.float32)
   off = 0  # in bf16 elements
-  for k0 in range(0, Kpad // 16, steps):
-    ks = min(steps, Kpad // 16 - k0)
-    for n in range(Npad):
+  for n0, nb, k0, ks in _blocks(Npad, Kpad, stage):
+    for n in range(nb):
       for kk in range(ks * 16):
-        byte = (kk // 8) * (Npad * 16) + (n // 8) * 128 + (n % 8) * 16 + (kk % 8) * 2
+        byte = (kk // 8) * (nb * 16) + (n // 8) * 128 + (n % 8) * 16 + (kk % 8) * 2
         h = int(img16[off + byte // 2])
-        dense[n, k0 * 16 + kk] = np.array([h << 16], dtype=np.uint32).view(np.float32)[0]
-    off += Npad * 16 * ks
+        dense[n0 + n, k0 * 16 + kk] = np.array([h << 16], dtype=np.uint32).view(np.float32)[0]
+    off += nb * 16 * ks
   assert off == img16.size
   return dense
 
@@ -61,8 +70,7 @@ def test_weight_image_layout_and_bias_fold(N, Npad, Kw, Kpad, stage):
   colmap[hi_col], colmap[lo_col] = -2, -3
   scale = 1.4426950408889634
   img, nch = _pack(W, b, Npad, colmap, scale, stage)
-  steps = min(stage // (Npad * 32), 8)
-  assert nch == -(-(Kpad // 16) // steps)
+  assert nch == len(_blocks(Npad, Kpad, stage))
   dense = _unpack(img, Npad, Kpad, stage)
   # weights: bf16(W * scale) in the mapped columns, zero elsewhere / in padded rows
   for k in range(Kpad):
@@ -118,5 +126,5 @@ def test_tile_image_offsets():
     for t in range(3):
       blk = offs[128 * t:128 * (t + 1)]
       assert blk.min() == t * KG * 2048 and blk.max() == (t + 1) * KG * 2048 - 16
-    # element (r, k): k-group stride 2048 inside a tile, as the UMMA descriptor (LBO = 2048, SBO = 128) expects
+    # element (r, k): k-group stride 2048 inside a tile, as the wgmma descriptor (LBO = 2048, SBO = 128) expects
     assert f(5, 3, KG) - f(5, 2, KG) == 2048 and f(13, 0, KG) - f(5, 0, KG) == 128
