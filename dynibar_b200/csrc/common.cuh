@@ -131,6 +131,8 @@ struct dyn_net {
   dyn::ChainImage quad;
   // sub-round pipelined twin kernel (view_twin3.cu)
   dyn::ChainImage twin3;
+  // warpgroup per-view stage (view_wg.cu): full-width weight chunks in consumption order
+  dyn::ChainImage wg;
 };
 
 // ---- device helpers ---------------------------------------------------------

@@ -1,6 +1,7 @@
 // Host-side dispatch of the fused per-(point, view) stage of the two aggregation networks: argument
-// block + choice between the twin-warp kernel (view_twin.cu, default), the quad-schedule kernel
-// (view_quad.cu) and the sub-round pipelined twin kernel (view_twin3.cu), kept for comparison.
+// block + choice between the warpgroup kernel (view_wg.cu, default) and the older schedules of the same work
+// that keep an fp32 accumulator array in memory: the twin-warp kernel (view_twin.cu), the quad-schedule
+// kernel (view_quad.cu) and the sub-round pipelined twin kernel (view_twin3.cu), kept for comparison.
 //
 // Reference semantics: ibrnet/projection.py:103-176, ibrnet/mlp_network.py:236-284
 // (dynamic) and :423-497 (static).
@@ -12,19 +13,20 @@
 
 namespace dyn {
 
-// the twin-warp kernel: the fastest of them on an H100 (bench.py --view-kernel twin | pipe | quad; DESIGN.md §3.2)
-constexpr int kDefaultViewKernel = 0;
+// the warpgroup kernel: accumulators in registers, the fastest on an H100 (bench.py --view-kernel; DESIGN.md §3.2)
+constexpr int kDefaultViewKernel = 4;
 
-// Three schedules of the same per-tile work: 0 = the twin-warp kernel (view_twin.cu: one CTA per SM, one
-// tile), 1 = the quad kernel (view_quad.cu: one CTA per SM alternating between two tiles), 2 = the twin-warp
-// kernel with sub-round pipelined layers (view_twin3.cu; 3 = the same with one barrier arrival per warp).
-// DYN_VIEW_KERNEL=twin|quad|pipe or dyn_debug_set_view_kernel().
+// Schedules of the same per-tile work: 0 = the twin-warp kernel (view_twin.cu: one CTA per SM, one tile),
+// 1 = the quad kernel (view_quad.cu: one CTA per SM alternating between two tiles), 2 = the twin-warp kernel
+// with sub-round pipelined layers (view_twin3.cu; 3 = the same with one barrier arrival per warp), 4 = the
+// warpgroup kernel (view_wg.cu).  DYN_VIEW_KERNEL=twin|quad|pipe or dyn_debug_set_view_kernel(); -1 = default.
 static int g_view_kernel = -1;
-void set_view_kernel(int which) { g_view_kernel = (which >= 0 && which <= 3) ? which : -1; }
+void set_view_kernel(int which) { g_view_kernel = (which >= 0 && which <= 4) ? which : -1; }
 static int view_kernel() {
   if (g_view_kernel < 0) {
     const char* e = getenv("DYN_VIEW_KERNEL");
-    g_view_kernel = e == nullptr ? kDefaultViewKernel : (e[0] == 'q' ? 1 : (e[0] == 'p' ? 2 : (e[0] == 'e' ? 3 : 0)));
+    const char c = e == nullptr ? 0 : e[0];
+    g_view_kernel = c == 't' ? 0 : (c == 'q' ? 1 : (c == 'p' ? 2 : (c == 'e' ? 3 : kDefaultViewKernel)));
   }
   return g_view_kernel;
 }
@@ -69,6 +71,7 @@ int launch_view_fused(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st
     case 1: return launch_view_quad(n, a, V, st);
     case 2: return launch_view_twin3(n, a, V, st, false);
     case 3: return launch_view_twin3(n, a, V, st, true);  // + one barrier arrival per warp ("elected")
+    case 4: return launch_view_wg(n, a, V, st);
     default: return launch_view_twin(n, a, V, st);
   }
 }

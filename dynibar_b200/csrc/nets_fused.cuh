@@ -155,6 +155,11 @@ size_t view_quad_bytes(int kind);
 int view_quad_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_view_quad(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);
 
+// warpgroup per-view stage (view_wg.cu, the default): accumulators in registers, two 64-row warpgroups per CTA
+size_t view_wg_bytes(int kind);
+int view_wg_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
+int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);
+
 void set_view_kernel(int which);
 int producer_lanes();  // DYN_PRODUCERS (default 1)
 int launch_view_fused(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);

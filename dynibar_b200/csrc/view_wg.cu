@@ -1,0 +1,780 @@
+// Fused per-(point, view) stage of the two aggregation networks, built for Hopper (reference:
+// ibrnet/projection.py:103-176, ibrnet/mlp_network.py:236-284 (dynamic) / :423-497 (static)).
+// Same work and outputs as view_twin.cu, per 64-row half-tile:
+//
+//   projection + masks + view-angle difference, bilinear gather of source RGB + features
+//   [static]  positional encodings -> ray_dir_fc (SS wgmma, N = 256) -> ray_dir_fc.2 (RS, N = 48)
+//   pooling weights, weighted mean/var over views -> base_fc.0 (SS, N = 256)
+//   base_fc.2 -> vis_fc.0 -> vis_fc.2 -> vis_fc2.0 (RS, N = 128), visibility logits, second pooling -> G
+//
+// One persistent CTA per SM: two consumer warpgroups and one producer warp.  Each consumer warpgroup owns
+// 64 rows (view slots) of the CTA's 128-row iteration and issues its own wgmmas, one instruction per k-step
+// for the whole layer width.  The accumulators stay in registers: the warps that issue a layer run its
+// epilogue on the fragments, and a hidden layer's output, packed to bf16 pairs, is the register A operand of
+// the next layer (tc::acc_to_afrag), so only the two front-end operands (positional encodings, pooled
+// features) go through shared memory.  While one warpgroup runs an epilogue, the other's wgmmas keep the
+// tensor cores busy.  Both warpgroups consume the same weight chunks from one ring; a slot is refilled only
+// when both have retired it, so the weights are fetched once per 128 rows.
+//
+// Fragment layout (warp w of the warpgroup, lane l, q = l % 4): accumulator i holds row 16 w + l / 4 + 8 h,
+// column 8 j + 2 q + e with j = i / 4, h = (i / 2) % 2, e = i % 2.  A row's dot products are quad shuffles
+// (xor 1, 2); a point's view slots are 8 or 16 aligned rows of one warp's 16-row slab, so sums over its views
+// are shuffles over the row lanes (xor 4, 8, 16) plus, for 16 slots, the in-thread h pair.
+// The front end (projection, gather, first pooling of the gathered channels) runs with two threads per row,
+// as in view_twin.cu: warps 0-1 of a warpgroup ("twin 0") and 2-3 ("twin 1") each take half of the channels.
+#include "fused_engine.cuh"
+#include "geometry.cuh"
+#include "nets.cuh"
+
+namespace dyn {
+
+using namespace tc;
+using namespace fe;
+
+namespace {
+
+constexpr int kWgRing = 8;
+constexpr int kWgStage = 16384;
+// two consumer warpgroups + a producer warpgroup (one thread streams the weights); setmaxnreg moves the
+// producer's registers to the consumers: 2 x 128 x 232 + 128 x 40 <= 64 K
+constexpr int kWgThreads = 3 * 128;
+constexpr int kConsumerRegs = 232, kProducerRegs = 40;
+constexpr int kWgMaxChunks = 32;
+// per warpgroup: positional-encoding operand (112 columns) | pooled operand of base_fc.0 (240 columns), 64 rows
+constexpr int kPeBytes = 14 * 1024, kPoolBytes = 30 * 1024, kWgATile = kPeBytes + kPoolBytes;
+// constants (floats): biases in true units; W6V = row 128 of vis_fc.2 (visibility logit), W8 = vis_fc2.2;
+// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; W1 / MK = per-row pooling weight and mask of each warpgroup
+constexpr int C_B1 = 0, C_B2 = 256, C_B3 = 304, C_B4 = 560, C_B5 = 688, C_B6 = 816, C_W6V = 944, C_B7 = 1072,
+              C_W8 = 1200, C_MISC = 1328, C_DFEAT = 1332, C_CAMS = 1372, C_W1 = 1628, C_MK = 1756;
+constexpr int kWgConst = 1884;
+constexpr int kWgSmem = kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 4 /* align */ + 16 * 8;
+static_assert(kWgSmem + kWgMaxChunks * 16 <= 227 * 1024, "shared memory of one CTA");
+
+// k-steps per weight chunk of a layer N wide (one ring stage; at most 8, as fe::append_block cuts them)
+__host__ __device__ constexpr int wg_chunk_ksteps(int N) { return kWgStage / (N * 32) < 8 ? kWgStage / (N * 32) : 8; }
+
+// 11 values of one PE component: [x, cos(2^k x) k=0..4, sin(2^k x) k=0..4]
+__device__ __forceinline__ void pe_comp(float x, float* o) {
+  float s, c;
+  __sincosf(x, &s, &c);
+  o[0] = x;
+#pragma unroll
+  for (int k = 0; k < 5; ++k) {
+    o[1 + k] = c;
+    o[6 + k] = s;
+    const float s2 = 2.f * s * c, c2 = 1.f - 2.f * s * s;
+    s = s2; c = c2;
+  }
+}
+
+// 8 consecutive columns [c0, c0 + 8) of a row of a 64-row operand tile -> one 16-byte store
+__device__ __forceinline__ void store8_64(uint8_t* arow, int c0, const float* v) {
+  *reinterpret_cast<uint4*>(arow + (c0 >> 3) * 1024) =
+      make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+}
+// columns (col, col + 1) of row r of a 64-row operand tile (col even)
+__device__ __forceinline__ void store2_64(uint8_t* tile, int r, int col, float x, float y) {
+  *reinterpret_cast<uint32_t*>(tile + (col >> 3) * 1024 + (r >> 3) * 128 + (r & 7) * 16 + (col & 7) * 2) =
+      pack_bf16x2(x, y);
+}
+
+// The weight ring as one consumer warpgroup sees it: chunk `cnt` sits in slot cnt % kWgRing.
+struct Ring {
+  uint8_t* base;
+  uint32_t bar0;  // [0, kWgRing) full, [kWgRing, 2 kWgRing) empty
+  uint32_t cnt;
+  bool prof;
+  long long wait_cycles;  // profiling: cycles spent waiting for weights
+  __device__ __forceinline__ uint32_t wait_full(uint32_t c) {
+    const uint32_t st = c % kWgRing;
+    const long long t0 = prof ? clock64() : 0;
+    mbar_wait(bar0 + 8u * st, (c / kWgRing) & 1);
+    if (prof) wait_cycles += clock64() - t0;
+    return smem_u32(base + st * kWgStage);
+  }
+  // this warp's wgmmas that read chunk c have retired (the empty barrier counts 4 warps x 2 warpgroups)
+  __device__ __forceinline__ void release(uint32_t c) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (kWgRing + c % kWgRing));
+  }
+};
+
+// Issues one layer, D[64 x N] = A[64 x 16 KS] W^T, chunk by chunk as the weights arrive; each chunk's slot is
+// released as soon as the next chunk's wgmmas are committed and its own have retired.  The last chunk stays in
+// flight: layer_finish waits for it.  mma(acc, kstep, b_desc, scale_d) issues one k-step.
+template <int N, int KS, class Mma>
+__device__ __forceinline__ void layer_issue(float* acc, Ring& rg, Mma mma) {
+  constexpr int KC = wg_chunk_ksteps(N), NCH = (KS + KC - 1) / KC;
+  fence_regs<N / 2>(acc);
+  wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    const uint32_t w = rg.wait_full(rg.cnt + c);
+#pragma unroll
+    for (int s = 0; s < KC; ++s)
+      if (c * KC + s < KS) mma(acc, c * KC + s, smem_desc(w + s * N * 32u, N * 16u, 128u), (c | s) ? 1u : 0u);
+    wgmma_commit();
+    if (c > 0) {
+      wgmma_wait<1>();
+      rg.release(rg.cnt + c - 1);
+    }
+  }
+  rg.cnt += NCH;
+}
+template <int N>
+__device__ __forceinline__ void layer_finish(float* acc, Ring& rg) {
+  wgmma_wait<0>();
+  fence_regs<N / 2>(acc);
+  rg.release(rg.cnt - 1);
+}
+
+template <int N, int KS>
+__device__ __forceinline__ void layer_ss(float* acc, uint32_t a_tile, Ring& rg) {
+  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
+    Wgmma<N, 0, 0>::mma(d, smem_desc(a_tile + ks * 2048u, 1024u, 128u), bd, sc);
+  });
+}
+template <int N, int KS>
+__device__ __forceinline__ void layer_rs(float* acc, const uint32_t (&af)[KS][4], Ring& rg) {
+  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) { WgmmaRS<N>::mma(d, af[ks], bd, sc); });
+  layer_finish<N>(acc, rg);
+}
+
+// ELU(acc + bias[column]) in place, N columns of fragment layout (q = lane % 4)
+template <int N>
+__device__ __forceinline__ void bias_elu(float* acc, const float* bias, int q) {
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      acc[4 * j + 2 * h] = elu_fast(acc[4 * j + 2 * h] + b.x);
+      acc[4 * j + 2 * h + 1] = elu_fast(acc[4 * j + 2 * h + 1] + b.y);
+    }
+  }
+}
+template <int KS>
+__device__ __forceinline__ void to_afrag(const float* acc, uint32_t (&af)[KS][4]) {
+#pragma unroll
+  for (int s = 0; s < KS; ++s) acc_to_afrag(acc, s, af[s]);
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// sum over the row lanes of a fragment (8 rows of one h)
+__device__ __forceinline__ float rows8_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  return v + __shfl_xor_sync(0xffffffffu, v, 16);
+}
+// sum over a point's view slots of per-row values v[h] (VP = 8: the point of row half h; VP = 16: both halves)
+template <int VP>
+__device__ __forceinline__ void views_sum(const float* v, float* s) {
+  if (VP == 16) {
+    s[0] = s[1] = rows8_sum(v[0] + v[1]);
+  } else {
+    s[0] = rows8_sum(v[0]);
+    s[1] = rows8_sum(v[1]);
+  }
+}
+
+template <int VP, bool ST>
+__global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_constant__ ViewFusedArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* ring = smem;
+  uint8_t* atiles = smem + kWgRing * kWgStage;
+  float* cst = reinterpret_cast<float*>(atiles + 2 * kWgATile);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 7) & ~7));
+  __shared__ __align__(16) FusedChunk s_tab[kWgMaxChunks];
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);  // warpgroup index, uniform to the compiler
+  const uint32_t bar0 = smem_u32(bars);
+  stage_chunks(s_tab, a.chunks, a.nchunks);
+  if (tid == 0) {
+    for (int i = 0; i < kWgRing; ++i) {
+      mbar_init(bar0 + 8u * i, 1);
+      mbar_init(bar0 + 8u * (kWgRing + i), 8);
+    }
+    mbar_fence_init();
+  }
+  {
+    const float* prm = a.params;
+    for (int i = tid; i < 256; i += blockDim.x) {
+      const int vv = i >> 4, j = i & 15;
+      cst[C_CAMS + i] = j < 12 ? a.cams.P[vv][j] : (j < 15 ? a.cams.center[vv][j - 12] : 0.f);
+      cst[C_B1 + i] = ST ? prm[a.o_b1 + i] : 0.f;
+      cst[C_B3 + i] = prm[a.o_b3 + i];
+    }
+    for (int i = tid; i < 128; i += blockDim.x) {
+      cst[C_B4 + i] = prm[a.o_b4 + i];
+      cst[C_B5 + i] = prm[a.o_b5 + i];
+      cst[C_B6 + i] = prm[a.o_b6 + i];
+      cst[C_W6V + i] = prm[a.o_w6 + 128 * 128 + i];
+      cst[C_B7 + i] = prm[a.o_b7 + i];
+      cst[C_W8 + i] = prm[a.o_w8 + i];
+    }
+    if (tid < 48) cst[C_B2 + tid] = (ST && tid < kF) ? prm[a.o_b2 + tid] : 0.f;
+    if (tid < 40) cst[C_DFEAT + tid] = (!ST && tid < kF) ? a.dfeat[tid] : 0.f;
+    if (tid == 0) {
+      cst[C_MISC + 0] = prm[a.o_b6 + 128];
+      cst[C_MISC + 1] = prm[a.o_b8];
+      cst[C_MISC + 2] = (ST && a.o_s >= 0) ? fabsf(prm[a.o_s]) : 0.f;
+    }
+  }
+  __syncthreads();
+
+  const long long n_rows = a.P * VP;
+  const int n_iter = (int)((n_rows + 127) / 128);
+  if (wg == 2) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (tid == 256) producer_loop<false, kWgRing, kWgStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
+    return;
+  }
+  setmaxnreg_inc<kConsumerRegs>();
+
+  const int t = tid & 127, ww = t >> 5, q = lane & 3;
+  uint8_t* pe_tile = atiles + wg * kWgATile;
+  uint8_t* pool_tile = pe_tile + kPeBytes;
+  const uint32_t pe_addr = smem_u32(pe_tile), pool_addr = smem_u32(pool_tile);
+  float* s_w1 = cst + C_W1 + 64 * wg;
+  float* s_mk = cst + C_MK + 64 * wg;
+  // row layout (front end): twin tw of row r
+  const int tw = t >> 6, r = t & 63, v = r & (VP - 1);
+  uint8_t* arow_pe = pe_tile + (r >> 3) * 128 + (r & 7) * 16;
+  uint8_t* arow_pool = pool_tile + (r >> 3) * 128 + (r & 7) * 16;
+  // fragment layout: rows fr[h] of the half-tile
+  const int fr[2] = {16 * ww + (lane >> 2), 16 * ww + (lane >> 2) + 8};
+
+  const bool prof = a.dbg != nullptr && blockIdx.x == 0 && t == 0;
+  Ring rg{ring, bar0, 0u, prof, 0};
+  int dbg_n = 0;
+  const long long t_begin = prof ? clock64() : 0;
+#define TS()                                                          \
+  do {                                                                \
+    if (prof && dbg_n < 64) a.dbg[wg * 64 + dbg_n++] = clock64();     \
+  } while (0)
+
+  const float wh = a.w_img, hh = a.h_img;
+  const bool want_rgb = (tw == 0) || (ST && a.mask_rgb);
+
+  for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
+    const long long row0 = (long long)it * 128 + 64 * wg;  // first row of this warpgroup
+    // ---- front end, row layout ----
+    const long long pl = (row0 + r) / VP;
+    const bool pt_ok = pl < a.P;
+    const bool valid = pt_ok && v < a.V;
+    const long long m = pl * a.V + v;
+    float p3[3] = {0.f, 0.f, 0.f};
+    if (pt_ok) { p3[0] = a.pts[pl * 3]; p3[1] = a.pts[pl * 3 + 1]; p3[2] = a.pts[pl * 3 + 2]; }
+    float q3[3] = {p3[0], p3[1], p3[2]};
+    if (!ST && valid) {
+      const float* qq = a.pts_seq + ((long long)v * a.seq_stride + pl) * 3;
+      q3[0] = qq[0]; q3[1] = qq[1]; q3[2] = qq[2];
+    }
+    // the previous iteration's wgmmas of every warp have retired before the operand tiles are rewritten
+    named_bar_sync(1 + wg, 128);
+    TS();  // 0: iteration start
+
+    const int vc = valid ? v : 0;
+    const float* cam = cst + C_CAMS + 16 * vc;
+    float pu, pv;
+    bool front;
+    project_point(cam, q3[0], q3[1], q3[2], pu, pv, front);
+    const bool inb = (pu <= wh - 1.f) && (pu >= 0.f) && (pv <= hh - 1.f) && (pv >= 0.f);
+    const float mask_proj = (valid && inb && front) ? 1.f : 0.f;
+
+    // ---- gather: this twin's 16 bf16 feature channels (+ RGB) at the 4 bilinear taps ----
+    float chv[24];
+#pragma unroll
+    for (int i = 0; i < 24; ++i) chv[i] = 0.f;
+    float rgb[3] = {0.f, 0.f, 0.f};
+    {
+      const float gx = 2.f * pu / (wh - 1.f) - 1.f, gy = 2.f * pv / (hh - 1.f) - 1.f;
+      uint4 tf[8];
+      float4 tr[4];
+      float tw4[4], twr[4];
+      {
+        const float fx = (gx + 1.f) * 0.5f * (float)(a.w - 1), fy = (gy + 1.f) * 0.5f * (float)(a.h - 1);
+        const float x0f = floorf(fx), y0f = floorf(fy);
+        const int x0 = (int)x0f, y0 = (int)y0f;
+        const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
+        const uint16_t* base = a.feat_bf + (long long)vc * a.h * a.w * kC + 16 * tw;
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+          for (int dx = 0; dx < 2; ++dx) {
+            // out-of-range taps (and padding rows) load a clamped texel with weight 0
+            const int xi = x0 + dx, yi = y0 + dy;
+            const bool in = valid && xi >= 0 && xi < a.w && yi >= 0 && yi < a.h;
+            tw4[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
+            const int xc = min(max(xi, 0), a.w - 1), yc = min(max(yi, 0), a.h - 1);
+            const uint4* tp = reinterpret_cast<const uint4*>(base + ((long long)yc * a.w + xc) * kC);
+            tf[2 * (2 * dy + dx)] = __ldg(tp);
+            tf[2 * (2 * dy + dx) + 1] = __ldg(tp + 1);
+          }
+      }
+      if (want_rgb) {
+        const float fx = (gx + 1.f) * 0.5f * (float)(a.W - 1), fy = (gy + 1.f) * 0.5f * (float)(a.H - 1);
+        const float x0f = floorf(fx), y0f = floorf(fy);
+        const int x0 = (int)x0f, y0 = (int)y0f;
+        const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
+        const float* base = a.rgba + (long long)vc * a.H * a.W * 4;
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+          for (int dx = 0; dx < 2; ++dx) {
+            const int xi = x0 + dx, yi = y0 + dy;
+            const bool in = valid && xi >= 0 && xi < a.W && yi >= 0 && yi < a.H;
+            twr[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
+            const int xc = min(max(xi, 0), a.W - 1), yc = min(max(yi, 0), a.H - 1);
+            tr[2 * dy + dx] = __ldg(reinterpret_cast<const float4*>(base + ((long long)yc * a.W + xc) * 4));
+          }
+      }
+#pragma unroll
+      for (int tp = 0; tp < 4; ++tp) {
+#pragma unroll
+        for (int hlf = 0; hlf < 2; ++hlf) {
+          const uint4 qv = tf[2 * tp + hlf];
+          const uint32_t u[4] = {qv.x, qv.y, qv.z, qv.w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float lo = __uint_as_float(u[j] << 16), hi = __uint_as_float(u[j] & 0xffff0000u);
+            if (tw == 0) {
+              chv[3 + 8 * hlf + 2 * j] += lo * tw4[tp];  // twin 0 keeps rgb in slots 0..2
+              chv[3 + 8 * hlf + 2 * j + 1] += hi * tw4[tp];
+            } else {
+              chv[8 * hlf + 2 * j] += lo * tw4[tp]; chv[8 * hlf + 2 * j + 1] += hi * tw4[tp];
+            }
+          }
+        }
+      }
+      if (want_rgb) {
+#pragma unroll
+        for (int tp = 0; tp < 4; ++tp) {
+          rgb[0] += tr[tp].x * twr[tp]; rgb[1] += tr[tp].y * twr[tp]; rgb[2] += tr[tp].z * twr[tp];
+        }
+      }
+    }
+
+    float rd[4];
+    {
+      float a0 = a.cams.tgt[0] - p3[0], a1 = a.cams.tgt[1] - p3[1], a2 = a.cams.tgt[2] - p3[2];
+      normalize3(a0, a1, a2);
+      float b0 = cam[12] - q3[0], b1 = cam[13] - q3[1], b2 = cam[14] - q3[2];
+      normalize3(b0, b1, b2);
+      rd[0] = a0 - b0; rd[1] = a1 - b1; rd[2] = a2 - b2;
+      rd[3] = a0 * b0 + a1 * b1 + a2 * b2;
+      normalize3(rd[0], rd[1], rd[2]);
+    }
+
+    float mask = mask_proj;
+    if (ST && a.mask_rgb) mask *= ((rgb[0] + rgb[1] + rgb[2]) > 1e-3f) ? 1.f : 0.f;
+    if (tw == 0) {
+      chv[0] = rgb[0]; chv[1] = rgb[1]; chv[2] = rgb[2];
+      if (valid) {
+        a.mask_proj[m] = mask_proj;
+        if (ST) {
+          a.mask_eff[m] = mask;
+          reinterpret_cast<float4*>(a.ray_diff)[m] = make_float4(rd[0], rd[1], rd[2], rd[3]);
+          a.rgb_in[m * 3] = rgb[0]; a.rgb_in[m * 3 + 1] = rgb[1]; a.rgb_in[m * 3 + 2] = rgb[2];
+        }
+      }
+    }
+    if (!ST) {  // dynamic: + time feature on this twin's channels (mlp_network.py:244-247)
+      const int c0 = tw == 0 ? 0 : 19, nc = tw == 0 ? 19 : 16;
+#pragma unroll
+      for (int i = 0; i < 19; ++i)
+        if (i < nc) chv[i] = valid ? chv[i] + cst[C_DFEAT + c0 + i] : 0.f;
+    }
+
+    // ---- pooling weights (both twins) ----
+    float w1;
+    if (ST && a.anti_alias) {
+      const float e = ex2f(cst[C_MISC + 2] * (rd[3] - 1.f) * 1.4426950408889634f);
+      const float emin = group_min<VP>(valid ? e : INFINITY);
+      w1 = valid ? (e - emin) * mask : 0.f;
+    } else {
+      w1 = mask;
+    }
+    w1 = w1 / (group_sum<VP>(w1) + 1e-8f);
+    if (tw == 0) { s_w1[r] = w1; s_mk[r] = mask; }
+
+    // ---- first pooling of the gathered channels (row layout): per twin groups of
+    //      [mean8 | var8 | feat8], twin 0 at columns 0..71 (3 groups), twin 1 at 72..119 (2 groups) ----
+#pragma unroll
+    for (int g = 0; g < 3; ++g) {
+      if (tw == 1 && g == 2) break;
+      float o[24];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float fv = chv[8 * g + j];
+        const float s1 = group_sum<VP>(w1 * fv);
+        const float d = fv - s1;
+        const float s2 = group_sum<VP>(w1 * d * d);
+        o[j] = s1; o[8 + j] = s2; o[16 + j] = fv;
+      }
+      const int cb = 72 * tw + 24 * g;
+      store8_64(arow_pool, cb, o);
+      store8_64(arow_pool, cb + 8, o + 8);
+      store8_64(arow_pool, cb + 16, o + 16);
+    }
+    if (!ST && tw == 1) {  // dynamic: K padding 120..127
+      const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      store8_64(arow_pool, 120, z);
+    }
+
+    float acc[128];  // accumulators of the 256-wide layers (the first 64 / 24 for the narrower ones)
+    if (ST) {
+      // ---- ray_dir_fc.0 operand: component-major PE, 56 columns per twin (layout in view_wg_build) ----
+      float pl6[6];
+      {
+        const float ox = cam[12], oy = cam[13], oz = cam[14];
+        float dx = p3[0] - ox, dy = p3[1] - oy, dz = p3[2] - oz;
+        normalize3(dx, dy, dz);
+        pl6[0] = dx; pl6[1] = dy; pl6[2] = dz;
+        pl6[3] = oy * dz - oz * dy;
+        pl6[4] = oz * dx - ox * dz;
+        pl6[5] = ox * dy - oy * dx;
+      }
+      // each 8-column group is stored as soon as it is complete (short live ranges)
+      float xin[56];
+      if (tw == 0) {
+        pe_comp(p3[0], xin);         store8_64(arow_pe, 0, xin);
+        pe_comp(p3[1], xin + 11);    store8_64(arow_pe, 8, xin + 8);
+        pe_comp(p3[2], xin + 22);    store8_64(arow_pe, 16, xin + 16); store8_64(arow_pe, 24, xin + 24);
+        pe_comp(pl6[0], xin + 33);   store8_64(arow_pe, 32, xin + 32);
+        pe_comp(pl6[1], xin + 44);   xin[55] = 0.f;
+        store8_64(arow_pe, 40, xin + 40);  store8_64(arow_pe, 48, xin + 48);
+      } else {
+        pe_comp(pl6[2], xin);        store8_64(arow_pe, 56, xin);
+        pe_comp(pl6[3], xin + 11);   store8_64(arow_pe, 64, xin + 8);
+        pe_comp(pl6[4], xin + 22);   store8_64(arow_pe, 72, xin + 16); store8_64(arow_pe, 80, xin + 24);
+        pe_comp(pl6[5], xin + 33);   store8_64(arow_pe, 88, xin + 32);
+        xin[44] = rd[0]; xin[45] = rd[1]; xin[46] = rd[2]; xin[47] = rd[3];
+#pragma unroll
+        for (int i = 48; i < 56; ++i) xin[i] = 0.f;
+        store8_64(arow_pe, 96, xin + 40);  store8_64(arow_pe, 104, xin + 48);
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);
+      TS();  // 1: F1 issue
+      layer_ss<256, 7>(acc, pe_addr, rg);
+      layer_finish<256>(acc, rg);
+      TS();  // 2: F1 done
+      // ---- F1 epilogue -> ray_dir_fc.2 (register A) ----
+      {
+        uint32_t af[16][4];
+        bias_elu<256>(acc, cst + C_B1, q);
+        to_afrag<16>(acc, af);
+        layer_rs<48, 16>(acc, af, rg);
+      }
+      TS();  // 3: F2 done
+      // ---- src_feat * ref_feat (35 channels, fragment columns j < 5) and their pooling over views:
+      //      mean at column 120 + n, var at 160 + n, feat at 200 + n ----
+      float f[2][10], w1h[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long prow = (row0 + fr[h]) / VP;
+        const bool ok = prow < a.P && ((fr[h] & (VP - 1)) < a.V);
+        const float* rf = a.ref_feat + (ok ? prow / a.S : 0) * kF;
+        w1h[h] = s_w1[fr[h]];
+#pragma unroll
+        for (int j = 0; j < 5; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = 8 * j + 2 * q + e;
+            f[h][2 * j + e] = (ok && n < kF) ? (acc[4 * j + 2 * h + e] + cst[C_B2 + n]) * __ldg(rf + n) : 0.f;
+          }
+      }
+#pragma unroll
+      for (int j = 0; j < 5; ++j) {
+        float mu[2][2], va[2][2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int i = 2 * j + e;
+          float tv[2] = {w1h[0] * f[0][i], w1h[1] * f[1][i]}, s1[2], s2[2];
+          views_sum<VP>(tv, s1);
+          const float d0 = f[0][i] - s1[0], d1 = f[1][i] - s1[1];
+          tv[0] = w1h[0] * d0 * d0;
+          tv[1] = w1h[1] * d1 * d1;
+          views_sum<VP>(tv, s2);
+          mu[0][e] = s1[0]; mu[1][e] = s1[1]; va[0][e] = s2[0]; va[1][e] = s2[1];
+        }
+        const int n = 8 * j + 2 * q;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          store2_64(pool_tile, fr[h], 120 + n, mu[h][0], mu[h][1]);
+          store2_64(pool_tile, fr[h], 160 + n, va[h][0], va[h][1]);
+          store2_64(pool_tile, fr[h], 200 + n, f[h][2 * j], f[h][2 * j + 1]);
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1 + wg, 128);
+    TS();  // 4: F3 issue
+    layer_ss<256, ST ? 15 : 8>(acc, pool_addr, rg);
+    layer_finish<256>(acc, rg);
+    TS();  // 5: F3 done
+    // ---- base_fc.0 epilogue -> base_fc.2 (register A) ----
+    {
+      uint32_t af[16][4];
+      bias_elu<256>(acc, cst + C_B3, q);
+      to_afrag<16>(acc, af);
+      layer_rs<128, 16>(acc, af, rg);
+    }
+    TS();  // 6: F4 done
+    // ---- x = ELU(base_fc.2) (fp32 residual); vis_fc.0 on bf16(x): its row scale w1 applies to the accumulator ----
+    float x[64];
+    bias_elu<128>(acc, cst + C_B4, q);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) x[i] = acc[i];
+    {
+      uint32_t af[8][4];
+      to_afrag<8>(x, af);
+      layer_rs<128, 8>(acc, af, rg);
+    }
+    TS();  // 7: F5 done
+    // ---- h = ELU(w1 (W x) + b) and the row's visibility logit (quad sum) -> vis_fc.2 ----
+    const float w1r[2] = {s_w1[fr[0]], s_w1[fr[1]]}, mk[2] = {s_mk[fr[0]], s_mk[fr[1]]};
+    float part[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float2 b = *reinterpret_cast<const float2*>(cst + C_B5 + 8 * j + 2 * q);
+      const float2 wv = *reinterpret_cast<const float2*>(cst + C_W6V + 8 * j + 2 * q);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float& h0 = acc[4 * j + 2 * h];
+        float& h1 = acc[4 * j + 2 * h + 1];
+        h0 = elu_fast(fmaf(h0, w1r[h], b.x));
+        h1 = elu_fast(fmaf(h1, w1r[h], b.y));
+        part[h] = fmaf(h1, wv.y, fmaf(h0, wv.x, part[h]));
+      }
+    }
+    part[0] = quad_sum(part[0]);
+    part[1] = quad_sum(part[1]);
+    {
+      uint32_t af[8][4];
+      to_afrag<8>(acc, af);
+      layer_rs<128, 8>(acc, af, rg);
+    }
+    TS();  // 8: F6 done
+    // ---- x += ELU(vis_fc.2); bf16(x) is vis_fc2.0's operand (vis1 applies to its accumulator) and, for the
+    //      static net, the blending head's input (X tile image, rows = view slots) ----
+    float vis1[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) vis1[h] = sigmoid_fast(elu_fast(cst[C_MISC + 0] + part[h])) * mk[h];
+    bias_elu<128>(acc, cst + C_B6, q);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) x[i] += acc[i];
+    {
+      uint32_t af[8][4];
+      to_afrag<8>(x, af);
+      if (ST) {
+        uint8_t* xo = reinterpret_cast<uint8_t*>(a.X);
+#pragma unroll
+        for (int s = 0; s < 8; ++s)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)  // af[s][k]: row fr[k & 1], 8-column group 2 s + (k >> 1)
+            *reinterpret_cast<uint32_t*>(xo + tile_image_off(row0 + fr[k & 1], 2 * s + (k >> 1), 16) + 4 * q) = af[s][k];
+      }
+      layer_rs<128, 8>(acc, af, rg);
+    }
+    TS();  // 9: F7 done
+    // ---- vis2 = sigmoid(vis_fc2.2 . ELU(vis1 (W x) + b)) * mask ----
+    float p7[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float2 b = *reinterpret_cast<const float2*>(cst + C_B7 + 8 * j + 2 * q);
+      const float2 wv = *reinterpret_cast<const float2*>(cst + C_W8 + 8 * j + 2 * q);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        p7[h] = fmaf(elu_fast(fmaf(acc[4 * j + 2 * h], vis1[h], b.x)), wv.x, p7[h]);
+        p7[h] = fmaf(elu_fast(fmaf(acc[4 * j + 2 * h + 1], vis1[h], b.y)), wv.y, p7[h]);
+      }
+    }
+    float vis2[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      vis2[h] = sigmoid_fast(cst[C_MISC + 1] + quad_sum(p7[h])) * mk[h];
+      const long long prow = (row0 + fr[h]) / VP;
+      const int vh = fr[h] & (VP - 1);
+      if (ST && q == 0 && prow < a.P && vh < a.V) a.vis2[prow * a.V + vh] = vis2[h];
+    }
+
+    // ---- second pooling: mean / second moment of x over the point's views, reduce-scattered over the row lanes:
+    //      afterwards lane l holds columns 8 j0 + 2 q + {0, 1} and 8 (j0 + 1) + 2 q + {0, 1} ----
+    float vsum[2], w2[2], Wsum[2], nval[2];
+    views_sum<VP>(vis2, vsum);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) w2[h] = vis2[h] / (vsum[h] + 1e-8f);
+    views_sum<VP>(w2, Wsum);
+    views_sum<VP>(mk, nval);
+    const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
+    const int j0 = (b4 ? 8 : 0) + (b3 ? 4 : 0) + (b2 ? 2 : 0);
+    uint8_t* gi = reinterpret_cast<uint8_t*>(a.G);
+#pragma unroll
+    for (int pi = 0; pi < (VP == 8 ? 2 : 1); ++pi) {
+      float st4[2][4];
+#pragma unroll
+      for (int qq = 0; qq < 2; ++qq) {
+        float s32[32], s16[16], s8[8];
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float x0 = x[4 * j + e], x1 = x[4 * j + 2 + e];
+            if (VP == 16)
+              s32[2 * j + e] = qq ? w2[0] * x0 * x0 + w2[1] * x1 * x1 : w2[0] * x0 + w2[1] * x1;
+            else
+              s32[2 * j + e] = pi ? (qq ? w2[1] * x1 * x1 : w2[1] * x1) : (qq ? w2[0] * x0 * x0 : w2[0] * x0);
+          }
+        rs_step<32>(s32, s16, b4, 16);
+        rs_step<16>(s16, s8, b3, 8);
+        rs_step<8>(s8, st4[qq], b2, 4);
+      }
+      const long long prow = (row0 + 16 * ww + 8 * pi) / VP;
+      if (prow < a.P) {
+        const float W = Wsum[pi];
+        float mu4[4], vr4[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          mu4[i] = st4[0][i];
+          vr4[i] = st4[1][i] - mu4[i] * mu4[i] * (2.f - W);
+        }
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int c = 8 * (j0 + k) + 2 * q;
+          *reinterpret_cast<uint32_t*>(gi + tile_image_off(prow, c >> 3, 34) + (c & 7) * 2) =
+              pack_bf16x2(mu4[2 * k], mu4[2 * k + 1]);
+          *reinterpret_cast<uint32_t*>(gi + tile_image_off(prow, 16 + (c >> 3), 34) + (c & 7) * 2) =
+              pack_bf16x2(vr4[2 * k], vr4[2 * k + 1]);
+        }
+        if (lane == 0) {
+          *reinterpret_cast<uint4*>(gi + tile_image_off(prow, 32, 34)) = make_uint4(pack_bf16x2(W / (float)a.V, 0.f), 0u, 0u, 0u);
+          *reinterpret_cast<uint4*>(gi + tile_image_off(prow, 33, 34)) = make_uint4(0x3F803F80u, 0u, 0u, 0u);  // 1, 1: bias columns of geometry_fc
+          a.nvalid[prow] = nval[pi];
+        }
+      }
+    }
+    TS();  // 10: outputs done
+  }
+#undef TS
+  if (prof) {
+    a.dbg[128 + wg] = clock64() - t_begin;  // warpgroup lifetime
+    a.dbg[130 + wg] = rg.wait_cycles;                // cycles waiting for weight chunks
+  }
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------
+// host: weight images, full layer width per chunk, in the order the warpgroups consume them
+// ---------------------------------------------------------------------------
+size_t view_wg_bytes(int kind) { (void)kind; return (size_t)(512 * 1024); }
+
+int view_wg_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes, cudaStream_t st) {
+  std::vector<uint8_t> img;
+  std::vector<FusedChunk> tab;
+  auto add = [&](const LinearP& l, int N, int Npad, int Kpad, std::vector<int> map) {
+    HostLayer L;
+    L.W = P + l.w; L.N = N; L.Kw = l.in; L.Npad = Npad; L.Kpad = Kpad; L.colmap = std::move(map);
+    append_block(L, img, tab, 0, 0, 0, 0, kWgStage, 0, Kpad / 16);
+  };
+  // base_fc.0 operand columns 0..119: the gathered channels (rgb + 32 features, + the time feature for the
+  // dynamic net) as [mean8 | var8 | feat8] groups, twin 0 channels 0..18 at 0..71, twin 1 channels 19..34 at
+  // 72..119; the concatenated input has C channels: mean c, var C + c, feat 2 C + c
+  auto gathered_map = [](std::vector<int>& m, int C) {
+    for (int s = 0; s < 19; ++s) {
+      const int b = 24 * (s / 8) + (s % 8);
+      m[b] = s; m[b + 8] = C + s; m[b + 16] = 2 * C + s;
+    }
+    for (int s = 0; s < 16; ++s) {
+      const int c = 19 + s, b = 72 + 24 * (s / 8) + (s % 8);
+      m[b] = c; m[b + 8] = C + c; m[b + 16] = 2 * C + c;
+    }
+  };
+  if (n->kind == DYN_NET_STATIC) {
+    const StaticLayout& L = n->sl;
+    // ray_dir_fc.0: component-major PE; twin 0 = comps 0..4 (+1 pad), twin 1 = comps 5..8, ray_diff, pad
+    std::vector<int> m1(112, -1);
+    auto comp_col = [](int ci, int j) {  // j: 0 = x, 1..5 = cos f_k, 6..10 = sin f_k
+      if (ci < 3) return j == 0 ? ci : (j <= 5 ? 3 + 3 * (j - 1) + ci : 18 + 3 * (j - 6) + ci);
+      const int d = ci - 3;
+      return j == 0 ? 33 + d : (j <= 5 ? 39 + 6 * (j - 1) + d : 69 + 6 * (j - 6) + d);
+    };
+    for (int ci = 0; ci < 5; ++ci)
+      for (int j = 0; j < 11; ++j) m1[11 * ci + j] = comp_col(ci, j);
+    for (int ci = 5; ci < 9; ++ci)
+      for (int j = 0; j < 11; ++j) m1[56 + 11 * (ci - 5) + j] = comp_col(ci, j);
+    for (int i = 0; i < 4; ++i) m1[100 + i] = 99 + i;
+    add(L.ray_dir0, 256, 256, 112, m1);
+    add(L.ray_dir2, kF, 48, 256, identity_map(256, 256));
+    // columns 120..239: the 35 channels src_feat * ref_feat (concat channels 35..69) as mean | var | feat blocks
+    std::vector<int> m3(240, -1);
+    gathered_map(m3, 70);
+    for (int c = 0; c < kF; ++c) {
+      m3[120 + c] = 35 + c; m3[160 + c] = 70 + 35 + c; m3[200 + c] = 140 + 35 + c;
+    }
+    add(L.base0, 256, 256, 240, m3);
+  } else {
+    const DynamicLayout& L = n->dl;
+    std::vector<int> m3(128, -1);
+    gathered_map(m3, kF);
+    add(L.base0, 256, 256, 128, m3);
+  }
+  const LinearP& base2 = n->kind == DYN_NET_STATIC ? n->sl.base2 : n->dl.base2;
+  const LinearP& vis0 = n->kind == DYN_NET_STATIC ? n->sl.vis0 : n->dl.vis0;
+  const LinearP& vis2 = n->kind == DYN_NET_STATIC ? n->sl.vis2 : n->dl.vis2;
+  const LinearP& vis2_0 = n->kind == DYN_NET_STATIC ? n->sl.vis2_0 : n->dl.vis2_0;
+  add(base2, 128, 128, 256, identity_map(256, 256));
+  add(vis0, 128, 128, 128, identity_map(128, 128));
+  add(vis2, 128, 128, 128, identity_map(128, 128));  // rows 0..127 of vis_fc.2; row 128 (the logit) in the epilogue
+  add(vis2_0, 128, 128, 128, identity_map(128, 128));
+  const size_t img_bytes = (img.size() + 255) & ~(size_t)255;
+  const size_t need = img_bytes + tab.size() * sizeof(FusedChunk);
+  if (need > dst_bytes) return fail(DYN_E_INVALID, "per-view images need %zu bytes, have %zu", need, dst_bytes);
+  if (tab.size() > (size_t)kWgMaxChunks) return fail(DYN_E_INVALID, "chunk table too long (%zu)", tab.size());
+  DYN_CUDA(cudaMemcpyAsync(dst_dev, img.data(), img.size(), cudaMemcpyHostToDevice, st));
+  DYN_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(dst_dev) + img_bytes, tab.data(),
+                           tab.size() * sizeof(FusedChunk), cudaMemcpyHostToDevice, st));
+  DYN_CUDA(cudaStreamSynchronize(st));
+  n->wg.img = dst_dev;
+  n->wg.tab = reinterpret_cast<const FusedChunk*>(reinterpret_cast<char*>(dst_dev) + img_bytes);
+  n->wg.nchunks = (int)tab.size();
+  return DYN_OK;
+}
+
+int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
+  if (n->wg.img == nullptr) return fail(DYN_E_INVALID, "net has no per-view weight images");
+  a.wimg = n->wg.img;
+  a.chunks = n->wg.tab;
+  a.nchunks = n->wg.nchunks;
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    DYN_CUDA(cudaGetDevice(&dev));
+    DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+#define PREP_WG(VPV, STV) \
+    DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem))
+    PREP_WG(8, true); PREP_WG(16, true); PREP_WG(8, false); PREP_WG(16, false);
+#undef PREP_WG
+  }
+  const int VP = V <= 8 ? 8 : 16;
+  const long long n_iter = (a.P * VP + 127) / 128;
+  const int grid = (int)(n_iter < sms ? n_iter : sms);
+  if (grid == 0) return DYN_OK;
+  const bool st_net = n->kind == DYN_NET_STATIC;
+  ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
+  if (st_net) {
+    if (VP == 8) view_wg_kernel<8, true><<<grid, kWgThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, true><<<grid, kWgThreads, kWgSmem, st>>>(a);
+  } else {
+    if (VP == 8) view_wg_kernel<8, false><<<grid, kWgThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, false><<<grid, kWgThreads, kWgSmem, st>>>(a);
+  }
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+}  // namespace dyn

@@ -386,14 +386,18 @@ int dyn_debug_pack_layer(const float* W, const float* bias, int N, int Kw, int N
  * 128-row tile: the layout activations use between the fused kernels. */
 size_t dyn_debug_tile_image_off(long long row, int kgroup, int kgroups);
 
-/* comparison hook: which kernel runs the fused per-view stage: 0 = twin-warp kernel (csrc/view_twin.cu: one
- * tile per CTA, the default), 1 = quad-schedule kernel (csrc/view_quad.cu: one CTA per SM alternating between
- * two tiles), 2 = twin-warp kernel with sub-round pipelined layers (csrc/view_twin3.cu).  The environment
- * variable DYN_VIEW_KERNEL=twin|quad|pipe sets the initial value. */
+/* comparison hook: which kernel runs the fused per-view stage: 4 = warpgroup kernel (csrc/view_wg.cu:
+ * accumulators in registers, two 64-row warpgroups per CTA; the default), 0 = twin-warp kernel
+ * (csrc/view_twin.cu: one tile per CTA), 1 = quad-schedule kernel (csrc/view_quad.cu: one CTA per SM
+ * alternating between two tiles), 2 = twin-warp kernel with sub-round pipelined layers (csrc/view_twin3.cu),
+ * 3 = the same with one barrier arrival per warp; -1 = the default.  The environment variable
+ * DYN_VIEW_KERNEL=twin|quad|pipe sets the initial value. */
 void dyn_debug_set_view_kernel(int which);
 
 /* profiling hook: when set, block 0 of the fused static per-view kernel writes clock64()
- * phase timestamps ([2 twins][64]) into dev_buf. */
+ * phase timestamps into dev_buf (zeroed, >= 616 int64): the twin-warp kernels [2 twins][64] and
+ * the MMA warpgroup's totals from index 128; the warpgroup kernel [2 warpgroups][64] at its layer
+ * boundaries, then per warpgroup its lifetime ([128 + wg]) and the cycles it waited for weights ([130 + wg]). */
 void dyn_debug_set_view_timestamps(long long* dev_buf);
 
 /* ---- building block: one nn.Linear on the tensor cores -----------------------
