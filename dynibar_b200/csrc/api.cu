@@ -133,9 +133,9 @@ size_t dyn_net_param_count(int kind) {
 
 size_t dyn_net_packed_bytes(int kind) {
   switch (kind) {
-    case DYN_NET_DYNAMIC: return (size_t)dynamic_layout().all.packed_bytes + view_twin_bytes(kind) + view_quad_bytes(kind) + view_twin3_bytes(kind) + view_wg_bytes(kind) + fused_chain_bytes(kind) + twin_chain_bytes(kind);
-    case DYN_NET_STATIC: return (size_t)static_layout(true).all.packed_bytes + view_twin_bytes(kind) + view_quad_bytes(kind) + view_twin3_bytes(kind) + view_wg_bytes(kind) + fused_chain_bytes(kind) + twin_chain_bytes(kind);
-    case DYN_NET_MOTION: return (size_t)motion_layout(8).all.packed_bytes + fused_chain_bytes(kind);
+    case DYN_NET_DYNAMIC: return (size_t)dynamic_layout().all.packed_bytes + view_twin_bytes(kind) + view_wg_bytes(kind) + twin_chain_bytes(kind);
+    case DYN_NET_STATIC: return (size_t)static_layout(true).all.packed_bytes + view_twin_bytes(kind) + view_wg_bytes(kind) + twin_chain_bytes(kind);
+    case DYN_NET_MOTION: return (size_t)motion_layout(8).all.packed_bytes + motion_fused_bytes();
     default: return 0;
   }
 }
@@ -217,16 +217,12 @@ int dyn_net_create_ex(int kind, const float* params, size_t n_params, void* pack
       if (!rc && kind != DYN_NET_MOTION) {
         rc = view_twin_build(n, hp, cur, view_twin_bytes(kind), (cudaStream_t)stream);
         cur += view_twin_bytes(kind);
-        if (!rc) rc = view_quad_build(n, hp, cur, view_quad_bytes(kind), (cudaStream_t)stream);
-        cur += view_quad_bytes(kind);
-        if (!rc) rc = view_twin3_build(n, hp, cur, view_twin3_bytes(kind), (cudaStream_t)stream);
-        cur += view_twin3_bytes(kind);
         if (!rc) rc = view_wg_build(n, hp, cur, view_wg_bytes(kind), (cudaStream_t)stream);
         cur += view_wg_bytes(kind);
+        if (!rc) rc = twin_chain_build(n, hp, cur, twin_chain_bytes(kind), (cudaStream_t)stream);
+      } else if (!rc) {
+        rc = motion_fused_build(n, hp, cur, motion_fused_bytes(), (cudaStream_t)stream);
       }
-      if (!rc) rc = fused_chain_build(n, hp, cur, fused_chain_bytes(kind), (cudaStream_t)stream);
-      cur += fused_chain_bytes(kind);
-      if (!rc) rc = twin_chain_build(n, hp, cur, twin_chain_bytes(kind), (cudaStream_t)stream);
       free(hp);
       if (rc) { free(n); return rc; }
     }

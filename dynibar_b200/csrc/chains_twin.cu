@@ -1,8 +1,7 @@
 // Row-local fused tensor-core chains in the twin-warp structure of view_twin.cu: CTAs with ONE 128-row tile
 // whose rows are served by TWO threads (warps w and w + 4 read the same accumulator lanes 32 (w & 3) ..
 // + 31 and split every layer's output columns), plus the MMA warpgroup (warps 8-11) and the weight producer
-// (warp 12).  The other versions of these kernels (chains_fused.cu: two tiles per CTA, one thread per row)
-// give each row a single thread; here two threads share the latency-bound epilogues.
+// (warp 12): two threads share each row's latency-bound epilogues.
 //
 //   rgbhead_twin_kernel : static per-view colour-blending head + masked softmax over views
 //                         (mlp_network.py:508-526)
@@ -107,10 +106,9 @@ __global__ void __launch_bounds__(kTwinThreads, 1) rgbhead_twin_kernel(const __g
   const int n_iter = (int)((a.P * VP + 127) / 128);
 
   if (warp == kProducerWarp) {
-    if ((tid & 31) < a.producers)
-      producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0, tid & 31, a.producers);
+    if ((tid & 31) == 0) producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0);
   } else if (warp >= 8) {
-    issuer_loop<false, 1, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kRhATile);
+    issuer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kRhATile);
   } else {
     const int tw = tid >> 7, r = tid & 127;
     uint8_t* arow = smem + (r >> 3) * 128 + (r & 7) * 16;
@@ -269,10 +267,9 @@ __global__ void __launch_bounds__(kTwinThreads, 1) point1_twin_kernel(const __gr
   const int tid = threadIdx.x, warp = tid >> 5;
   const int n_iter = (int)((a.P + 127) / 128);
   if (warp == kProducerWarp) {
-    if ((tid & 31) < a.producers)
-      producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0, tid & 31, a.producers);
+    if ((tid & 31) == 0) producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0);
   } else if (warp >= 8) {
-    issuer_loop<false, 1, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kP1ATile);
+    issuer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kP1ATile);
   } else {
     const int tw = tid >> 7, r = tid & 127;
     uint8_t* arow = smem + (r >> 3) * 128 + (r & 7) * 16;
@@ -374,10 +371,9 @@ __global__ void __launch_bounds__(kTwinThreads, 1) point2_twin_kernel(const __gr
   __syncthreads();
   const int n_iter = (int)((a.P + 127) / 128);
   if (warp == kProducerWarp) {
-    if ((tid & 31) < a.producers)
-      producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0, tid & 31, a.producers);
+    if ((tid & 31) == 0) producer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, a.wimg, n_iter, c.ring, c.bar0);
   } else if (warp >= 8) {
-    issuer_loop<false, 1, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kP2ATile);
+    issuer_loop<false, kTRing, kTStage>(s_tab, a.nchunks, n_iter, smem, c.ring, c.bar0, c.tmem_base, kP2ATile);
   } else {
     const int tw = tid >> 7, r = tid & 127;
     uint8_t* arow = smem + (r >> 3) * 128 + (r & 7) * 16;
@@ -698,7 +694,6 @@ int launch_point1_twin(const dyn_net* n, Point1Args& a, cudaStream_t st) {
   if (!n->chain_tw[0].img) return fail(DYN_E_INVALID, "net has no twin point-stage images");
   a.wimg = n->chain_tw[0].img; a.chunks = n->chain_tw[0].tab; a.nchunks = n->chain_tw[0].nchunks;
   a.params = n->params;
-  a.producers = producer_lanes();
   static bool prepared = false;
   if (!prepared) {
     DYN_CUDA(cudaFuncSetAttribute(point1_twin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kP1Smem));
@@ -713,7 +708,6 @@ int launch_point2_twin(const dyn_net* n, Point2Args& a, cudaStream_t st) {
   const bool dynamic = n->kind == DYN_NET_DYNAMIC;
   a.wimg = n->chain_tw[1].img; a.chunks = n->chain_tw[1].tab; a.nchunks = n->chain_tw[1].nchunks;
   a.params = n->params;
-  a.producers = producer_lanes();
   a.shift = n->shift;
   static bool prepared = false;
   if (!prepared) {
@@ -738,8 +732,7 @@ int launch_rgbhead_twin(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st) {
   if (!n->chain_tw[2].img) return fail(DYN_E_INVALID, "static net has no twin blending-head images");
   a.wimg = n->chain_tw[2].img; a.chunks = n->chain_tw[2].tab; a.nchunks = n->chain_tw[2].nchunks;
   a.params = n->params;
-  a.producers = producer_lanes();
-  a.o_brgb2 = n->sl.rgb2.b; a.o_wrgb4 = n->sl.rgb4.w; a.o_brgb4 = n->sl.rgb4.b;
+  a.o_wrgb4 = n->sl.rgb4.w; a.o_brgb4 = n->sl.rgb4.b;
   static bool prepared = false;
   if (!prepared) {
     DYN_CUDA(cudaFuncSetAttribute(rgbhead_twin_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRhSmem));

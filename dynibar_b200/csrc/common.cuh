@@ -119,18 +119,13 @@ struct dyn_net {
   dyn::DynamicLayout dl;
   dyn::StaticLayout sl;
   dyn::MotionLayout ml;
-  // row-local fused chains (chains_fused.cu): motion: [0]; aggregation nets:
-  // [0] point stage 1, [1] point stage 2, [2] static blending head
-  dyn::ChainImage chain[3];
-  // the same chains in the twin-warp structure (chains_twin.cu): [0] point stage 1, [1] point stage 2,
+  // MotionMLP in one fused kernel (motion_fused.cu): motion net only
+  dyn::ChainImage motion;
+  // row-local chains of the aggregation nets (chains_twin.cu): [0] point stage 1, [1] point stage 2,
   // [2] static blending head
   dyn::ChainImage chain_tw[3];
   // twin-warp per-view stage (view_twin.cu): weight images in its column layout
   dyn::ChainImage twin;
-  // quad-schedule per-view stage (view_quad.cu)
-  dyn::ChainImage quad;
-  // sub-round pipelined twin kernel (view_twin3.cu)
-  dyn::ChainImage twin3;
   // warpgroup per-view stage (view_wg.cu): full-width weight chunks in consumption order
   dyn::ChainImage wg;
 };

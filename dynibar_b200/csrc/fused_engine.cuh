@@ -1,4 +1,4 @@
-// Shared machinery of the fused tensor-core kernels (nets_fused.cu, chains_fused.cu, chains_twin.cu,
+// Shared machinery of the fused tensor-core kernels (nets_fused.cu, motion_fused.cu, chains_twin.cu,
 // view_*.cu): smem budget constants, fast activations, A-tile stores, view-group shuffles, the
 // table-driven weight producer and MMA warpgroup, and the host-side packing of weight chunks into
 // wgmma B-operand images.
@@ -165,11 +165,11 @@ __device__ __forceinline__ void stage_chunks(FusedChunk* s, const FusedChunk* __
 // barrier slots: [0..3] w_full, [4..7] w_empty, [8] a_ready(tile0), [9] acc_full(tile0),
 //                [10] a_ready(tile1), [11] acc_full(tile1)
 // Two schedules:
-//   lock-step (PP = false): both 128-row tiles consume every weight chunk together
-//     (weights stream once per 256 rows); one a_ready (256 arrivals) / acc_full pair.
-//   ping-pong (PP = true): per ROUND (chunks from a wait-flag to a last-flag) tile 0
-//     then tile 1, each with its own barriers (128 arrivals), so the MMA of one tile
-//     overlaps the epilogue of the other; weights stream twice.
+//   one tile (PP = false): one 128-row tile served by two threads per row (twin warps); one a_ready
+//     (2 x 128 arrivals) / acc_full pair.
+//   ping-pong (PP = true): two 128-row tiles, one thread per row; per ROUND (chunks from a wait-flag
+//     to a last-flag) tile 0 then tile 1, each with its own barriers (128 arrivals), so the MMA of one
+//     tile overlaps the epilogue of the other; weights stream twice.
 // generic layout for a ring of `ring` slots: [0,ring) w_full, [ring,2 ring) w_empty, then per tile a_ready, acc_full
 __device__ __forceinline__ uint32_t bar_aready(uint32_t bar0, int tile, int ring = kRing) { return bar0 + 8u * (2 * ring + 2 * tile); }
 __device__ __forceinline__ uint32_t bar_acc(uint32_t bar0, int tile, int ring = kRing) { return bar0 + 8u * (2 * ring + 1 + 2 * tile); }
@@ -194,12 +194,10 @@ __device__ __forceinline__ int round_end(const FusedChunk* __restrict__ chunks, 
   return c + 1 < nchunks ? c + 1 : nchunks;
 }
 
-// `nlanes` lanes of the producer warp share the chunk stream round-robin (lane p issues the chunks with
-// cnt % nlanes == p; RING % nlanes == 0, so a lane always refills the same ring slots).
+// Called by one thread: streams the weight chunks of every iteration through the ring.
 template <bool PP, int RING = kRing, int STAGE = kStageBytes>
 __device__ __forceinline__ void producer_loop(const FusedChunk* __restrict__ chunks, int nchunks,
-                                              const void* wimg, int n_iter, uint8_t* ring, uint32_t bar0,
-                                              uint32_t lane = 0, uint32_t nlanes = 1) {
+                                              const void* wimg, int n_iter, uint8_t* ring, uint32_t bar0) {
   const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(wimg);
   uint32_t cnt = 0;
   for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
@@ -207,7 +205,6 @@ __device__ __forceinline__ void producer_loop(const FusedChunk* __restrict__ chu
       const int c1 = PP ? round_end(chunks, c0, nchunks) : nchunks;
       for (int rep = 0; rep < (PP ? 2 : 1); ++rep) {
         for (int c = c0; c < c1; ++c, ++cnt) {
-          if (cnt % nlanes != lane) continue;
           const uint32_t st = cnt % RING;
           if (cnt >= RING) mbar_wait(bar0 + 8u * (RING + st), ((cnt / RING) - 1) & 1);
           const FusedChunk ch = chunks[c];
@@ -220,71 +217,63 @@ __device__ __forceinline__ void producer_loop(const FusedChunk* __restrict__ chu
   }
 }
 
-// One N-block of a chunk for the accumulator sets of the tiles this chunk serves: 2 x 64-row wgmmas per k-step.
-template <int NB, int NA>
-__device__ __forceinline__ void mma_chunk(float (&acc)[NA][2][kNB / 2], const uint32_t* a_addr, int t0,
-                                          const FusedChunk& ch, uint32_t w_addr) {
+// One N-block of a chunk for the accumulators of one tile: 2 x 64-row wgmmas per k-step.
+template <int NB>
+__device__ __forceinline__ void mma_chunk(float (&acc)[2][kNB / 2], uint32_t a_addr, const FusedChunk& ch,
+                                          uint32_t w_addr) {
   const uint32_t lbo_b = (uint32_t)NB * 16u;
+  const uint32_t aa = a_addr + (uint32_t)ch.a_kgroup * 2048u;
+  for (int ks = 0; ks < ch.ksteps; ++ks) {
+    const uint64_t bd = smem_desc(w_addr + ks * 2u * lbo_b, lbo_b, 128u);
+    const uint32_t sc = ((ch.flags & 8) && ks == 0) ? 0u : 1u;
 #pragma unroll
-  for (int t = 0; t < NA; ++t) {
-    const uint32_t aa = a_addr[t0 + t] + (uint32_t)ch.a_kgroup * 2048u;
-    for (int ks = 0; ks < ch.ksteps; ++ks) {
-      const uint64_t bd = smem_desc(w_addr + ks * 2u * lbo_b, lbo_b, 128u);
-      const uint32_t sc = ((ch.flags & 8) && ks == 0) ? 0u : 1u;
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        Wgmma<NB, 0, 0>::mma(acc[t][h], smem_desc(aa + ks * 4096u + h * 1024u, 2048u, 128u), bd, sc);
-    }
+    for (int h = 0; h < 2; ++h)
+      Wgmma<NB, 0, 0>::mma(acc[h], smem_desc(aa + ks * 4096u + h * 1024u, 2048u, 128u), bd, sc);
   }
 }
-// accumulator sets <-> accumulator memory (tile t at columns col0 + 256 t + d_col)
-template <int NB, int NA>
-__device__ __forceinline__ void acc_chunk_io(float (&acc)[NA][2][kNB / 2], int t0, int col0, bool store) {
+// accumulators <-> accumulator memory (the tile at columns col0 + 256 tile, col0 including d_col)
+template <int NB>
+__device__ __forceinline__ void acc_chunk_io(float (&acc)[2][kNB / 2], int tile, int col0, bool store) {
 #pragma unroll
-  for (int t = 0; t < NA; ++t)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (store) acc_store_frag<NB>(acc[t][h], 64 * h, col0 + 256 * (t0 + t));
-      else acc_load_frag<NB>(acc[t][h], 64 * h, col0 + 256 * (t0 + t));
-    }
+  for (int h = 0; h < 2; ++h) {
+    if (store) acc_store_frag<NB>(acc[h], 64 * h, col0 + 256 * tile);
+    else acc_load_frag<NB>(acc[h], 64 * h, col0 + 256 * tile);
+  }
 }
 
 // one chunk start to finish: resume the N-block from accumulator memory if it continues one, multiply,
 // wait for the wgmmas to retire, store the N-block if it ends here
-template <int NB, int NA>
-__device__ __forceinline__ void run_chunk(float (&acc)[NA][2][kNB / 2], const uint32_t* a_addr, int t0,
-                                          const FusedChunk& ch, uint32_t w_addr, uint32_t tmem_base) {
+template <int NB>
+__device__ __forceinline__ void run_chunk(float (&acc)[2][kNB / 2], uint32_t a_addr, int tile, const FusedChunk& ch,
+                                          uint32_t w_addr, uint32_t tmem_base) {
   const int col0 = (int)(tmem_base & 0xffffu) + ch.d_col;
-  if ((ch.flags & 40) == 32) acc_chunk_io<NB>(acc, t0, col0, false);
-#pragma unroll
-  for (int t = 0; t < NA; ++t) { fence_regs<NB / 2>(acc[t][0]); fence_regs<NB / 2>(acc[t][1]); }
+  if ((ch.flags & 40) == 32) acc_chunk_io<NB>(acc, tile, col0, false);
+  fence_regs<NB / 2>(acc[0]); fence_regs<NB / 2>(acc[1]);
   wgmma_fence();
-  mma_chunk<NB>(acc, a_addr, t0, ch, w_addr);
+  mma_chunk<NB>(acc, a_addr, ch, w_addr);
   wgmma_commit();
   wgmma_wait<0>();
-#pragma unroll
-  for (int t = 0; t < NA; ++t) { fence_regs<NB / 2>(acc[t][0]); fence_regs<NB / 2>(acc[t][1]); }
-  if (ch.flags & 16) acc_chunk_io<NB>(acc, t0, col0, true);
+  fence_regs<NB / 2>(acc[0]); fence_regs<NB / 2>(acc[1]);
+  if (ch.flags & 16) acc_chunk_io<NB>(acc, tile, col0, true);
 }
 
 // Called by ALL 128 threads of the MMA warpgroup (warps 4k .. 4k + 3 of the CTA).
 // FusedChunk.flags: 1 = wait for a_ready before this chunk, 2 = last chunk of a
-// round (signal acc_full), 4 = wait for the second operand barrier (one-tile kernels: the
-// a_ready slot of tile 1) before this chunk, 8 = first k-step overwrites D (start of a layer),
+// round (signal acc_full), 8 = first k-step overwrites D (start of a layer),
 // 16 / 32 = last / first chunk of an N-block (store it to TMEM / without 8: continue from TMEM);
 // d_col = accumulator column offset inside the tile's 256-column TMEM region.
-// NT = 128-row tiles per CTA (1 or 2), RING = weight-ring slots in use.
-template <bool PP, int NT = 2, int RING = kRing, int STAGE = kStageBytes>
+// RING = weight-ring slots in use.
+template <bool PP, int RING = kRing, int STAGE = kStageBytes>
 __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunks, int nchunks, int n_iter,
                                             uint8_t* smem, uint8_t* ring, uint32_t bar0,
                                             uint32_t tmem_base, int a_tile_bytes = kATileBytes,
                                             long long* dbg = nullptr) {
-  // wgmma is issued by the whole warpgroup; the accumulators of one N-block (<= kNB columns) of every tile the
+  // wgmma is issued by the whole warpgroup; the accumulators of one N-block (<= kNB columns) of the tile the
   // chunk serves stay in registers across the N-block's chunks
   {
-    float acc[PP ? 1 : NT][2][kNB / 2];
+    float acc[2][kNB / 2];
     const bool lead = threadIdx.x % 128 == 0;
-    uint32_t cnt = 0, a_cnt[2] = {0, 0}, a2_cnt = 0;
+    uint32_t cnt = 0, a_cnt[2] = {0, 0};
     long long t_a = 0, t_w = 0, t_begin = clock64();
     const uint32_t a_addr[2] = {smem_u32(smem), smem_u32(smem + a_tile_bytes)};
     for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
@@ -298,10 +287,6 @@ __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunk
               mbar_wait(bar_aready(bar0, PP ? rep : 0, RING), a_cnt[PP ? rep : 0] & 1);
               ++a_cnt[PP ? rep : 0];
             }
-            if (!PP && NT == 1 && (ch.flags & 4)) {  // second operand barrier of a two-sub-round layer
-              mbar_wait(bar_aready(bar0, 1, RING), a2_cnt & 1);
-              ++a2_cnt;
-            }
             long long t1 = dbg ? clock64() : 0;
             const uint32_t st = cnt % RING;
             mbar_wait(bar0 + 8u * st, (cnt / RING) & 1);
@@ -313,12 +298,12 @@ __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunk
               t_w += t2 - t1;
             }
             const uint32_t w_addr = smem_u32(ring + st * STAGE);
-            const int tile0 = PP ? rep : 0;
+            const int tile = PP ? rep : 0;
             switch (ch.npad) {
-              case 16: run_chunk<16>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
-              case 32: run_chunk<32>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
-              case 48: run_chunk<48>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
-              case 64: run_chunk<64>(acc, a_addr, tile0, ch, w_addr, tmem_base); break;
+              case 16: run_chunk<16>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
+              case 32: run_chunk<32>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
+              case 48: run_chunk<48>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
+              case 64: run_chunk<64>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
               default: __trap();  // the host packer emits N-blocks of 16, 32, 48 or 64 columns only
             }
             __syncwarp();
@@ -424,38 +409,15 @@ inline void append_block(const HostLayer& L, std::vector<uint8_t>& img, std::vec
 }
 
 // A layer as N-blocks of at most kNB output columns, each streamed over all of K before the next one (the
-// MMA warpgroup keeps one N-block's accumulators in registers).  The operand waits of `first_flags` (1, 4) go
+// MMA warpgroup keeps one N-block's accumulators in registers).  The operand wait of `first_flags` (1) goes
 // on the layer's first chunk, its 8 ("overwrite D") on the first chunk of every N-block.
 inline void append_layer(const HostLayer& L, std::vector<uint8_t>& img, std::vector<FusedChunk>& tab,
                          int d_col = 0, int a_kgroup0 = 0, int first_flags = 9, bool last = true,
                          int stage_bytes = kStageBytes) {
   for (int n0 = 0; n0 < L.Npad; n0 += kNB)
     append_block(layer_rows(L, n0, L.Npad - n0 < kNB ? L.Npad - n0 : kNB), img, tab, d_col + n0, a_kgroup0,
-                 32 | (n0 == 0 ? first_flags & 5 : 0) | (first_flags & 8),
+                 32 | (n0 == 0 ? first_flags & 1 : 0) | (first_flags & 8),
                  16 | (last && n0 + kNB >= L.Npad ? 2 : 0), stage_bytes, 0, L.Kpad / 16);
-}
-
-// A layer issued in SUB-ROUNDS: `plan[r]` lists the runs (first k-step, number of k-steps) of operand columns
-// that sub-round r consumes; the issuer waits for one operand arrival round per sub-round (chunk flag 1) and
-// signals the epilogue only after the last one (flag 2).  The row warps arrive after every block of operand
-// columns they finish, so the k-steps over finished columns overlap the epilogue of the remaining ones.
-// Every sub-round covers all N-blocks; sub-round 1 continues from the partial sums sub-round 0 stored.
-// Chunk c of a run starting at k-step k0 reads the operand tile at k-group a_kgroup0 + 2 * (k0 + ...).
-using LayerPlan = std::vector<std::vector<std::pair<int, int>>>;
-inline void append_layer_plan(const HostLayer& L, std::vector<uint8_t>& img, std::vector<FusedChunk>& tab,
-                              int d_col, int a_kgroup0, const LayerPlan& plan, int stage_bytes = kStageBytes) {
-  const size_t nr = plan.size() < 2 ? plan.size() : 2;  // at most two sub-rounds (two operand barriers)
-  for (size_t r = 0; r < nr; ++r)
-    for (int n0 = 0; n0 < L.Npad; n0 += kNB)
-      for (size_t q = 0; q < plan[r].size(); ++q) {
-        // sub-round 0 waits on the operand barrier (flag 1), sub-round 1 on the SECOND operand barrier (flag 4):
-        // a row thread arrives on each of them exactly once per layer -- with a single barrier a fast thread's
-        // second arrival could complete the phase that a slow thread has not reached yet
-        const int first = q > 0 ? 0 : 32 | (n0 == 0 ? (r == 0 ? 1 : 4) : 0) | (r == 0 ? 8 : 0);
-        const int last = q + 1 < plan[r].size() ? 0 : 16 | (r + 1 == nr && n0 + kNB >= L.Npad ? 2 : 0);
-        append_block(layer_rows(L, n0, L.Npad - n0 < kNB ? L.Npad - n0 : kNB), img, tab, d_col + n0, a_kgroup0,
-                     first, last, stage_bytes, plan[r][q].first, plan[r][q].first + plan[r][q].second);
-      }
 }
 
 inline std::vector<int> identity_map(int K, int Kpad) {
@@ -463,22 +425,6 @@ inline std::vector<int> identity_map(int K, int Kpad) {
   for (int i = 0; i < K; ++i) m[i] = i;
   return m;
 }
-// [mean8 | var8 | feat8] per channel group; C channels, source columns
-// [0,C) mean, [C,2C) var, [2C,3C) per-view feature
-inline std::vector<int> pooled_map(int C, int groups, int Kpad) {
-  std::vector<int> m(Kpad, -1);
-  for (int g = 0; g < groups; ++g)
-    for (int j = 0; j < 8; ++j) {
-      const int c = 8 * g + j;
-      if (c < C) {
-        m[24 * g + j] = c;
-        m[24 * g + 8 + j] = C + c;
-        m[24 * g + 16 + j] = 2 * C + c;
-      }
-    }
-  return m;
-}
-
 
 }  // namespace fe
 }  // namespace dyn

@@ -14,7 +14,6 @@ struct FusedChunk {
   uint8_t ksteps;        // K = 16 * ksteps in this chunk
   uint8_t flags;         // 1: wait for the operand (a_ready) before this chunk
                          // 2: last chunk of a round (signal the epilogue)
-                         // 4: wait for the second operand barrier (sub-round 1 of a pipelined layer)
                          // 8: first k-step overwrites D (start of a layer)
                          // 16 / 32: last / first chunk of an N-block (fused_engine.cuh: issuer_loop)
   uint16_t a_kgroup;     // first 8-column group of the A tile this chunk consumes
@@ -49,12 +48,10 @@ struct ViewFusedArgs {
   float* vis2;       // static [P*V]
   float* ray_diff;   // static [P*V,4]
   float* rgb_in;     // static [P*V,3] gathered source colours
-  int producers;     // lanes of the producer warp that stream weight chunks (1 or 2)
-  int ablate;        // profiling only (DYN_ABLATE): 1 skip gather loads, 2 skip X/vis/mask stores, 4 skip pooled-output stores, 8 skip second pooling
   long long* dbg;    // optional: clock64() phase timestamps of block 0 (profiling builds/tests only)
 };
 
-// ---- row-local fused chains (chains_fused.cu) ----
+// ---- MotionMLP (motion_fused.cu) ----
 struct MotionFusedArgs {
   const float* x;  // [N, ldx] xyz (+ time column when time_is_column)
   int ldx, time_is_column;
@@ -68,9 +65,9 @@ struct MotionFusedArgs {
   const void* wimg;
   const FusedChunk* chunks;
   int nchunks;
-  int producers;  // lanes of the producer warp that stream weight chunks
 };
 
+// ---- row-local twin-warp chains (chains_twin.cu) ----
 struct Point1Args {
   const float* G;       // [P, kGStride]
   const float* posenc;  // [S,128] sinusoid table (dynamic) or null
@@ -79,11 +76,9 @@ struct Point1Args {
   float* g2;                 // [P,128] fp32 (residual of the ray transformer)
   __nv_bfloat16 *Q, *K, *V;  // [P,128] bf16 (operands of the attention)
   const float* params;
-  int o_bgeo0, o_bgeo2;
   const void* wimg;
   const FusedChunk* chunks;
   int nchunks;
-  int producers;  // lanes of the producer warp that stream weight chunks
 };
 
 struct Point2Args {
@@ -99,12 +94,10 @@ struct Point2Args {
   float* GW;     // static:  [P,128] per-point part of rgb_fc.0 (bias included)
   float* sigma;  // static:  [P] masked density
   const float* params;
-  int o_lnw, o_lnb, o_brefpts0, o_brefpts2, o_boutgeo0, o_woutgeo2, o_boutgeo2, o_brgb0, o_brgb2,
-      o_wrgb4, o_brgb4;
+  int o_lnw, o_lnb, o_woutgeo2, o_boutgeo2, o_wrgb4, o_brgb4;
   const void* wimg;
   const FusedChunk* chunks;
   int nchunks;
-  int producers;  // lanes of the producer warp that stream weight chunks
 };
 
 struct RgbHeadArgs {
@@ -113,47 +106,31 @@ struct RgbHeadArgs {
   int V;
   float* raw;  // [P,4]
   const float* params;
-  int o_brgb2, o_wrgb4, o_brgb4;
+  int o_wrgb4, o_brgb4;
   const void* wimg;
   const FusedChunk* chunks;
   int nchunks;
-  int producers;  // lanes of the producer warp that stream weight chunks
 };
 
 int debug_pack_layer(const float* W, const float* bias, int N, int Kw, int Npad, int Kpad, const int* colmap,
                      float scale, int stage_bytes, void* out_img, size_t out_bytes, size_t* img_bytes,
                      int* nchunks);
 size_t debug_tile_image_off(long long row, int kgroup, int kgroups);
-size_t fused_chain_bytes(int kind);
-int fused_chain_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes,
-                      cudaStream_t st);
+size_t motion_fused_bytes();
+int motion_fused_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_motion_fused(const dyn_net* n, MotionFusedArgs& a, cudaStream_t st);
-int launch_point1_fused(const dyn_net* n, Point1Args& a, cudaStream_t st);
-int launch_point2_fused(const dyn_net* n, Point2Args& a, cudaStream_t st);
-int launch_rgbhead_fused(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st);
 
-// twin-warp versions of the row-local chains (chains_twin.cu, the default); DYN_CHAINS=fused selects chains_fused.cu
+// the point stages and the static blending head (chains_twin.cu)
 size_t twin_chain_bytes(int kind);
 int twin_chain_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_point1_twin(const dyn_net* n, Point1Args& a, cudaStream_t st);
 int launch_point2_twin(const dyn_net* n, Point2Args& a, cudaStream_t st);
 int launch_rgbhead_twin(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st);
-bool use_twin_chains();
 
 // twin-warp per-view stage (view_twin.cu)
 size_t view_twin_bytes(int kind);
 int view_twin_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_view_twin(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);
-
-// sub-round pipelined twin-warp per-view stage (view_twin3.cu)
-size_t view_twin3_bytes(int kind);
-int view_twin3_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
-int launch_view_twin3(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st, bool elected_arrive = false);
-
-// quad-schedule per-view stage (view_quad.cu): one CTA per SM, two tiles, four threads per row
-size_t view_quad_bytes(int kind);
-int view_quad_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
-int launch_view_quad(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);
 
 // warpgroup per-view stage (view_wg.cu, the default): accumulators in registers, two 64-row warpgroups per CTA
 size_t view_wg_bytes(int kind);
@@ -161,7 +138,6 @@ int view_wg_build(dyn_net* n, const float* host_params, void* dst_dev, size_t ds
 int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);
 
 void set_view_kernel(int which);
-int producer_lanes();  // DYN_PRODUCERS (default 1)
 int launch_view_fused(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st);
 
 }  // namespace dyn

@@ -11,7 +11,7 @@
 //
 // Engine: fused_engine.cuh (operand tile in shared memory written by the epilogues, accumulators
 // in TMEM, weights streamed through a cp.async.bulk ring, table-driven MMA warpgroup).  Every row is
-// served by TWO threads in twin warps w and w + 4*NT (same TMEM lane quadrant), which is what the
+// served by TWO threads in twin warps w and w + 4 (same TMEM lane quadrant), which is what the
 // latency-bound epilogues need; each twin owns half of every layer's output columns and half of the
 // gathered / pooled channels, and the twins exchange only two scalars per row and iteration (the
 // partial visibility logits).
@@ -19,7 +19,6 @@
 // One CTA per SM with one 128-row tile:
 //   warps 0-3  : twin 0 (quadrant = w & 3)  warps 4-7 : twin 1 of the same rows
 //   warps 8-11 : MMA warpgroup (wgmma)      warp 12   : weight producer
-// (the alternating two-tile schedule lives in view_quad.cu).
 //
 // Latency hiding inside a CTA: the source views are read in
 // their packed per-frame layouts (bf16 channels-last features: 2 x 16-byte loads per tap and twin; RGBA
@@ -27,7 +26,6 @@
 // positional-encoding operand has been built and handed to the tensor cores, the per-ray reference
 // feature is loaded before the wait for ray_dir_fc.2, the next iteration's points before the last wait,
 // and the camera matrices sit in shared memory (lanes of a warp index different views).
-#include <cstdlib>
 #include "fused_engine.cuh"
 #include "geometry.cuh"
 #include "nets.cuh"
@@ -39,19 +37,18 @@ using namespace fe;
 
 namespace {
 
-constexpr bool kTwinPP = true;  // ping-pong between the tiles of a two-tile CTA
 constexpr int kTwinATile = 69632;  // K <= 256 (+ one k-step of bias columns): 34 k-groups
 // T_B5 / T_B7 hold log2(e) * bias, T_W6V / T_W8 hold ln(2) * weight (the hidden activations of vis_fc.0 and
 // vis_fc2.0 live on the exp2 scale); the biases of base_fc.2 and vis_fc.2 ride in the MMA
 constexpr int T_B2 = 0, T_B5 = 48, T_W6V = 176, T_B7 = 304, T_W8 = 432, T_MISC = 560, T_DFEAT = 576,
               T_CAMS = 624 /* 16 views x (P 12 + centre 3 + pad) */, T_XCH = T_CAMS + 256;  // + 2 x [2][128] exchange
 constexpr int kTwinConst = T_XCH + 512;
-// NT = 128-row tiles per CTA (only NT = 1 is instantiated); 8 KB weight stages leave room for TMEM in shared memory.
+// two 8 KB weight stages leave room for TMEM in shared memory
 constexpr int kTwinStage = 8192;
-constexpr int twin_ring(int nt) { return nt == 1 ? 2 : 4; }
-constexpr int twin_threads(int nt) { return nt * 256 + 32 * (kIssuerWarps + 1); }
-// shared memory: operand tile(s) | weight ring | constants | barriers (256 B) | accumulator memory (one tile)
-constexpr int twin_smem(int nt) { return nt * kTwinATile + twin_ring(nt) * kTwinStage + kTwinConst * 4 + 256 + kAccSmemBytes; }
+constexpr int kTwinRing = 2;
+constexpr int kTwinThreads = 256 + 32 * (kIssuerWarps + 1);
+// shared memory: operand tile | weight ring | constants | barriers (256 B) | accumulator memory (one tile)
+constexpr int kTwinSmem = kTwinATile + kTwinRing * kTwinStage + kTwinConst * 4 + 256 + kAccSmemBytes;
 
 __device__ __forceinline__ void pair_sync(int pair) {
   asm volatile("bar.sync %0, 64;" ::"r"(pair + 1) : "memory");
@@ -100,15 +97,13 @@ __device__ __forceinline__ void elu_block_to_A(uint8_t* arow, uint32_t tacc, int
   }
 }
 
-template <int VP, bool ST, int NT>
-__global__ void __launch_bounds__(twin_threads(NT), 1)
-    view_twin_kernel(const __grid_constant__ ViewFusedArgs a) {
-  constexpr int ROWS = 128 * NT;          // rows per iteration
-  constexpr int RING = twin_ring(NT);
-  constexpr bool PP = (NT == 2) && kTwinPP;
-  constexpr int W_ISSUE = 8 * NT, W_PROD = 8 * NT + kIssuerWarps;  // MMA warpgroup, weight producer
+template <int VP, bool ST>
+__global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid_constant__ ViewFusedArgs a) {
+  constexpr int ROWS = 128;  // rows per iteration
+  constexpr int RING = kTwinRing;
+  constexpr int W_ISSUE = 8, W_PROD = 8 + kIssuerWarps;  // MMA warpgroup, weight producer
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* ring = smem + NT * kTwinATile;
+  uint8_t* ring = smem + kTwinATile;
   float* cst = reinterpret_cast<float*>(ring + RING * kTwinStage);
   uint64_t* bars = reinterpret_cast<uint64_t*>(cst + kTwinConst);
   uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 24);
@@ -117,7 +112,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
   __shared__ __align__(16) FusedChunk s_tab[kMaxChunks];
   stage_chunks(s_tab, a.chunks, a.nchunks);
 
-  if (tid == 0) init_barriers(bar0, PP, /*arrivals=*/NT == 2 ? 256 : 128, RING);
+  if (tid == 0) init_barriers(bar0, /*pp=*/false, /*arrivals=*/128, RING);
   {
     const float* prm = a.params;
     for (int i = tid; i < 256; i += blockDim.x) {  // camera matrices: lanes index them by view
@@ -138,8 +133,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       cst[T_MISC + 2] = (ST && a.o_s >= 0) ? fabsf(prm[a.o_s]) : 0.f;
     }
   }
-  static_assert(NT == 1, "the accumulator memory in shared memory holds one tile");
-  if (warp == W_ISSUE) tmem_alloc_smem(smem_u32(tmem_slot), smem + twin_smem(NT) - kAccSmemBytes);
+  if (warp == W_ISSUE) tmem_alloc_smem(smem_u32(tmem_slot), smem + kTwinSmem - kAccSmemBytes);
   tc_fence_before_sync();
   __syncthreads();
   tc_fence_after_sync();
@@ -149,24 +143,19 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
   const int n_iter = (int)((n_rows + ROWS - 1) / ROWS);
 
   if (warp == W_PROD) {
-    if ((tid & 31) < a.producers)
-      producer_loop<PP, RING, kTwinStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0, tid & 31, a.producers);
+    if ((tid & 31) == 0) producer_loop<false, RING, kTwinStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
   } else if (warp >= W_ISSUE) {
-    issuer_loop<PP, NT, RING, kTwinStage>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base, kTwinATile,
-                           a.dbg ? a.dbg + 128 : nullptr);
+    issuer_loop<false, RING, kTwinStage>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base, kTwinATile,
+                                         a.dbg ? a.dbg + 128 : nullptr);
   } else {
-    const int tw = tid / ROWS;         // twin index
-    const int t = tid % ROWS;          // row slot inside the iteration
-    const int tile = t >> 7, r = t & 127;
-    uint8_t* arow = smem + tile * kTwinATile + (r >> 3) * 128 + (r & 7) * 16;
-    const uint32_t tacc = tmem_addr(tmem_base, (uint32_t)((warp & 3) * 32), (uint32_t)(tile * 256));
+    const int tw = tid >> 7, t = tid & 127;  // twin index, row of the tile
+    uint8_t* arow = smem + (t >> 3) * 128 + (t & 7) * 16;
+    const uint32_t tacc = tmem_addr(tmem_base, (uint32_t)((warp & 3) * 32), 0u);
     const int v = t % VP;
     const int gl = t & (VP - 1);
-    const int pair = warp & (4 * NT - 1);
-    const int bt = PP ? tile : 0;  // barrier tile
+    const int pair = warp & 3;
     float* xch5 = cst + T_XCH;        // [2][128] partial visibility logits of vis_fc
     float* xch7 = cst + T_XCH + 256;  // [2][128] partial logits of vis_fc2
-    static_assert(NT == 1, "exchange arrays are sized for one tile per CTA");
     if (tw == 0) {
       // persistent bias columns of base_fc.2 (K = 256 + 16): k-groups 32, 33 = [1, 1, 0 ...] (hi, lo)
       float o[8] = {1.f, 1.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -224,7 +213,6 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       float tw4[4], twr[4];
       {
         const float gx = 2.f * pu / (wh - 1.f) - 1.f, gy = 2.f * pv / (hh - 1.f) - 1.f;
-        const bool ld = valid && !(a.ablate & 1);
         {
           const float fx = (gx + 1.f) * 0.5f * (float)(a.w - 1), fy = (gy + 1.f) * 0.5f * (float)(a.h - 1);
           const float x0f = floorf(fx), y0f = floorf(fy);
@@ -238,7 +226,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
               // out-of-range taps (and padding rows) load a clamped texel with weight 0: no branch, all loads
               // of this thread are in flight together
               const int xi = x0 + dx, yi = y0 + dy;
-              const bool in = ld && xi >= 0 && xi < a.w && yi >= 0 && yi < a.h;
+              const bool in = valid && xi >= 0 && xi < a.w && yi >= 0 && yi < a.h;
               tw4[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
               const int xc = min(max(xi, 0), a.w - 1), yc = min(max(yi, 0), a.h - 1);
               const uint4* tp = reinterpret_cast<const uint4*>(base + ((long long)yc * a.w + xc) * kC);
@@ -257,7 +245,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
 #pragma unroll
             for (int dx = 0; dx < 2; ++dx) {
               const int xi = x0 + dx, yi = y0 + dy;
-              const bool in = ld && xi >= 0 && xi < a.W && yi >= 0 && yi < a.H;
+              const bool in = valid && xi >= 0 && xi < a.W && yi >= 0 && yi < a.H;
               twr[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
               const int xc = min(max(xi, 0), a.W - 1), yc = min(max(yi, 0), a.H - 1);
               tr[2 * dy + dx] = __ldg(reinterpret_cast<const float4*>(base + ((long long)yc * a.W + xc) * 4));
@@ -312,7 +300,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
         }
         fence_proxy_async_smem();
         tc_fence_before_sync();
-        mbar_arrive(bar_aready(bar0, bt, RING));
+        mbar_arrive(bar_aready(bar0, 0, RING));
       }
 
       TS();  // 1: after F1 operand + arrive
@@ -353,7 +341,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       if (ST && a.mask_rgb) mask *= ((rgb[0] + rgb[1] + rgb[2]) > 1e-3f) ? 1.f : 0.f;
       if (tw == 0) {
         chv[0] = rgb[0]; chv[1] = rgb[1]; chv[2] = rgb[2];
-        if (valid && !(a.ablate & 2)) {
+        if (valid) {
           a.mask_proj[m] = mask_proj;
           if (ST) {
             a.mask_eff[m] = mask;
@@ -366,13 +354,13 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       TS();  // 2: after gather
       if (ST) {
         // ---- F1 epilogue: this twin's 128 of the 256 columns ----
-        mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+        mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
         TS();  // 3: F1 acc ready
         tc_fence_after_sync();
         elu_log2_block_to_A<128>(arow, tacc, 128 * tw);
         fence_proxy_async_smem();
         tc_fence_before_sync();
-        mbar_arrive(bar_aready(bar0, bt, RING));
+        mbar_arrive(bar_aready(bar0, 0, RING));
         TS();  // 4: F1 epilogue done
         // ---- F2: src_feat (35 of 48 columns) * ref_feat; twin 0 keeps 0..17, twin 1 keeps 18..34.
         //      The per-ray reference feature is loaded BEFORE the wait (its L2 latency hides behind the MMA) ----
@@ -382,7 +370,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
 #pragma unroll
           for (int i = 0; i < 18; ++i) rfv[i] = (tw == 0 || i < 17) ? __ldg(rf + i) : 0.f;
         }
-        mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+        mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
         TS();  // 5: F2 acc ready
         tc_fence_after_sync();
         float s48[48];
@@ -448,23 +436,23 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       }
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, bt, RING));
+      mbar_arrive(bar_aready(bar0, 0, RING));
 
       TS();  // 6: pool1 done + arrive
       // ---- F3: ELU(base_fc.0), this twin's 128 columns ----
-      mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 7: F3 acc ready
       tc_fence_after_sync();
       elu_log2_block_to_A<128>(arow, tacc, 128 * tw);
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, bt, RING));
+      mbar_arrive(bar_aready(bar0, 0, RING));
 
       const int c0 = 64 * tw;  // this twin's columns of the 128-wide layers
       TS();  // 8: F3 epilogue done
       // ---- F4: x = ELU(base_fc.2) -> TMEM [128,256); A = x (the pooling weight w1 of vis_fc.0's input is applied
       //      to the accumulator in the next epilogue: W (w1 x) = w1 (W x)); bias folded, accumulator on the exp2 scale ----
-      mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 9: F4 acc ready
       tc_fence_after_sync();
 #pragma unroll 1
@@ -487,11 +475,11 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       tmem_wait_st();
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, bt, RING));
+      mbar_arrive(bar_aready(bar0, 0, RING));
 
       TS();  // 10: F4 epilogue done
       // ---- F5: h = ELU(vis_fc.0) -> A; partial visibility logit ----
-      mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 11: F5 acc ready
       tc_fence_after_sync();
       {
@@ -513,11 +501,11 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       }
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, bt, RING));
+      mbar_arrive(bar_aready(bar0, 0, RING));
 
       TS();  // 12: F5 epilogue done
       // ---- F6: x += ELU(vis_fc.2[:128]); A = x * vis1 ----
-      mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 13: F6 acc ready
       tc_fence_after_sync();
       // both twins arrived on a_ready before this MMA ran: the partial logits are visible
@@ -539,7 +527,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
         for (int i = 0; i < 4; ++i)
           pk[i] = make_uint4(pack_bf16x2(xs[8 * i], xs[8 * i + 1]), pack_bf16x2(xs[8 * i + 2], xs[8 * i + 3]),
                              pack_bf16x2(xs[8 * i + 4], xs[8 * i + 5]), pack_bf16x2(xs[8 * i + 6], xs[8 * i + 7]));
-        if (ST && !(a.ablate & 2)) {
+        if (ST) {
           uint8_t* xo = reinterpret_cast<uint8_t*>(a.X) + tile_image_off((long long)it * ROWS + t, cb >> 3, 16);
 #pragma unroll
           for (int i = 0; i < 4; ++i) *reinterpret_cast<uint4*>(xo + i * 2048) = pk[i];
@@ -550,12 +538,12 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       tmem_wait_st();
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, bt, RING));
+      mbar_arrive(bar_aready(bar0, 0, RING));
 
       TS();  // 14: F6 epilogue done
       if (it + (int)gridDim.x < n_iter) fetch_point(it + (int)gridDim.x);  // next iteration's point
       // ---- F7: vis2 = sigmoid(vis_fc2.2 . ELU(vis_fc2.0)) * mask ----
-      mbar_wait(bar_acc(bar0, bt, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 15: F7 acc ready
       tc_fence_after_sync();
       {
@@ -575,14 +563,14 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
       pair_sync(pair);
       const float v2 = cst[T_MISC + 1] + xch7[t] + xch7[128 + t];
       const float vis2 = sigmoid_fast(v2) * mask;
-      if (ST && valid && tw == 0 && !(a.ablate & 2)) a.vis2[m] = vis2;
+      if (ST && valid && tw == 0) a.vis2[m] = vis2;
       const float vsum = group_sum<VP>(vis2);
       const float w2 = vis2 / (vsum + 1e-8f);
       const float W = group_sum<VP>(w2);
       const float nval = group_sum<VP>(mask);
 
       // ---- second pooling on this twin's 64 channels: reduce-scatter of sum(w x), sum(w x^2) ----
-      if (!(a.ablate & 8)) {
+      {
         const bool b0 = gl & 1, b1 = gl & 2, b2 = gl & 4, b3 = gl & 8;
         constexpr int NO = VP == 16 ? 4 : 8;
         const int cbase = c0 + (b0 ? 32 : 0) + (b1 ? 16 : 0) + (b2 ? 8 : 0) + ((VP == 16 && b3) ? 4 : 0);
@@ -615,7 +603,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
             for (int i = 0; i < NO; ++i) dst[i] = s3[i < 8 ? i : 0];
           }
         }
-        if (pt_ok && !(a.ablate & 4)) {
+        if (pt_ok) {
           // pooled statistics as the bf16 tile image of geometry_fc's operand (34 k-groups:
           // mean 0..127 | var 128..255 | weight 256 | zero pad), rows = points
           uint8_t* gi = reinterpret_cast<uint8_t*>(a.G);
@@ -652,7 +640,7 @@ __global__ void __launch_bounds__(twin_threads(NT), 1)
   __syncthreads();
   if (warp == W_ISSUE) {
     tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 256 * NT);
+    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -754,34 +742,31 @@ int launch_view_twin(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st)
   a.wimg = n->twin.img;
   a.chunks = n->twin.tab;
   a.nchunks = n->twin.nchunks;
-  // one-time set-up (profiling knob DYN_ABLATE, SM count, dynamic shared-memory opt-in of every instantiation)
-  static int ablate = -1, sms = 0;
-  if (ablate < 0) {
-    const char* e = getenv("DYN_ABLATE");
+  // one-time set-up (SM count, dynamic shared-memory opt-in of every instantiation)
+  static int sms = 0;
+  if (sms == 0) {
     int dev = 0;
     DYN_CUDA(cudaGetDevice(&dev));
     DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
 #define PREP_VT(VPV, STV) \
-    DYN_CUDA(cudaFuncSetAttribute(view_twin_kernel<VPV, STV, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, twin_smem(1)))
+    DYN_CUDA(cudaFuncSetAttribute(view_twin_kernel<VPV, STV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTwinSmem))
     PREP_VT(8, true); PREP_VT(16, true); PREP_VT(8, false); PREP_VT(16, false);
 #undef PREP_VT
-    ablate = e ? atoi(e) : 0;
   }
-  a.ablate = ablate;
   const int VP = V <= 8 ? 8 : 16;
   const long long n_iter = (a.P * VP + 127) / 128;
-  static_assert(2 * twin_smem(1) > 227 * 1024, "one CTA per SM");  // shared memory holds the accumulators
+  static_assert(2 * kTwinSmem > 227 * 1024, "one CTA per SM");  // shared memory holds the accumulators
   const long long slots = sms;
   const int grid = (int)(n_iter < slots ? n_iter : slots);
   if (grid == 0) return DYN_OK;
   const bool st_net = n->kind == DYN_NET_STATIC;
   ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
   if (st_net) {
-    if (VP == 8) view_twin_kernel<8, true, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
-    else view_twin_kernel<16, true, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
+    if (VP == 8) view_twin_kernel<8, true><<<grid, kTwinThreads, kTwinSmem, st>>>(a);
+    else view_twin_kernel<16, true><<<grid, kTwinThreads, kTwinSmem, st>>>(a);
   } else {
-    if (VP == 8) view_twin_kernel<8, false, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
-    else view_twin_kernel<16, false, 1><<<grid, twin_threads(1), twin_smem(1), st>>>(a);
+    if (VP == 8) view_twin_kernel<8, false><<<grid, kTwinThreads, kTwinSmem, st>>>(a);
+    else view_twin_kernel<16, false><<<grid, kTwinThreads, kTwinSmem, st>>>(a);
   }
   DYN_LAUNCH_CHECK();
   return DYN_OK;

@@ -388,10 +388,9 @@ size_t dyn_debug_tile_image_off(long long row, int kgroup, int kgroups);
 
 /* comparison hook: which kernel runs the fused per-view stage: 4 = warpgroup kernel (csrc/view_wg.cu:
  * accumulators in registers, two 64-row warpgroups per CTA; the default), 0 = twin-warp kernel
- * (csrc/view_twin.cu: one tile per CTA), 1 = quad-schedule kernel (csrc/view_quad.cu: one CTA per SM
- * alternating between two tiles), 2 = twin-warp kernel with sub-round pipelined layers (csrc/view_twin3.cu),
- * 3 = the same with one barrier arrival per warp; -1 = the default.  The environment variable
- * DYN_VIEW_KERNEL=twin|quad|pipe sets the initial value. */
+ * (csrc/view_twin.cu: one tile per CTA); -1 = the default.  1 - 3 selected the quad-schedule and the
+ * sub-round pipelined twin kernels, which have been removed: with them the fused per-view stage fails
+ * with DYN_E_INVALID. */
 void dyn_debug_set_view_kernel(int which);
 
 /* profiling hook: when set, block 0 of the fused static per-view kernel writes clock64()
