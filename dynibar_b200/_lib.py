@@ -68,6 +68,7 @@ SIGNATURES = {
     "dyn_resample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "dyn_debug_set_view_timestamps": (None, [_vp]),
     "dyn_debug_set_view_kernel": (None, [_i]),
+    "dyn_debug_set_view_capture": (None, [_vp] * 7),
     "dyn_debug_point_chain": (_i, [_vp] * 5 + [_i, _i] + [_vp] * 9),
     "dyn_debug_pack_layer": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _f, _i, _vp, _sz, _vp, _vp]),
     "dyn_debug_tile_image_off": (_sz, [C.c_longlong, _i, _i]),

@@ -263,6 +263,11 @@ static long long* g_view_dbg = nullptr;
 void dyn_debug_set_view_timestamps(long long* dev_buf) { g_view_dbg = dev_buf; }
 long long* view_dbg_ptr() { return g_view_dbg; }
 
+void dyn_debug_set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
+                                float* rgb_in) {
+  set_view_capture(G, nvalid, X, vis2, mask_eff, ray_diff, rgb_in);
+}
+
 int dyn_net_static_fused(dyn_net_t net, const float* pts, const float* ray_o, const float* ray_d,
                          const float* query_cam, const float* src_rgbs, const float* src_cams,
                          const void* feat_cl, int R, int S, int V, int H, int W, int C, int h, int w,

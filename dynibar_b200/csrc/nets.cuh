@@ -33,6 +33,8 @@ int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, 
 int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, const float* pts,
                       const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
                       float* O, float* out_a, float* out_b, float* posenc_ws, cudaStream_t st);
+void set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
+                      float* rgb_in);
 // tensor-core ray-transformer attention (attention_tc.cu); S must divide 128
 bool attention_tc_supported(int S);
 int launch_attention_tc(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __nv_bfloat16* V,

@@ -947,6 +947,66 @@ int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, con
   return rc;
 }
 
+// Unit-test hook (dyn_debug_set_view_capture): the per-view stage's outputs of every internal chunk, unpacked
+// into caller buffers at the chunk's row offset.  Off (all NULL) on the product path.
+struct ViewCapture {
+  float *G, *nvalid, *X, *vis2, *mask_eff, *ray_diff, *rgb_in;
+};
+static ViewCapture g_view_cap = {};
+static bool g_view_cap_on = false;
+
+void set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
+                      float* rgb_in) {
+  g_view_cap = ViewCapture{G, nvalid, X, vis2, mask_eff, ray_diff, rgb_in};
+  g_view_cap_on = G || nvalid || X || vis2 || mask_eff || ray_diff || rgb_in;
+}
+
+// bf16 tile image with KG k-groups -> fp32 rows of 8 KG columns (the inverse of rows_to_image_kernel): image row
+// p VP + v becomes output row p V + v for v < V, so view slots become view rows and padding slots are dropped
+__global__ void image_to_rows_kernel(const uint8_t* __restrict__ img, int KG, long long P, int V, int VP,
+                                     float* __restrict__ dst) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= P * V * KG) return;
+  const int kg = (int)(e % KG);
+  const long long row = e / KG, p = row / V;
+  const int v = (int)(row % V);
+  const uint4 u = *reinterpret_cast<const uint4*>(img + fe::tile_image_off(p * VP + v, kg, KG));
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+  float* o = dst + row * KG * 8 + 8 * kg;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    o[2 * j] = __uint_as_float(w[j] << 16);
+    o[2 * j + 1] = __uint_as_float(w[j] & 0xffff0000u);
+  }
+}
+
+// copies one chunk's per-view outputs (points [p0, p0 + P)) into the capture buffers
+static int capture_view_outputs(const ViewFusedArgs& va, long long p0, long long P, int V, cudaStream_t st) {
+  const ViewCapture& c = g_view_cap;
+  const long long M = P * V, m0 = p0 * V;
+  const int VP = V <= 8 ? 8 : 16;
+  if (c.G) {
+    image_to_rows_kernel<<<cdiv(P * 34, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(va.G), 34, P, 1, 1,
+                                                            c.G + p0 * kGStride);
+    DYN_LAUNCH_CHECK();
+  }
+  if (c.X && va.X) {
+    image_to_rows_kernel<<<cdiv(M * 16, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(va.X), 16, P, V, VP,
+                                                            c.X + m0 * 128);
+    DYN_LAUNCH_CHECK();
+  }
+  auto copy = [&](float* dst, const float* src, long long n) -> int {
+    if (dst && src) DYN_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return DYN_OK;
+  };
+  RUN(copy(c.nvalid ? c.nvalid + p0 : nullptr, va.nvalid, P));
+  RUN(copy(c.vis2 ? c.vis2 + m0 : nullptr, va.vis2, M));
+  RUN(copy(c.mask_eff ? c.mask_eff + m0 : nullptr, va.mask_eff, M));
+  RUN(copy(c.ray_diff ? c.ray_diff + m0 * 4 : nullptr, va.ray_diff, M * 4));
+  RUN(copy(c.rgb_in ? c.rgb_in + m0 * 3 : nullptr, va.rgb_in, M * 3));
+  return DYN_OK;
+}
+
 static int fill_view_args(ViewFusedArgs* a, const float* query_cam, const float* src_rgbs,
                           const float* src_cams, const void* feat_cl, int V, int S, int H, int W,
                           int h, int w, cudaStream_t st) {
@@ -984,6 +1044,7 @@ int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, con
     va.X = d.X; va.vis2 = d.vis2; va.ray_diff = d.rd; va.rgb_in = d.rgbin;
     va.dbg = view_dbg_ptr();
     RUN(launch_view_fused(n, va, V, st));
+    if (g_view_cap_on) RUN(capture_view_outputs(va, p0, P, V, st));
     {
       Point2Args p2;
       memset(&p2, 0, sizeof(p2));
@@ -1025,6 +1086,7 @@ int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, 
     va.G = d.G; va.nvalid = d.t.nvalid; va.mask_proj = mask_out + p0 * V; va.mask_eff = nullptr;
     va.X = nullptr; va.vis2 = nullptr; va.ray_diff = nullptr; va.rgb_in = nullptr;
     RUN(launch_view_fused(n, va, V, st));
+    if (g_view_cap_on) RUN(capture_view_outputs(va, p0, P, V, st));
     {
       Point2Args p2;
       memset(&p2, 0, sizeof(p2));

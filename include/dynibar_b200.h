@@ -399,6 +399,17 @@ void dyn_debug_set_view_kernel(int which);
  * boundaries, then per warpgroup its lifetime ([128 + wg]) and the cycles it waited for weights ([130 + wg]). */
 void dyn_debug_set_view_timestamps(long long* dev_buf);
 
+/* unit-test hook: while any pointer is set, every dyn_net_static_fused / dyn_net_dynamic_fused call copies the
+ * outputs of the fused per-view stage (the kernel dyn_debug_set_view_kernel selects) into these DEVICE buffers,
+ * chunk by chunk at the chunk's row offset, before the per-point stage runs on them (P = R*S points, V views):
+ *   G [P, 272]: pooled mean 0..127 | variance 128..255 | mean pooling weight 256 | 0 | bias columns 264, 265 = 1
+ *     (fp32 copy of the bf16 operand of geometry_fc);  nvalid [P]: valid views per point;
+ *   static net only: X [P, V, 128] per-view features after the visibility residual (bf16 values as fp32),
+ *     vis2 [P, V], mask_eff [P, V] (projector mask after the mask_rgb test), ray_diff [P, V, 4], rgb_in [P, V, 3].
+ * Any pointer may be NULL (not captured); all NULL turns the hook off. */
+void dyn_debug_set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff,
+                                float* ray_diff, float* rgb_in);
+
 /* ---- building block: one nn.Linear on the tensor cores -----------------------
  * Y[M,N] = act(X[M,K] W[N,K]^T + b) with bf16 operands / fp32 accumulation
  * (wgmma).  act: 0 none, 1 ELU, 2 ReLU, 3 sigmoid.  N <= 256.  packed_ws must
