@@ -70,6 +70,8 @@ SIGNATURES = {
     "dyn_debug_set_view_kernel": (None, [_i]),
     "dyn_debug_set_view_capture": (None, [_vp] * 7),
     "dyn_debug_point_chain": (_i, [_vp] * 5 + [_i, _i] + [_vp] * 9),
+    "dyn_debug_attention": (_i, [_vp] * 4 + [_i, _i, _vp, _vp]),
+    "dyn_debug_rgb_head": (_i, [_vp] * 8 + [C.c_longlong, _i, _vp, _vp]),
     "dyn_debug_pack_layer": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _f, _i, _vp, _sz, _vp, _vp]),
     "dyn_debug_tile_image_off": (_sz, [C.c_longlong, _i, _i]),
     "dyn_linear_tc_packed_bytes": (_sz, [_i, _i]),

@@ -299,9 +299,24 @@ int dyn_net_dynamic_fused(dyn_net_t net, const float* pts, const float* pts_seq,
 int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid, const float* pts,
                           const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
                           float* O, float* out_a, float* out_b, float* posenc_ws, void* stream) {
-  DYN_CHECK_ARG(net && G && nvalid && g2 && Q && K && V && O && out_a && posenc_ws);
+  DYN_CHECK_ARG(net && net->kind != DYN_NET_MOTION && G && nvalid && g2 && out_a && posenc_ws);
+  DYN_CHECK_ARG(R >= 0 && S >= 1);
   return debug_point_chain(net, G, nvalid, pts, ray_dir, R, S, g2, Q, K, V, O, out_a, out_b, posenc_ws,
                            (cudaStream_t)stream);
+}
+
+int dyn_debug_attention(const float* Q, const float* K, const float* V, const float* nvalid, int R, int S, float* O,
+                        void* stream) {
+  DYN_CHECK_ARG(Q && K && V && nvalid && O && R >= 0 && S >= 1);
+  return debug_attention(Q, K, V, nvalid, R, S, O, (cudaStream_t)stream);
+}
+
+int dyn_debug_rgb_head(dyn_net_t net, const float* X, const float* vis2, const float* ray_diff, const float* mask_eff,
+                       const float* rgb_in, const float* GW, const float* sigma, long long P, int V, float* raw,
+                       void* stream) {
+  DYN_CHECK_ARG(net && net->kind == DYN_NET_STATIC && X && vis2 && ray_diff && mask_eff && rgb_in && GW && sigma);
+  DYN_CHECK_ARG(raw && P >= 0 && V >= 1 && V <= 16);
+  return debug_rgb_head(net, X, vis2, ray_diff, mask_eff, rgb_in, GW, sigma, P, V, raw, (cudaStream_t)stream);
 }
 
 int dyn_debug_pack_layer(const float* W, const float* bias, int N, int Kw, int Npad, int Kpad,

@@ -413,7 +413,10 @@ __global__ void __launch_bounds__(kTwinThreads, 1) point2_twin_kernel(const __gr
       t_ready(c.bar0);
       t_wait(c.bar0, acc_cnt);  // fc (no bias) + residual; LayerNorm (eps 1e-6) statistics via TMEM scratch
       {
-        float sum = 0.f, sq = 0.f;
+        // this twin's 64 columns in one pass, shifted by one of its own values so that a large mean does not
+        // cancel (E[x^2] - mean^2 loses the variance in fp32 then); the twins' (mean, sum of squared
+        // deviations) pairs are combined with the pairwise update of Chan et al.
+        float shift = 0.f, sum = 0.f, sq = 0.f;
 #pragma unroll 1
         for (int half = 0; half < 2; ++half) {
           const int cb = c0 + 32 * half;
@@ -429,19 +432,22 @@ __global__ void __launch_bounds__(kTwinThreads, 1) point2_twin_kernel(const __gr
           for (int i = 0; i < 8; ++i) {
             acc[4 * i] += rs[i].x; acc[4 * i + 1] += rs[i].y; acc[4 * i + 2] += rs[i].z; acc[4 * i + 3] += rs[i].w;
           }
+          if (half == 0) shift = acc[0];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) { sum += acc[i]; sq = fmaf(acc[i], acc[i], sq); }
+          for (int i = 0; i < 32; ++i) {
+            const float d = acc[i] - shift;
+            sum += d;
+            sq = fmaf(d, d, sq);
+          }
           tmem_st32(tacc + 128 + cb, acc);
         }
-        x_sum[tw * 128 + r] = sum;
-        x_sq[tw * 128 + r] = sq;
+        x_sum[tw * 128 + r] = shift + sum * (1.f / 64.f);
+        x_sq[tw * 128 + r] = fmaxf(sq - sum * sum * (1.f / 64.f), 0.f);
         tmem_wait_st();
         pair_sync_tw(pair);
-        sum = x_sum[r] + x_sum[128 + r];
-        sq = x_sq[r] + x_sq[128 + r];
-        const float mean = sum * (1.f / 128.f);
-        const float var = fmaxf(sq * (1.f / 128.f) - mean * mean, 0.f);
-        const float rstd = rsqrtf(var + 1e-6f);
+        const float m0 = x_sum[r], m1 = x_sum[128 + r];
+        const float mean = 0.5f * (m0 + m1), dm = m0 - m1;
+        const float rstd = rsqrtf((x_sq[r] + x_sq[128 + r] + 32.f * dm * dm) * (1.f / 128.f) + 1e-6f);
 #pragma unroll 1
         for (int half = 0; half < 2; ++half) {
           const int cb = c0 + 32 * half;

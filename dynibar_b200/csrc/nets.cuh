@@ -33,6 +33,11 @@ int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, 
 int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, const float* pts,
                       const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
                       float* O, float* out_a, float* out_b, float* posenc_ws, cudaStream_t st);
+int debug_attention(const float* Q, const float* K, const float* V, const float* nvalid, int R, int S, float* O,
+                    cudaStream_t st);
+int debug_rgb_head(const dyn_net* n, const float* X, const float* vis2, const float* ray_diff, const float* mask_eff,
+                   const float* rgb_in, const float* GW, const float* sigma, long long P, int V, float* raw,
+                   cudaStream_t st);
 void set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
                       float* rgb_in);
 // tensor-core ray-transformer attention (attention_tc.cu); S must divide 128

@@ -427,6 +427,30 @@ __global__ void attention_kernel(const void* __restrict__ Q, const void* __restr
   }
 }
 
+// The SIMT kernel runs one thread per query sample in one block per ray, so S is capped by the kernel's
+// block-size limit, which its register count puts below 1024 (queried once per process).
+template <bool BF>
+static int check_simt_attention(int S) {
+  static int max_threads = 0;
+  if (max_threads == 0) {
+    cudaFuncAttributes fa;
+    DYN_CUDA(cudaFuncGetAttributes(&fa, attention_kernel<BF>));
+    max_threads = fa.maxThreadsPerBlock;
+  }
+  if (((S + 31) / 32) * 32 > max_threads)
+    return fail(DYN_E_INVALID, "ray transformer: the SIMT attention kernel supports S <= %d samples per ray (got %d)",
+                max_threads, S);
+  return DYN_OK;
+}
+
+// Whether the ray transformer can run S samples per ray: the fused path's tensor-core kernels take any S that
+// divides 128, everything else (and every S of the staged path) runs on a SIMT kernel.  Every entry point that
+// reaches an attention launch (the nets, the test hooks) checks this once, before it launches anything.
+static int check_attention_samples(int S, bool fused) {
+  if (fused) return attention_tc_supported(S) ? DYN_OK : check_simt_attention<true>(S);
+  return check_simt_attention<false>(S);
+}
+
 // out = LayerNorm(a + resid) * w + b, eps 1e-6 (mlp_network.py:100-102). Warp per row.
 __global__ void resid_ln_kernel(const float* __restrict__ a, const float* __restrict__ resid,
                                 const float* __restrict__ w, const float* __restrict__ b, long long P,
@@ -589,9 +613,8 @@ static int run_point_tail(const dyn_net* n, const Layout& L, const float* G, int
   RUN(run_lin(n, L.wk, L1(n, L.wk, t.G2, t.K, P, ACT_NONE), prec, st));
   RUN(run_lin(n, L.wv, L1(n, L.wv, t.G2, t.V, P, ACT_NONE), prec, st));
   {
-    int threads = ((S + 31) / 32) * 32;
+    int threads = ((S + 31) / 32) * 32;  // S <= the kernel's block limit (check_attention_samples at net entry)
     size_t smem = (size_t)2 * S * 32 * sizeof(float);
-    if (threads > 1024) return fail(DYN_E_INVALID, "ray transformer supports S <= 1024 (got %d)", S);
     if (smem > 48 * 1024)
       DYN_CUDA(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)smem));
@@ -646,6 +669,7 @@ int net_dynamic_f32(const dyn_net* n, const float* pts, const float* rgb_feat, c
                     const float* mask, float time, int R_all, int S, int V, float* raw, void* ws,
                     size_t ws_bytes, int prec, cudaStream_t st, bool train) {
   const DynamicLayout& L = n->dl;
+  RUN(check_attention_samples(S, false));
   const int RC = net_rows_per_chunk(S, V);
   if (train && R_all > RC) return fail(DYN_E_INVALID, "training forward: %d rays exceed one internal chunk (%d)", R_all, RC);
   for (int r0 = 0; r0 < R_all; r0 += RC) {
@@ -700,6 +724,7 @@ int net_static_f32(const dyn_net* n, const float* pts, const float* ref_rays, co
                    const float* rgb_feat, const float* ray_diff, const float* mask, int R_all, int S,
                    int V, float* raw, void* ws, size_t ws_bytes, int prec, cudaStream_t st, bool train) {
   const StaticLayout& L = n->sl;
+  RUN(check_attention_samples(S, false));
   const int RC = net_rows_per_chunk(S, V);
   if (train && R_all > RC) return fail(DYN_E_INVALID, "training forward: %d rays exceed one internal chunk (%d)", R_all, RC);
   for (int r0 = 0; r0 < R_all; r0 += RC) {
@@ -848,8 +873,23 @@ size_t net_fused_workspace(int kind, int R, int S, int V) {
   return fused_alloc(b, kind == DYN_NET_STATIC, R < rc ? R : rc, S, V, &d);
 }
 
+// ray-transformer attention of the fused path on bf16 tile images (16 k-groups): the tensor-core kernels when S
+// divides 128, else the SIMT kernel (one block per ray)
+static int run_attention_fused(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __nv_bfloat16* V,
+                               const float* nvalid, long long P, int R, int S, __nv_bfloat16* O, cudaStream_t st) {
+  if (attention_tc_supported(S)) return launch_attention_tc(Q, K, V, nvalid, P, S, O, st);
+  const int threads = ((S + 31) / 32) * 32;  // S <= the kernel's block limit (check_attention_samples at entry)
+  const size_t smem = (size_t)2 * S * 32 * sizeof(float);
+  if (smem > 48 * 1024)
+    DYN_CUDA(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ProfScope prof(PROF_ATTENTION, st);
+  attention_kernel<true><<<R, threads, smem, st>>>(Q, K, V, nvalid, S, O);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
 // per-point stage on the fused chains: point1 (geometry_fc, Q|K|V) -> ray-transformer
-// attention (tensor cores when S divides 128, else the SIMT kernel) -> point2 (fc + LayerNorm + heads);
+// attention -> point2 (fc + LayerNorm + heads);
 // G, Q, K, V, O are bf16 tile images, g2 / GW use the fp32 tile layout (fused_engine.cuh)
 static int run_point_fused(const dyn_net* n, const float* G, long long P, int R, int S, bool dynamic,
                            float* posenc_tab, TrunkBufs& t, Point2Args& p2, cudaStream_t st) {
@@ -868,38 +908,31 @@ static int run_point_fused(const dyn_net* n, const float* G, long long P, int R,
     p1.posenc = posenc_tab;
   }
   RUN(launch_point1_twin(n, p1, st));
-  if (attention_tc_supported(S)) {
-    RUN(launch_attention_tc(Qb, Kb, Vb, t.nvalid, P, S, Ob, st));
-  } else {
-    int threads = ((S + 31) / 32) * 32;
-    size_t smem = (size_t)2 * S * 32 * sizeof(float);
-    if (threads > 1024) return fail(DYN_E_INVALID, "ray transformer supports S <= 1024 (got %d)", S);
-    if (smem > 48 * 1024)
-      DYN_CUDA(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)smem));
-    ProfScope prof(PROF_ATTENTION, st);
-    attention_kernel<true><<<R, threads, smem, st>>>(Qb, Kb, Vb, t.nvalid, S, Ob);
-    DYN_LAUNCH_CHECK();
-  }
+  RUN(run_attention_fused(Qb, Kb, Vb, t.nvalid, P, R, S, Ob, st));
   p2.O = Ob; p2.g2 = t.G2; p2.nvalid = t.nvalid; p2.P = P; p2.S = S;
   return launch_point2_twin(n, p2, st);
 }
 
-// unit-test hook: the per-point fused stage on caller-provided G / nvalid
-// fp32 rows -> bf16 tile image with KG k-groups (columns >= ncols are zero)
-__global__ void rows_to_image_kernel(const float* __restrict__ src, int ld, int ncols, long long P, int KG,
-                                     uint8_t* __restrict__ img) {
+// ---------------------------------------------------------------------------
+// Unit-test hooks of the per-point stage and the blending head: plain fp32 rows in and out; the tile layouts
+// the fused kernels exchange are converted here (scratch is allocated per call: these entry points are not on
+// the product path).
+// ---------------------------------------------------------------------------
+// fp32 rows of `ld` floats -> bf16 tile image with KG k-groups (columns >= ncols are zero); row p V + v becomes
+// image row p VP + v (V = VP = 1: row for row; the blending head's view slots otherwise)
+__global__ void rows_to_image_kernel(const float* __restrict__ src, int ld, int ncols, long long P, int V, int VP,
+                                     int KG, uint8_t* __restrict__ img) {
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= P * KG) return;
-  const long long row = e / KG;
-  const int kg = (int)(e % KG);
-  float v[8];
+  if (e >= P * V * KG) return;
+  const long long row = e / KG, p = row / V;
+  const int kg = (int)(e % KG), v = (int)(row % V);
+  float v8[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = (8 * kg + i < ncols) ? src[row * ld + 8 * kg + i] : 0.f;
-  if (KG == 34 && kg == 33) { v[0] = 1.f; v[1] = 1.f; }  // bias columns of the geometry_fc layers (chains_twin.cu)
-  *reinterpret_cast<uint4*>(img + fe::tile_image_off(row, kg, KG)) =
-      make_uint4(fe::pack_bf16x2(v[0], v[1]), fe::pack_bf16x2(v[2], v[3]), fe::pack_bf16x2(v[4], v[5]),
-                 fe::pack_bf16x2(v[6], v[7]));
+  for (int i = 0; i < 8; ++i) v8[i] = (8 * kg + i < ncols) ? src[row * ld + 8 * kg + i] : 0.f;
+  if (KG == 34 && kg == 33) { v8[0] = 1.f; v8[1] = 1.f; }  // bias columns of the geometry_fc layers (chains_twin.cu)
+  *reinterpret_cast<uint4*>(img + fe::tile_image_off(p * VP + v, kg, KG)) =
+      make_uint4(fe::pack_bf16x2(v8[0], v8[1]), fe::pack_bf16x2(v8[2], v8[3]), fe::pack_bf16x2(v8[4], v8[5]),
+                 fe::pack_bf16x2(v8[6], v8[7]));
 }
 // fp32 tile layout (tile_f32_off) -> fp32 rows [P,128]
 __global__ void tile_f32_to_rows_kernel(const uint8_t* __restrict__ src, long long P, float* __restrict__ dst) {
@@ -909,58 +942,14 @@ __global__ void tile_f32_to_rows_kernel(const uint8_t* __restrict__ src, long lo
   const int cg = (int)(e & 31);
   reinterpret_cast<float4*>(dst)[row * 32 + cg] = *reinterpret_cast<const float4*>(src + fe::tile_f32_off(row, cg));
 }
-
-// Unit-test hook: plain fp32 rows in and out; the tile layouts the fused kernels exchange are
-// converted here (scratch is allocated per call: this entry point is not on the product path).
-// The Q, K, V, O arguments are ignored (those intermediates live in tile-image scratch).
-int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, const float* pts,
-                      const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
-                      float* O, float* out_a, float* out_b, float* posenc_ws, cudaStream_t st) {
-  (void)Q; (void)K; (void)V; (void)O;
-  const long long P = (long long)R * S;
-  if (P == 0) return DYN_OK;
-  const long long Pt = ((P + 255) / 256) * 256;
-  const size_t g_bytes = fe::tile_image_bytes(Pt, 34), t_bytes = (size_t)Pt * 512;
-  uint8_t* scratch = nullptr;
-  DYN_CUDA(cudaMalloc(&scratch, g_bytes + 6 * t_bytes));
-  DYN_CUDA(cudaMemsetAsync(scratch, 0, g_bytes + 6 * t_bytes, st));
-  uint8_t* gimg = scratch;
-  float* buf[6];
-  for (int i = 0; i < 6; ++i) buf[i] = reinterpret_cast<float*>(scratch + g_bytes + (size_t)i * t_bytes);
-  rows_to_image_kernel<<<cdiv(P * 34, 256), 256, 0, st>>>(G, kGStride, 257, P, 34, gimg);
-  TrunkBufs t;
-  memset(&t, 0, sizeof(t));
-  t.G2 = buf[0]; t.Q = buf[1]; t.K = buf[2]; t.V = buf[3]; t.O = buf[4]; t.nvalid = const_cast<float*>(nvalid);
-  Point2Args p2;
-  memset(&p2, 0, sizeof(p2));
-  const bool dynamic = n->kind == DYN_NET_DYNAMIC;
-  if (dynamic) { p2.pts = pts; p2.ray_dir = ray_dir; p2.raw = out_a; }
-  else { p2.GW = buf[5]; p2.sigma = out_b; }
-  int rc = run_point_fused(n, reinterpret_cast<const float*>(gimg), P, R, S, dynamic, posenc_ws, t, p2, st);
-  if (rc == DYN_OK) {
-    tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[0]), P, g2);
-    if (!dynamic)
-      tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[5]), P, out_a);
-  }
-  cudaStreamSynchronize(st);
-  cudaFree(scratch);
-  return rc;
+// fp32 rows [P,128] -> fp32 tile layout
+__global__ void rows_to_tile_f32_kernel(const float* __restrict__ src, long long P, uint8_t* __restrict__ dst) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= P * 32) return;
+  const long long row = e >> 5;
+  const int cg = (int)(e & 31);
+  *reinterpret_cast<float4*>(dst + fe::tile_f32_off(row, cg)) = reinterpret_cast<const float4*>(src)[row * 32 + cg];
 }
-
-// Unit-test hook (dyn_debug_set_view_capture): the per-view stage's outputs of every internal chunk, unpacked
-// into caller buffers at the chunk's row offset.  Off (all NULL) on the product path.
-struct ViewCapture {
-  float *G, *nvalid, *X, *vis2, *mask_eff, *ray_diff, *rgb_in;
-};
-static ViewCapture g_view_cap = {};
-static bool g_view_cap_on = false;
-
-void set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
-                      float* rgb_in) {
-  g_view_cap = ViewCapture{G, nvalid, X, vis2, mask_eff, ray_diff, rgb_in};
-  g_view_cap_on = G || nvalid || X || vis2 || mask_eff || ray_diff || rgb_in;
-}
-
 // bf16 tile image with KG k-groups -> fp32 rows of 8 KG columns (the inverse of rows_to_image_kernel): image row
 // p VP + v becomes output row p V + v for v < V, so view slots become view rows and padding slots are dropped
 __global__ void image_to_rows_kernel(const uint8_t* __restrict__ img, int KG, long long P, int V, int VP,
@@ -978,6 +967,115 @@ __global__ void image_to_rows_kernel(const uint8_t* __restrict__ img, int KG, lo
     o[2 * j] = __uint_as_float(w[j] << 16);
     o[2 * j + 1] = __uint_as_float(w[j] & 0xffff0000u);
   }
+}
+
+// bf16 tile image (16 k-groups) -> fp32 rows [P,128], when the caller asked for them
+static int image_rows_out(const void* img, long long P, float* dst, cudaStream_t st) {
+  if (!dst) return DYN_OK;
+  image_to_rows_kernel<<<cdiv(P * 16, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(img), 16, P, 1, 1, dst);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+// The per-point fused stage on caller-provided G / nvalid; Q, K, V, O (any may be NULL) receive the bf16 values
+// the kernels exchanged.
+int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, const float* pts,
+                      const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
+                      float* O, float* out_a, float* out_b, float* posenc_ws, cudaStream_t st) {
+  RUN(check_attention_samples(S, true));
+  const long long P = (long long)R * S;
+  if (P == 0) return DYN_OK;
+  const long long Pt = ((P + 255) / 256) * 256;
+  const size_t g_bytes = fe::tile_image_bytes(Pt, 34), t_bytes = (size_t)Pt * 512;
+  uint8_t* scratch = nullptr;
+  DYN_CUDA(cudaMalloc(&scratch, g_bytes + 6 * t_bytes));
+  DYN_CUDA(cudaMemsetAsync(scratch, 0, g_bytes + 6 * t_bytes, st));
+  uint8_t* gimg = scratch;
+  float* buf[6];
+  for (int i = 0; i < 6; ++i) buf[i] = reinterpret_cast<float*>(scratch + g_bytes + (size_t)i * t_bytes);
+  rows_to_image_kernel<<<cdiv(P * 34, 256), 256, 0, st>>>(G, kGStride, 257, P, 1, 1, 34, gimg);
+  TrunkBufs t;
+  memset(&t, 0, sizeof(t));
+  t.G2 = buf[0]; t.Q = buf[1]; t.K = buf[2]; t.V = buf[3]; t.O = buf[4]; t.nvalid = const_cast<float*>(nvalid);
+  Point2Args p2;
+  memset(&p2, 0, sizeof(p2));
+  const bool dynamic = n->kind == DYN_NET_DYNAMIC;
+  if (dynamic) { p2.pts = pts; p2.ray_dir = ray_dir; p2.raw = out_a; }
+  else { p2.GW = buf[5]; p2.sigma = out_b; }
+  int rc = run_point_fused(n, reinterpret_cast<const float*>(gimg), P, R, S, dynamic, posenc_ws, t, p2, st);
+  if (rc == DYN_OK) {
+    tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[0]), P, g2);
+    if (!dynamic)
+      tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[5]), P, out_a);
+    const float* img[4] = {t.Q, t.K, t.V, t.O};
+    float* dst[4] = {Q, K, V, O};
+    for (int i = 0; i < 4 && rc == DYN_OK; ++i) rc = image_rows_out(img[i], P, dst[i], st);
+  }
+  cudaStreamSynchronize(st);
+  cudaFree(scratch);
+  return rc;
+}
+
+// The fused path's ray-transformer attention (run_attention_fused) on caller-provided Q, K, V [P,128] fp32 rows
+// (rounded to bf16 as the kernels read them) -> O [P,128] (bf16 values).
+int debug_attention(const float* Q, const float* K, const float* V, const float* nvalid, int R, int S, float* O,
+                    cudaStream_t st) {
+  RUN(check_attention_samples(S, true));
+  const long long P = (long long)R * S;
+  if (P == 0) return DYN_OK;
+  const size_t t_bytes = fe::tile_image_bytes(P, 16);
+  uint8_t* scratch = nullptr;
+  DYN_CUDA(cudaMalloc(&scratch, 4 * t_bytes));
+  DYN_CUDA(cudaMemsetAsync(scratch, 0, 4 * t_bytes, st));
+  const float* src[3] = {Q, K, V};
+  for (int i = 0; i < 3; ++i)
+    rows_to_image_kernel<<<cdiv(P * 16, 256), 256, 0, st>>>(src[i], 128, 128, P, 1, 1, 16, scratch + i * t_bytes);
+  auto img = [&](int i) { return reinterpret_cast<__nv_bfloat16*>(scratch + i * t_bytes); };
+  int rc = run_attention_fused(img(0), img(1), img(2), nvalid, P, R, S, img(3), st);
+  if (rc == DYN_OK) rc = image_rows_out(img(3), P, O, st);
+  cudaStreamSynchronize(st);
+  cudaFree(scratch);
+  return rc;
+}
+
+// The static blending head (launch_rgbhead_twin) on per-view rows in the layout dyn_debug_set_view_capture
+// produces: X [P,V,128] goes into the view-slot bf16 tile image (padding slots zero, whole 256-row iterations
+// as in fused_alloc), GW [P,128] into the fp32 tile layout.
+int debug_rgb_head(const dyn_net* n, const float* X, const float* vis2, const float* ray_diff, const float* mask_eff,
+                   const float* rgb_in, const float* GW, const float* sigma, long long P, int V, float* raw,
+                   cudaStream_t st) {
+  if (P == 0) return DYN_OK;
+  const int VP = V <= 8 ? 8 : 16;
+  const long long slots = ((P * VP + 255) / 256) * 256;
+  const size_t x_bytes = (size_t)slots * 256, gw_bytes = (size_t)((P + 127) / 128) * 65536;
+  uint8_t* scratch = nullptr;
+  DYN_CUDA(cudaMalloc(&scratch, x_bytes + gw_bytes));
+  DYN_CUDA(cudaMemsetAsync(scratch, 0, x_bytes + gw_bytes, st));
+  rows_to_image_kernel<<<cdiv(P * V * 16, 256), 256, 0, st>>>(X, 128, 128, P, V, VP, 16, scratch);
+  rows_to_tile_f32_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(GW, P, scratch + x_bytes);
+  RgbHeadArgs rh;
+  memset(&rh, 0, sizeof(rh));
+  rh.X = reinterpret_cast<const float*>(scratch); rh.vis2 = vis2; rh.ray_diff = ray_diff; rh.mask_eff = mask_eff;
+  rh.rgb_in = rgb_in; rh.GW = reinterpret_cast<const float*>(scratch + x_bytes); rh.sigma = sigma;
+  rh.P = P; rh.V = V; rh.raw = raw;
+  const int rc = launch_rgbhead_twin(n, rh, st);
+  cudaStreamSynchronize(st);
+  cudaFree(scratch);
+  return rc;
+}
+
+// Unit-test hook (dyn_debug_set_view_capture): the per-view stage's outputs of every internal chunk, unpacked
+// into caller buffers at the chunk's row offset.  Off (all NULL) on the product path.
+struct ViewCapture {
+  float *G, *nvalid, *X, *vis2, *mask_eff, *ray_diff, *rgb_in;
+};
+static ViewCapture g_view_cap = {};
+static bool g_view_cap_on = false;
+
+void set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
+                      float* rgb_in) {
+  g_view_cap = ViewCapture{G, nvalid, X, vis2, mask_eff, ray_diff, rgb_in};
+  g_view_cap_on = G || nvalid || X || vis2 || mask_eff || ray_diff || rgb_in;
 }
 
 // copies one chunk's per-view outputs (points [p0, p0 + P)) into the capture buffers
@@ -1024,6 +1122,7 @@ int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, con
                      float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st) {
   const StaticLayout& L = n->sl;
   const int prec = DYN_PREC_BF16;
+  RUN(check_attention_samples(S, true));
   ViewFusedArgs va{};
   RUN(fill_view_args(&va, query_cam, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st));
   const int RC = net_rows_per_chunk(S, V);
@@ -1068,6 +1167,7 @@ int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, 
                       int w, float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st) {
   const DynamicLayout& L = n->dl;
   const int prec = DYN_PREC_BF16;
+  RUN(check_attention_samples(S, true));
   ViewFusedArgs va{};
   RUN(fill_view_args(&va, query_cam, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st));
   const long long P_all = (long long)R_all * S;

@@ -358,8 +358,8 @@ int dyn_encoder_forward(const float* params, size_t n_params, const float* image
 /* ---- unit-test hook: the fused per-point stage (geometry_fc -> ray transformer
  * -> heads; mlp_network.py:283-315 / :496-506) on caller-provided pooled
  * features G [R*S, 272] (257 used) and nvalid [R*S].  Outputs g2 [R*S,128] (plain
- * fp32 rows; the Q, K, V, O arguments are ignored: those intermediates live in
- * the kernels' internal tile-image scratch); dynamic net: out_a = raw [R*S,4]; static net:
+ * fp32 rows); Q, K, V, O [R*S,128]: the bf16 values the kernels exchanged, as fp32 rows
+ * (each may be NULL: not written); dynamic net: out_a = raw [R*S,4]; static net:
  * out_a = per-point part of rgb_fc.0 [R*S,128], out_b = masked sigma [R*S].
  * posenc_ws: S*128 floats of scratch. */
 int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid,
@@ -367,6 +367,18 @@ int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid,
                           float* g2, float* Q, float* K, float* V, float* O,
                           float* out_a, float* out_b, float* posenc_ws,
                           void* stream);
+/* unit-test hook: the fused path's ray-transformer attention (the kernel the product picks for S) on
+ * caller-provided Q, K, V [R*S,128] fp32 rows, which are rounded to bf16 as the kernels read them, and
+ * nvalid [R*S] -> O [R*S,128] (bf16 values as fp32).  S the kernels cannot run fails with DYN_E_INVALID. */
+int dyn_debug_attention(const float* Q, const float* K, const float* V, const float* nvalid,
+                        int R, int S, float* O, void* stream);
+/* unit-test hook: the static net's per-view blending head and masked softmax over views on rows in the
+ * layout dyn_debug_set_view_capture produces: X [P,V,128] (rounded to bf16), vis2, mask_eff [P,V],
+ * ray_diff [P,V,4], rgb_in [P,V,3], GW [P,128] (per-point part of rgb_fc.0, bias included), sigma [P]
+ * -> raw [P,4] = blended rgb | sigma.  V <= 16. */
+int dyn_debug_rgb_head(dyn_net_t net, const float* X, const float* vis2, const float* ray_diff,
+                       const float* mask_eff, const float* rgb_in, const float* GW,
+                       const float* sigma, long long P, int V, float* raw, void* stream);
 
 /* ---- unit-test hook (HOST only, no GPU needed): pack one nn.Linear [N, Kw] into the bf16
  * wgmma weight image the fused kernels stream (dynibar_b200/csrc/fused_engine.cuh:

@@ -188,78 +188,6 @@ def test_fused_view_stage_matches_staged(golden, name):
                       max_bad_frac=5e-3)
 
 
-@pytest.mark.parametrize("kind", ["dynamic", "static"])
-@pytest.mark.parametrize("S,R", [(64, 37), (128, 37), (20, 37), (16, 37), (32, 37), (64, 1301), (128, 701)])
-def test_fused_point_stage(kind, S, R):
-  """point1 (geometry_fc, Q|K|V) -> attention -> point2 (fc + LayerNorm + heads) on random
-  pooled features, against the oracle's formulas with bf16 GEMM operands.  The two large R give every
-  CTA of the persistent kernels several tiles (the attention kernel's next-tile prefetch path)."""
-  from dynibar_b200 import _lib, weights
-  torch.manual_seed(S)
-  P = R * S
-  model, args = synthetic.make_model(S, 0, mono=True, seed=4)
-  mod = model.net_coarse_dy if kind == "dynamic" else model.net_coarse_st
-  w = orc._sd(mod)
-  G = torch.zeros(P, 272)
-  G[:, :257] = torch.randn(P, 257) * 0.5
-  G[:, 128:256] = G[:, 128:256].abs() * 0.2
-  nvalid = torch.randint(0, 4, (P,)).float()
-  pts = torch.randn(P, 3) * 3
-  ray_dir = torch.nn.functional.normalize(torch.randn(R, 3), dim=-1)
-  # ---- oracle (fp32) ----
-  orc.set_gemm_mode("bf16")
-  try:
-    g = orc._elu(orc._lin(orc._elu(orc._lin(G[:, :257], w["geometry_fc.0.weight"], w["geometry_fc.0.bias"])),
-                          w["geometry_fc.2.weight"], w["geometry_fc.2.bias"])).reshape(R, S, 128)
-    if kind == "dynamic":
-      g = g + orc.sinusoid_table(S)[None]
-    g3 = orc.ray_attention(w, g, (nvalid.reshape(R, S) > 1).float())
-    if kind == "dynamic":
-      h = torch.cat([g3, orc.periodic_embed(pts.reshape(R, S, 3), 5)], -1)
-      h = orc._elu(orc._lin(orc._elu(orc._lin(h, w["ref_pts_fc.0.weight"], w["ref_pts_fc.0.bias"])),
-                            w["ref_pts_fc.2.weight"], w["ref_pts_fc.2.bias"]))
-    else:
-      h = g3
-    sigma = orc._lin(orc._elu(orc._lin(h, w["out_geometry_fc.0.weight"], w["out_geometry_fc.0.bias"])),
-                     w["out_geometry_fc.2.weight"], w["out_geometry_fc.2.bias"])[..., 0]
-    if kind == "dynamic":
-      hh = torch.cat([h, orc.periodic_embed(ray_dir, 4)[:, None, :].expand(-1, S, -1)], -1)
-      hh = orc._elu(orc._lin(hh, w["rgb_fc.0.weight"], w["rgb_fc.0.bias"]))
-      hh = orc._elu(orc._lin(hh, w["rgb_fc.2.weight"], w["rgb_fc.2.bias"]))
-      rgb = torch.sigmoid(orc._lin(hh, w["rgb_fc.4.weight"], w["rgb_fc.4.bias"]))
-    else:
-      gw = orc._lin(h, w["rgb_fc.0.weight"][:, :128], w["rgb_fc.0.bias"])
-  finally:
-    orc.set_gemm_mode("fp32")
-  # ---- library ----
-  mod = mod.to(DEV)
-  net = weights.packed_of(mod, torch.device(DEV))
-  d = lambda x: x.to(DEV).contiguous()
-  bufs = [torch.zeros(P, 128, device=DEV) for _ in range(5)]
-  out_a = torch.zeros(P, 128 if kind == "static" else 4, device=DEV)
-  out_b = torch.zeros(P, device=DEV)
-  pws = torch.zeros(S * 128, device=DEV)
-  Gd, nvd, ptd, rdd = d(G), d(nvalid), d(pts), d(ray_dir)
-  _lib.check(_lib.lib.dyn_debug_point_chain(net.handle, Gd.data_ptr(), nvd.data_ptr(), ptd.data_ptr(),
-                                            rdd.data_ptr(), R, S, *[b.data_ptr() for b in bufs],
-                                            out_a.data_ptr(), out_b.data_ptr(), pws.data_ptr(),
-                                            _lib.stream()))
-  torch.cuda.synchronize()
-  g2 = bufs[0].cpu().reshape(R, S, 128)
-  assert_close_frac("g2", g2, g, rtol=2e-2, atol=2e-2, max_bad_frac=1e-3)
-  ok = (nvalid >= 1)
-  if kind == "dynamic":
-    raw = out_a.cpu()
-    assert_close_frac("sigma", raw[:, 3][ok], (sigma.reshape(-1) - mod.shift)[ok], rtol=0, atol=2e-2,
-                      max_bad_frac=2e-3)
-    assert (raw[:, 3][~ok] == -1e9).all() and (raw[:, :3][~ok] == 0).all()
-    assert_close_frac("rgb", raw[:, :3][ok], rgb.reshape(-1, 3)[ok], rtol=0, atol=1e-2, max_bad_frac=2e-3)
-  else:
-    assert_close_frac("GW", out_a.cpu(), gw.reshape(-1, 128), rtol=2e-2, atol=3e-2, max_bad_frac=2e-3)
-    assert_close_frac("sigma", out_b.cpu()[ok], sigma.reshape(-1)[ok], rtol=0, atol=2e-2, max_bad_frac=2e-3)
-    assert (out_b.cpu()[~ok] == -1e9).all()
-
-
 def _run_mode(cfg, precision, mono=False):
   from dynibar_b200 import render_ray as rr
   from dynibar_b200.projection import Projector
