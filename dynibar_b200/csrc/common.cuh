@@ -121,9 +121,9 @@ struct dyn_net {
   dyn::MotionLayout ml;
   // MotionMLP in one fused kernel (motion_fused.cu): motion net only
   dyn::ChainImage motion;
-  // row-local chains of the aggregation nets (chains_twin.cu): [0] point stage 1, [1] point stage 2,
+  // row-local chains of the aggregation nets (chains_wg.cu): [0] point stage 1, [1] point stage 2,
   // [2] static blending head
-  dyn::ChainImage chain_tw[3];
+  dyn::ChainImage chain[3];
   // twin-warp per-view stage (view_twin.cu): weight images in its column layout
   dyn::ChainImage twin;
   // warpgroup per-view stage (view_wg.cu): full-width weight chunks in consumption order

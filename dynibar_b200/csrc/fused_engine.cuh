@@ -1,4 +1,4 @@
-// Shared machinery of the fused tensor-core kernels (nets_fused.cu, motion_fused.cu, chains_twin.cu,
+// Shared machinery of the fused tensor-core kernels (nets_fused.cu, motion_fused.cu, chains_wg.cu,
 // view_*.cu): smem budget constants, fast activations, A-tile stores, view-group shuffles, the
 // table-driven weight producer and MMA warpgroup, and the host-side packing of weight chunks into
 // wgmma B-operand images.
@@ -43,19 +43,6 @@ __device__ __forceinline__ float elu_from_log2(float x2) {
 }
 __device__ __forceinline__ float sigmoid_fast(float x) {
   return __frcp_rn(1.f + ex2f(-x * 1.4426950408889634f));
-}
-
-// Software-pipelined accumulator read-out: NH half-blocks of 16 columns; the load of half h + 1 is issued
-// before fn(h, values) processes half h.  colf(h) = accumulator column of half h.
-template <int NH, class ColFn, class Fn>
-__device__ __forceinline__ void tmem_pipe16(uint32_t tacc, ColFn colf, Fn fn) {
-  float buf[2][16];
-  tmem_ld16(tacc + colf(0), buf[0]);
-#pragma unroll
-  for (int h = 0; h < NH; ++h) {
-    if (h + 1 < NH) tmem_ld16(tacc + colf(h + 1), buf[(h + 1) & 1]);
-    fn(h, buf[h & 1]);
-  }
 }
 
 // 8 consecutive columns [c0, c0+8) of this thread's row -> one 16-byte store

@@ -907,10 +907,10 @@ static int run_point_fused(const dyn_net* n, const float* G, long long P, int R,
     DYN_LAUNCH_CHECK();
     p1.posenc = posenc_tab;
   }
-  RUN(launch_point1_twin(n, p1, st));
+  RUN(launch_point1_wg(n, p1, st));
   RUN(run_attention_fused(Qb, Kb, Vb, t.nvalid, P, R, S, Ob, st));
   p2.O = Ob; p2.g2 = t.G2; p2.nvalid = t.nvalid; p2.P = P; p2.S = S;
-  return launch_point2_twin(n, p2, st);
+  return launch_point2_wg(n, p2, st);
 }
 
 // ---------------------------------------------------------------------------
@@ -929,7 +929,7 @@ __global__ void rows_to_image_kernel(const float* __restrict__ src, int ld, int 
   float v8[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) v8[i] = (8 * kg + i < ncols) ? src[row * ld + 8 * kg + i] : 0.f;
-  if (KG == 34 && kg == 33) { v8[0] = 1.f; v8[1] = 1.f; }  // bias columns of the geometry_fc layers (chains_twin.cu)
+  if (KG == 34 && kg == 33) { v8[0] = 1.f; v8[1] = 1.f; }  // bias columns of the geometry_fc layers (chains_wg.cu)
   *reinterpret_cast<uint4*>(img + fe::tile_image_off(p * VP + v, kg, KG)) =
       make_uint4(fe::pack_bf16x2(v8[0], v8[1]), fe::pack_bf16x2(v8[2], v8[3]), fe::pack_bf16x2(v8[4], v8[5]),
                  fe::pack_bf16x2(v8[6], v8[7]));
@@ -1038,7 +1038,7 @@ int debug_attention(const float* Q, const float* K, const float* V, const float*
   return rc;
 }
 
-// The static blending head (launch_rgbhead_twin) on per-view rows in the layout dyn_debug_set_view_capture
+// The static blending head (launch_rgbhead_wg) on per-view rows in the layout dyn_debug_set_view_capture
 // produces: X [P,V,128] goes into the view-slot bf16 tile image (padding slots zero, whole 256-row iterations
 // as in fused_alloc), GW [P,128] into the fp32 tile layout.
 int debug_rgb_head(const dyn_net* n, const float* X, const float* vis2, const float* ray_diff, const float* mask_eff,
@@ -1058,7 +1058,7 @@ int debug_rgb_head(const dyn_net* n, const float* X, const float* vis2, const fl
   rh.X = reinterpret_cast<const float*>(scratch); rh.vis2 = vis2; rh.ray_diff = ray_diff; rh.mask_eff = mask_eff;
   rh.rgb_in = rgb_in; rh.GW = reinterpret_cast<const float*>(scratch + x_bytes); rh.sigma = sigma;
   rh.P = P; rh.V = V; rh.raw = raw;
-  const int rc = launch_rgbhead_twin(n, rh, st);
+  const int rc = launch_rgbhead_wg(n, rh, st);
   cudaStreamSynchronize(st);
   cudaFree(scratch);
   return rc;
@@ -1154,7 +1154,7 @@ int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, con
       memset(&rh, 0, sizeof(rh));
       rh.X = d.X; rh.vis2 = d.vis2; rh.ray_diff = d.rd; rh.mask_eff = d.meff; rh.rgb_in = d.rgbin;
       rh.GW = d.ch; rh.sigma = d.sig; rh.P = P; rh.V = V; rh.raw = raw + p0 * 4;
-      RUN(launch_rgbhead_twin(n, rh, st));
+      RUN(launch_rgbhead_wg(n, rh, st));
     }
     (void)prec; (void)M;
   }

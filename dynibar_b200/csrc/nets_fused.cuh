@@ -67,7 +67,7 @@ struct MotionFusedArgs {
   int nchunks;
 };
 
-// ---- row-local twin-warp chains (chains_twin.cu) ----
+// ---- row-local chains of the aggregation nets (chains_wg.cu) ----
 struct Point1Args {
   const float* G;       // [P, kGStride]
   const float* posenc;  // [S,128] sinusoid table (dynamic) or null
@@ -120,12 +120,13 @@ size_t motion_fused_bytes();
 int motion_fused_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_motion_fused(const dyn_net* n, MotionFusedArgs& a, cudaStream_t st);
 
-// the point stages and the static blending head (chains_twin.cu)
-size_t twin_chain_bytes(int kind);
-int twin_chain_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
-int launch_point1_twin(const dyn_net* n, Point1Args& a, cudaStream_t st);
-int launch_point2_twin(const dyn_net* n, Point2Args& a, cudaStream_t st);
-int launch_rgbhead_twin(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st);
+// the point stages and the static blending head (chains_wg.cu): accumulators in registers, two 64-row
+// warpgroups per CTA
+size_t chain_wg_bytes(int kind);
+int chain_wg_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
+int launch_point1_wg(const dyn_net* n, Point1Args& a, cudaStream_t st);
+int launch_point2_wg(const dyn_net* n, Point2Args& a, cudaStream_t st);
+int launch_rgbhead_wg(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st);
 
 // twin-warp per-view stage (view_twin.cu)
 size_t view_twin_bytes(int kind);

@@ -7,39 +7,25 @@
 //   pooling weights, weighted mean/var over views -> base_fc.0 (SS, N = 256)
 //   base_fc.2 -> vis_fc.0 -> vis_fc.2 -> vis_fc2.0 (RS, N = 128), visibility logits, second pooling -> G
 //
-// One persistent CTA per SM: two consumer warpgroups and one producer warp.  Each consumer warpgroup owns
-// 64 rows (view slots) of the CTA's 128-row iteration and issues its own wgmmas, one instruction per k-step
-// for the whole layer width.  The accumulators stay in registers: the warps that issue a layer run its
-// epilogue on the fragments, and a hidden layer's output, packed to bf16 pairs, is the register A operand of
-// the next layer (tc::acc_to_afrag), so only the two front-end operands (positional encodings, pooled
-// features) go through shared memory.  While one warpgroup runs an epilogue, the other's wgmmas keep the
-// tensor cores busy.  Both warpgroups consume the same weight chunks from one ring; a slot is refilled only
-// when both have retired it, so the weights are fetched once per 128 rows.
-//
-// Fragment layout (warp w of the warpgroup, lane l, q = l % 4): accumulator i holds row 16 w + l / 4 + 8 h,
-// column 8 j + 2 q + e with j = i / 4, h = (i / 2) % 2, e = i % 2.  A row's dot products are quad shuffles
-// (xor 1, 2); a point's view slots are 8 or 16 aligned rows of one warp's 16-row slab, so sums over its views
-// are shuffles over the row lanes (xor 4, 8, 16) plus, for 16 slots, the in-thread h pair.
+// Built on the warpgroup engine (wg_engine.cuh): each consumer warpgroup owns 64 rows (view slots) of the CTA's
+// 128-row iteration, accumulators stay in registers, and only the two front-end operands (positional encodings,
+// pooled features) go through shared memory.  While one warpgroup runs an epilogue, the other's wgmmas keep the
+// tensor cores busy.  A point's view slots are 8 or 16 aligned rows of one warp's 16-row slab, so sums over its
+// views are shuffles over the row lanes (wg_engine.cuh: views_sum).
 // The front end (projection, gather, first pooling of the gathered channels) runs with two threads per row,
 // as in view_twin.cu: warps 0-1 of a warpgroup ("twin 0") and 2-3 ("twin 1") each take half of the channels.
-#include "fused_engine.cuh"
 #include "geometry.cuh"
 #include "nets.cuh"
+#include "wg_engine.cuh"
 
 namespace dyn {
 
 using namespace tc;
 using namespace fe;
+using namespace wg;
 
 namespace {
 
-constexpr int kWgRing = 8;
-constexpr int kWgStage = 16384;
-// two consumer warpgroups + a producer warpgroup (one thread streams the weights); setmaxnreg moves the
-// producer's registers to the consumers: 2 x 128 x 232 + 128 x 40 <= 64 K
-constexpr int kWgThreads = 3 * 128;
-constexpr int kConsumerRegs = 232, kProducerRegs = 40;
-constexpr int kWgMaxChunks = 32;
 // per warpgroup: positional-encoding operand (112 columns) | pooled operand of base_fc.0 (240 columns), 64 rows
 constexpr int kPeBytes = 14 * 1024, kPoolBytes = 30 * 1024, kWgATile = kPeBytes + kPoolBytes;
 // constants (floats): biases in true units; W6V = row 128 of vis_fc.2 (visibility logit), W8 = vis_fc2.2;
@@ -49,9 +35,6 @@ constexpr int C_B1 = 0, C_B2 = 256, C_B3 = 304, C_B4 = 560, C_B5 = 688, C_B6 = 8
 constexpr int kWgConst = 1884;
 constexpr int kWgSmem = kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 4 /* align */ + 16 * 8;
 static_assert(kWgSmem + kWgMaxChunks * 16 <= 227 * 1024, "shared memory of one CTA");
-
-// k-steps per weight chunk of a layer N wide (one ring stage; at most 8, as fe::append_block cuts them)
-__host__ __device__ constexpr int wg_chunk_ksteps(int N) { return kWgStage / (N * 32) < 8 ? kWgStage / (N * 32) : 8; }
 
 // 11 values of one PE component: [x, cos(2^k x) k=0..4, sin(2^k x) k=0..4]
 __device__ __forceinline__ void pe_comp(float x, float* o) {
@@ -67,116 +50,10 @@ __device__ __forceinline__ void pe_comp(float x, float* o) {
   }
 }
 
-// 8 consecutive columns [c0, c0 + 8) of a row of a 64-row operand tile -> one 16-byte store
-__device__ __forceinline__ void store8_64(uint8_t* arow, int c0, const float* v) {
-  *reinterpret_cast<uint4*>(arow + (c0 >> 3) * 1024) =
-      make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-}
 // columns (col, col + 1) of row r of a 64-row operand tile (col even)
 __device__ __forceinline__ void store2_64(uint8_t* tile, int r, int col, float x, float y) {
   *reinterpret_cast<uint32_t*>(tile + (col >> 3) * 1024 + (r >> 3) * 128 + (r & 7) * 16 + (col & 7) * 2) =
       pack_bf16x2(x, y);
-}
-
-// The weight ring as one consumer warpgroup sees it: chunk `cnt` sits in slot cnt % kWgRing.
-struct Ring {
-  uint8_t* base;
-  uint32_t bar0;  // [0, kWgRing) full, [kWgRing, 2 kWgRing) empty
-  uint32_t cnt;
-  bool prof;
-  long long wait_cycles;  // profiling: cycles spent waiting for weights
-  __device__ __forceinline__ uint32_t wait_full(uint32_t c) {
-    const uint32_t st = c % kWgRing;
-    const long long t0 = prof ? clock64() : 0;
-    mbar_wait(bar0 + 8u * st, (c / kWgRing) & 1);
-    if (prof) wait_cycles += clock64() - t0;
-    return smem_u32(base + st * kWgStage);
-  }
-  // this warp's wgmmas that read chunk c have retired (the empty barrier counts 4 warps x 2 warpgroups)
-  __device__ __forceinline__ void release(uint32_t c) {
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (kWgRing + c % kWgRing));
-  }
-};
-
-// Issues one layer, D[64 x N] = A[64 x 16 KS] W^T, chunk by chunk as the weights arrive; each chunk's slot is
-// released as soon as the next chunk's wgmmas are committed and its own have retired.  The last chunk stays in
-// flight: layer_finish waits for it.  mma(acc, kstep, b_desc, scale_d) issues one k-step.
-template <int N, int KS, class Mma>
-__device__ __forceinline__ void layer_issue(float* acc, Ring& rg, Mma mma) {
-  constexpr int KC = wg_chunk_ksteps(N), NCH = (KS + KC - 1) / KC;
-  fence_regs<N / 2>(acc);
-  wgmma_fence();
-#pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    const uint32_t w = rg.wait_full(rg.cnt + c);
-#pragma unroll
-    for (int s = 0; s < KC; ++s)
-      if (c * KC + s < KS) mma(acc, c * KC + s, smem_desc(w + s * N * 32u, N * 16u, 128u), (c | s) ? 1u : 0u);
-    wgmma_commit();
-    if (c > 0) {
-      wgmma_wait<1>();
-      rg.release(rg.cnt + c - 1);
-    }
-  }
-  rg.cnt += NCH;
-}
-template <int N>
-__device__ __forceinline__ void layer_finish(float* acc, Ring& rg) {
-  wgmma_wait<0>();
-  fence_regs<N / 2>(acc);
-  rg.release(rg.cnt - 1);
-}
-
-template <int N, int KS>
-__device__ __forceinline__ void layer_ss(float* acc, uint32_t a_tile, Ring& rg) {
-  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
-    Wgmma<N, 0, 0>::mma(d, smem_desc(a_tile + ks * 2048u, 1024u, 128u), bd, sc);
-  });
-}
-template <int N, int KS>
-__device__ __forceinline__ void layer_rs(float* acc, const uint32_t (&af)[KS][4], Ring& rg) {
-  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) { WgmmaRS<N>::mma(d, af[ks], bd, sc); });
-  layer_finish<N>(acc, rg);
-}
-
-// ELU(acc + bias[column]) in place, N columns of fragment layout (q = lane % 4)
-template <int N>
-__device__ __forceinline__ void bias_elu(float* acc, const float* bias, int q) {
-#pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      acc[4 * j + 2 * h] = elu_fast(acc[4 * j + 2 * h] + b.x);
-      acc[4 * j + 2 * h + 1] = elu_fast(acc[4 * j + 2 * h + 1] + b.y);
-    }
-  }
-}
-template <int KS>
-__device__ __forceinline__ void to_afrag(const float* acc, uint32_t (&af)[KS][4]) {
-#pragma unroll
-  for (int s = 0; s < KS; ++s) acc_to_afrag(acc, s, af[s]);
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-// sum over the row lanes of a fragment (8 rows of one h)
-__device__ __forceinline__ float rows8_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 4);
-  v += __shfl_xor_sync(0xffffffffu, v, 8);
-  return v + __shfl_xor_sync(0xffffffffu, v, 16);
-}
-// sum over a point's view slots of per-row values v[h] (VP = 8: the point of row half h; VP = 16: both halves)
-template <int VP>
-__device__ __forceinline__ void views_sum(const float* v, float* s) {
-  if (VP == 16) {
-    s[0] = s[1] = rows8_sum(v[0] + v[1]);
-  } else {
-    s[0] = rows8_sum(v[0]);
-    s[1] = rows8_sum(v[1]);
-  }
 }
 
 template <int VP, bool ST>
@@ -679,7 +556,7 @@ int view_wg_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes, c
   auto add = [&](const LinearP& l, int N, int Npad, int Kpad, std::vector<int> map) {
     HostLayer L;
     L.W = P + l.w; L.N = N; L.Kw = l.in; L.Npad = Npad; L.Kpad = Kpad; L.colmap = std::move(map);
-    append_block(L, img, tab, 0, 0, 0, 0, kWgStage, 0, Kpad / 16);
+    append_wg_layer(L, img, tab);
   };
   // base_fc.0 operand columns 0..119: the gathered channels (rgb + 32 features, + the time feature for the
   // dynamic net) as [mean8 | var8 | feat8] groups, twin 0 channels 0..18 at 0..71, twin 1 channels 19..34 at
@@ -731,18 +608,7 @@ int view_wg_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes, c
   add(vis0, 128, 128, 128, identity_map(128, 128));
   add(vis2, 128, 128, 128, identity_map(128, 128));  // rows 0..127 of vis_fc.2; row 128 (the logit) in the epilogue
   add(vis2_0, 128, 128, 128, identity_map(128, 128));
-  const size_t img_bytes = (img.size() + 255) & ~(size_t)255;
-  const size_t need = img_bytes + tab.size() * sizeof(FusedChunk);
-  if (need > dst_bytes) return fail(DYN_E_INVALID, "per-view images need %zu bytes, have %zu", need, dst_bytes);
-  if (tab.size() > (size_t)kWgMaxChunks) return fail(DYN_E_INVALID, "chunk table too long (%zu)", tab.size());
-  DYN_CUDA(cudaMemcpyAsync(dst_dev, img.data(), img.size(), cudaMemcpyHostToDevice, st));
-  DYN_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(dst_dev) + img_bytes, tab.data(),
-                           tab.size() * sizeof(FusedChunk), cudaMemcpyHostToDevice, st));
-  DYN_CUDA(cudaStreamSynchronize(st));
-  n->wg.img = dst_dev;
-  n->wg.tab = reinterpret_cast<const FusedChunk*>(reinterpret_cast<char*>(dst_dev) + img_bytes);
-  n->wg.nchunks = (int)tab.size();
-  return DYN_OK;
+  return upload_wg_image(img, tab, dst_dev, dst_bytes, "per-view", &n->wg, st);
 }
 
 int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
