@@ -135,7 +135,7 @@ size_t dyn_net_packed_bytes(int kind) {
   switch (kind) {
     case DYN_NET_DYNAMIC: return (size_t)dynamic_layout().all.packed_bytes + view_twin_bytes(kind) + view_wg_bytes(kind) + chain_wg_bytes(kind);
     case DYN_NET_STATIC: return (size_t)static_layout(true).all.packed_bytes + view_twin_bytes(kind) + view_wg_bytes(kind) + chain_wg_bytes(kind);
-    case DYN_NET_MOTION: return (size_t)motion_layout(8).all.packed_bytes + motion_fused_bytes();
+    case DYN_NET_MOTION: return (size_t)motion_layout(8).all.packed_bytes + motion_wg_bytes();
     default: return 0;
   }
 }
@@ -221,7 +221,7 @@ int dyn_net_create_ex(int kind, const float* params, size_t n_params, void* pack
         cur += view_wg_bytes(kind);
         if (!rc) rc = chain_wg_build(n, hp, cur, chain_wg_bytes(kind), (cudaStream_t)stream);
       } else if (!rc) {
-        rc = motion_fused_build(n, hp, cur, motion_fused_bytes(), (cudaStream_t)stream);
+        rc = motion_wg_build(n, hp, cur, motion_wg_bytes(), (cudaStream_t)stream);
       }
       free(hp);
       if (rc) { free(n); return rc; }

@@ -68,7 +68,7 @@ __device__ __forceinline__ void chain_producers(const FusedChunk* s_tab, int nch
   setmaxnreg_dec<kProducerRegs>();
   const int t = threadIdx.x & 127;
   if (t == 0) {
-    producer_loop<false, kWgRing, kWgStage>(s_tab, nchunks, wimg, n_iter, smem, bar0);
+    producer_loop<kWgRing, kWgStage>(s_tab, nchunks, wimg, n_iter, smem, bar0);
   } else if (t == 32) {
     const uint8_t* s = reinterpret_cast<const uint8_t*>(src);
     const uint32_t dst = smem_u32(smem + kWgRing * kWgStage);
@@ -97,16 +97,6 @@ template <int NA>
 __device__ __forceinline__ void elu_log2_all(float* acc) {
 #pragma unroll
   for (int i = 0; i < NA; ++i) acc[i] = elu_log2(acc[i]);
-}
-
-// One layer whose first KR k-steps take A from register fragments and the rest from a 64-row operand tile.
-template <int N, int KS, int KR>
-__device__ __forceinline__ void layer_rs_ss(float* acc, const uint32_t (*af)[4], uint32_t tile64, Ring& rg) {
-  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
-    if (ks < KR) WgmmaRS<N>::mma(d, af[ks < KR ? ks : 0], bd, sc);
-    else Wgmma<N, 0, 0>::mma(d, smem_desc(tile64 + (ks - KR) * 2048u, 1024u, 128u), bd, sc);
-  });
-  layer_finish<N>(acc, rg);
 }
 
 // the float pair (row, c .. c + 1) of an fp32 tile-layout array (fused_engine.cuh: tile_f32_off), c even

@@ -119,7 +119,7 @@ struct dyn_net {
   dyn::DynamicLayout dl;
   dyn::StaticLayout sl;
   dyn::MotionLayout ml;
-  // MotionMLP in one fused kernel (motion_fused.cu): motion net only
+  // MotionMLP in one fused kernel (motion_wg.cu): full-width weight chunks in consumption order; motion net only
   dyn::ChainImage motion;
   // row-local chains of the aggregation nets (chains_wg.cu): [0] point stage 1, [1] point stage 2,
   // [2] static blending head

@@ -1,4 +1,4 @@
-// Shared machinery of the fused tensor-core kernels (nets_fused.cu, motion_fused.cu, chains_wg.cu,
+// Shared machinery of the fused tensor-core kernels (nets_fused.cu, motion_wg.cu, chains_wg.cu,
 // view_*.cu): smem budget constants, fast activations, A-tile stores, view-group shuffles, the
 // table-driven weight producer and MMA warpgroup, and the host-side packing of weight chunks into
 // wgmma B-operand images.
@@ -15,11 +15,7 @@ using namespace tc;
 
 constexpr int kRing = 4;
 constexpr int kStageBytes = 16384;
-constexpr int kATileBytes = 69632;  // 128 rows x 272 cols bf16 (34 k-groups: geometry_fc.0 has K = 257)
-constexpr int kConstFloats = 2048;
 constexpr int kNB = 64;              // widest N-block of a chunk (accumulator registers of the MMA warpgroup)
-constexpr int kSmemFused = 2 * kATileBytes + kRing * kStageBytes + kConstFloats * 4 + 256;
-// barrier slots inside the fused kernels: [0..3] w_full, [4..7] w_empty, [8] a_ready, [9] acc_full
 
 __device__ __forceinline__ float ex2f(float x) {
   float y;
@@ -149,62 +145,41 @@ __device__ __forceinline__ void stage_chunks(FusedChunk* s, const FusedChunk* __
 }
 
 // ---- control warps: the weight producer and the MMA warpgroup --------------------
-// barrier slots: [0..3] w_full, [4..7] w_empty, [8] a_ready(tile0), [9] acc_full(tile0),
-//                [10] a_ready(tile1), [11] acc_full(tile1)
-// Two schedules:
-//   one tile (PP = false): one 128-row tile served by two threads per row (twin warps); one a_ready
-//     (2 x 128 arrivals) / acc_full pair.
-//   ping-pong (PP = true): two 128-row tiles, one thread per row; per ROUND (chunks from a wait-flag
-//     to a last-flag) tile 0 then tile 1, each with its own barriers (128 arrivals), so the MMA of one
-//     tile overlaps the epilogue of the other; weights stream twice.
-// generic layout for a ring of `ring` slots: [0,ring) w_full, [ring,2 ring) w_empty, then per tile a_ready, acc_full
-__device__ __forceinline__ uint32_t bar_aready(uint32_t bar0, int tile, int ring = kRing) { return bar0 + 8u * (2 * ring + 2 * tile); }
-__device__ __forceinline__ uint32_t bar_acc(uint32_t bar0, int tile, int ring = kRing) { return bar0 + 8u * (2 * ring + 1 + 2 * tile); }
+// One 128-row tile served by two threads per row (twin warps), one a_ready / acc_full barrier pair.
+// barrier layout for a ring of `ring` slots: [0,ring) w_full, [ring,2 ring) w_empty, then a_ready, acc_full
+__device__ __forceinline__ uint32_t bar_aready(uint32_t bar0, int ring = kRing) { return bar0 + 8u * (2 * ring); }
+__device__ __forceinline__ uint32_t bar_acc(uint32_t bar0, int ring = kRing) { return bar0 + 8u * (2 * ring + 1); }
 
 // The MMA warpgroup: 4 warps, warp-index aligned (wgmma is issued by a whole warpgroup).  w_empty completes
 // when each of its warps has retired the wgmmas that read the slot (one arrival per warp), acc_full when
 // all of its threads have stored their accumulator fragments (one arrival per thread).
 constexpr int kIssuerWarps = 4;
-// `arrivals` = row threads per 128-row tile (128, or 256 in the twin-warp kernels)
-__device__ __forceinline__ void init_barriers(uint32_t bar0, bool pp, int arrivals = 128, int ring = kRing) {
+// `arrivals` = row threads that signal a_ready per 128-row tile
+__device__ __forceinline__ void init_barriers(uint32_t bar0, int arrivals, int ring = kRing) {
   for (int i = 0; i < ring; ++i) { mbar_init(bar0 + 8u * i, 1); mbar_init(bar0 + 8u * (ring + i), kIssuerWarps); }
-  mbar_init(bar_aready(bar0, 0, ring), pp ? arrivals : 2 * arrivals);
-  mbar_init(bar_acc(bar0, 0, ring), 32 * kIssuerWarps);
-  mbar_init(bar_aready(bar0, 1, ring), arrivals);
-  mbar_init(bar_acc(bar0, 1, ring), 32 * kIssuerWarps);
+  mbar_init(bar_aready(bar0, ring), arrivals);
+  mbar_init(bar_acc(bar0, ring), 32 * kIssuerWarps);
   mbar_fence_init();
 }
 
-__device__ __forceinline__ int round_end(const FusedChunk* __restrict__ chunks, int c0, int nchunks) {
-  int c = c0;
-  while (c < nchunks && !(chunks[c].flags & 2)) ++c;
-  return c + 1 < nchunks ? c + 1 : nchunks;
-}
-
 // Called by one thread: streams the weight chunks of every iteration through the ring.
-template <bool PP, int RING = kRing, int STAGE = kStageBytes>
+template <int RING = kRing, int STAGE = kStageBytes>
 __device__ __forceinline__ void producer_loop(const FusedChunk* __restrict__ chunks, int nchunks,
                                               const void* wimg, int n_iter, uint8_t* ring, uint32_t bar0) {
   const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(wimg);
   uint32_t cnt = 0;
   for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
-    for (int c0 = 0; c0 < nchunks;) {
-      const int c1 = PP ? round_end(chunks, c0, nchunks) : nchunks;
-      for (int rep = 0; rep < (PP ? 2 : 1); ++rep) {
-        for (int c = c0; c < c1; ++c, ++cnt) {
-          const uint32_t st = cnt % RING;
-          if (cnt >= RING) mbar_wait(bar0 + 8u * (RING + st), ((cnt / RING) - 1) & 1);
-          const FusedChunk ch = chunks[c];
-          mbar_arrive_expect_tx(bar0 + 8u * st, ch.bytes);
-          bulk_g2s(smem_u32(ring + st * STAGE), wsrc + ch.off, ch.bytes, bar0 + 8u * st);
-        }
-      }
-      c0 = c1;
+    for (int c = 0; c < nchunks; ++c, ++cnt) {
+      const uint32_t st = cnt % RING;
+      if (cnt >= RING) mbar_wait(bar0 + 8u * (RING + st), ((cnt / RING) - 1) & 1);
+      const FusedChunk ch = chunks[c];
+      mbar_arrive_expect_tx(bar0 + 8u * st, ch.bytes);
+      bulk_g2s(smem_u32(ring + st * STAGE), wsrc + ch.off, ch.bytes, bar0 + 8u * st);
     }
   }
 }
 
-// One N-block of a chunk for the accumulators of one tile: 2 x 64-row wgmmas per k-step.
+// One N-block of a chunk for the accumulators of the tile: 2 x 64-row wgmmas per k-step.
 template <int NB>
 __device__ __forceinline__ void mma_chunk(float (&acc)[2][kNB / 2], uint32_t a_addr, const FusedChunk& ch,
                                           uint32_t w_addr) {
@@ -218,30 +193,30 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[2][kNB / 2], uint32_t a_a
       Wgmma<NB, 0, 0>::mma(acc[h], smem_desc(aa + ks * 4096u + h * 1024u, 2048u, 128u), bd, sc);
   }
 }
-// accumulators <-> accumulator memory (the tile at columns col0 + 256 tile, col0 including d_col)
+// accumulators <-> accumulator memory (columns from col0, col0 including d_col)
 template <int NB>
-__device__ __forceinline__ void acc_chunk_io(float (&acc)[2][kNB / 2], int tile, int col0, bool store) {
+__device__ __forceinline__ void acc_chunk_io(float (&acc)[2][kNB / 2], int col0, bool store) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    if (store) acc_store_frag<NB>(acc[h], 64 * h, col0 + 256 * tile);
-    else acc_load_frag<NB>(acc[h], 64 * h, col0 + 256 * tile);
+    if (store) acc_store_frag<NB>(acc[h], 64 * h, col0);
+    else acc_load_frag<NB>(acc[h], 64 * h, col0);
   }
 }
 
 // one chunk start to finish: resume the N-block from accumulator memory if it continues one, multiply,
 // wait for the wgmmas to retire, store the N-block if it ends here
 template <int NB>
-__device__ __forceinline__ void run_chunk(float (&acc)[2][kNB / 2], uint32_t a_addr, int tile, const FusedChunk& ch,
+__device__ __forceinline__ void run_chunk(float (&acc)[2][kNB / 2], uint32_t a_addr, const FusedChunk& ch,
                                           uint32_t w_addr, uint32_t tmem_base) {
   const int col0 = (int)(tmem_base & 0xffffu) + ch.d_col;
-  if ((ch.flags & 40) == 32) acc_chunk_io<NB>(acc, tile, col0, false);
+  if ((ch.flags & 40) == 32) acc_chunk_io<NB>(acc, col0, false);
   fence_regs<NB / 2>(acc[0]); fence_regs<NB / 2>(acc[1]);
   wgmma_fence();
   mma_chunk<NB>(acc, a_addr, ch, w_addr);
   wgmma_commit();
   wgmma_wait<0>();
   fence_regs<NB / 2>(acc[0]); fence_regs<NB / 2>(acc[1]);
-  if (ch.flags & 16) acc_chunk_io<NB>(acc, tile, col0, true);
+  if (ch.flags & 16) acc_chunk_io<NB>(acc, col0, true);
 }
 
 // Called by ALL 128 threads of the MMA warpgroup (warps 4k .. 4k + 3 of the CTA).
@@ -250,59 +225,51 @@ __device__ __forceinline__ void run_chunk(float (&acc)[2][kNB / 2], uint32_t a_a
 // 16 / 32 = last / first chunk of an N-block (store it to TMEM / without 8: continue from TMEM);
 // d_col = accumulator column offset inside the tile's 256-column TMEM region.
 // RING = weight-ring slots in use.
-template <bool PP, int RING = kRing, int STAGE = kStageBytes>
+template <int RING = kRing, int STAGE = kStageBytes>
 __device__ __forceinline__ void issuer_loop(const FusedChunk* __restrict__ chunks, int nchunks, int n_iter,
                                             uint8_t* smem, uint8_t* ring, uint32_t bar0,
-                                            uint32_t tmem_base, int a_tile_bytes = kATileBytes,
-                                            long long* dbg = nullptr) {
-  // wgmma is issued by the whole warpgroup; the accumulators of one N-block (<= kNB columns) of the tile the
-  // chunk serves stay in registers across the N-block's chunks
+                                            uint32_t tmem_base, long long* dbg = nullptr) {
+  // wgmma is issued by the whole warpgroup; the accumulators of one N-block (<= kNB columns) stay in
+  // registers across the N-block's chunks
   {
     float acc[2][kNB / 2];
     const bool lead = threadIdx.x % 128 == 0;
-    uint32_t cnt = 0, a_cnt[2] = {0, 0};
+    uint32_t cnt = 0, a_cnt = 0;
     long long t_a = 0, t_w = 0, t_begin = clock64();
-    const uint32_t a_addr[2] = {smem_u32(smem), smem_u32(smem + a_tile_bytes)};
+    const uint32_t a_addr = smem_u32(smem);
     for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
-      for (int c0 = 0; c0 < nchunks;) {
-        const int c1 = PP ? round_end(chunks, c0, nchunks) : nchunks;
-        for (int rep = 0; rep < (PP ? 2 : 1); ++rep) {
-          for (int c = c0; c < c1; ++c, ++cnt) {
-            const FusedChunk ch = chunks[c];
-            long long t0 = dbg ? clock64() : 0;
-            if (ch.flags & 1) {
-              mbar_wait(bar_aready(bar0, PP ? rep : 0, RING), a_cnt[PP ? rep : 0] & 1);
-              ++a_cnt[PP ? rep : 0];
-            }
-            long long t1 = dbg ? clock64() : 0;
-            const uint32_t st = cnt % RING;
-            mbar_wait(bar0 + 8u * st, (cnt / RING) & 1);
-            tc_fence_after_sync();
-            long long t2 = 0;
-            if (dbg) {
-              t2 = clock64();
-              t_a += t1 - t0;
-              t_w += t2 - t1;
-            }
-            const uint32_t w_addr = smem_u32(ring + st * STAGE);
-            const int tile = PP ? rep : 0;
-            switch (ch.npad) {
-              case 16: run_chunk<16>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
-              case 32: run_chunk<32>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
-              case 48: run_chunk<48>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
-              case 64: run_chunk<64>(acc, a_addr[tile], tile, ch, w_addr, tmem_base); break;
-              default: __trap();  // the host packer emits N-blocks of 16, 32, 48 or 64 columns only
-            }
-            __syncwarp();
-            if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (RING + st));  // this warp's wgmmas have retired
-            if (ch.flags & 2) mbar_arrive(bar_acc(bar0, PP ? rep : 0, RING));
-            if (dbg && blockIdx.x == 0 && lead && cnt < 120) {
-              dbg[8 + 4 * cnt + 0] = t0; dbg[8 + 4 * cnt + 1] = t1;
-              dbg[8 + 4 * cnt + 2] = t2; dbg[8 + 4 * cnt + 3] = clock64();
-            }
-          }
+      for (int c = 0; c < nchunks; ++c, ++cnt) {
+        const FusedChunk ch = chunks[c];
+        long long t0 = dbg ? clock64() : 0;
+        if (ch.flags & 1) {
+          mbar_wait(bar_aready(bar0, RING), a_cnt & 1);
+          ++a_cnt;
         }
-        c0 = c1;
+        long long t1 = dbg ? clock64() : 0;
+        const uint32_t st = cnt % RING;
+        mbar_wait(bar0 + 8u * st, (cnt / RING) & 1);
+        tc_fence_after_sync();
+        long long t2 = 0;
+        if (dbg) {
+          t2 = clock64();
+          t_a += t1 - t0;
+          t_w += t2 - t1;
+        }
+        const uint32_t w_addr = smem_u32(ring + st * STAGE);
+        switch (ch.npad) {
+          case 16: run_chunk<16>(acc, a_addr, ch, w_addr, tmem_base); break;
+          case 32: run_chunk<32>(acc, a_addr, ch, w_addr, tmem_base); break;
+          case 48: run_chunk<48>(acc, a_addr, ch, w_addr, tmem_base); break;
+          case 64: run_chunk<64>(acc, a_addr, ch, w_addr, tmem_base); break;
+          default: __trap();  // the host packer emits N-blocks of 16, 32, 48 or 64 columns only
+        }
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (RING + st));  // this warp's wgmmas have retired
+        if (ch.flags & 2) mbar_arrive(bar_acc(bar0, RING));
+        if (dbg && blockIdx.x == 0 && lead && cnt < 120) {
+          dbg[8 + 4 * cnt + 0] = t0; dbg[8 + 4 * cnt + 1] = t1;
+          dbg[8 + 4 * cnt + 2] = t2; dbg[8 + 4 * cnt + 3] = clock64();
+        }
       }
     }
     if (dbg != nullptr && blockIdx.x == 0 && lead) {

@@ -789,12 +789,12 @@ int motion_f32(const dyn_net* n, const float* x, int ldx, bool time_is_column, f
                long long N_all, float* coeff, void* ws, size_t ws_bytes, int prec, cudaStream_t st) {
   const MotionLayout& L = n->ml;
   if (prec == DYN_PREC_BF16 && n->motion.img != nullptr) {
-    // whole MLP in one tensor-core kernel (motion_fused.cu); no workspace needed
+    // whole MLP in one tensor-core kernel (motion_wg.cu); no workspace needed
     MotionFusedArgs a;
     memset(&a, 0, sizeof(a));
     a.x = x; a.ldx = ldx; a.time_is_column = time_is_column ? 1 : 0; a.time = time;
-    a.N = N_all; a.S = 0; a.n_last = 0; a.coeff = coeff;
-    return launch_motion_fused(n, a, st);
+    a.N = N_all; a.coeff = coeff;
+    return launch_motion_wg(n, a, st);
   }
   for (long long i0 = 0; i0 < N_all; i0 += kMotionRows) {
     long long N = (N_all - i0) < kMotionRows ? (N_all - i0) : kMotionRows;

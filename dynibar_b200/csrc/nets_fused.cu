@@ -47,4 +47,30 @@ int launch_view_fused(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st
   }
 }
 
+// host-only unit-test hooks behind dyn_debug_pack_layer / dyn_debug_tile_image_off
+int debug_pack_layer(const float* W, const float* bias, int N, int Kw, int Npad, int Kpad, const int* colmap,
+                     float scale, int stage_bytes, void* out_img, size_t out_bytes, size_t* img_bytes,
+                     int* nchunks) {
+  using namespace fe;
+  if (N < 1 || Npad < N || (Npad % 16) != 0 || Npad > 256 || (Kpad % 16) != 0 || Kpad < 16 || Kw < 1 ||
+      stage_bytes < Npad * 32)
+    return fail(DYN_E_INVALID, "dyn_debug_pack_layer: bad shape N=%d Npad=%d Kpad=%d stage=%d", N, Npad, Kpad,
+                stage_bytes);
+  HostLayer L;
+  L.W = W; L.N = N; L.Kw = Kw; L.Npad = Npad; L.Kpad = Kpad;
+  L.colmap.assign(colmap, colmap + Kpad);
+  for (int c : L.colmap)
+    if (c >= Kw || c < kBiasLo) return fail(DYN_E_INVALID, "dyn_debug_pack_layer: colmap entry %d out of range", c);
+  L.bias = bias; L.scale = scale;
+  std::vector<uint8_t> img;
+  std::vector<FusedChunk> tab;
+  append_layer(L, img, tab, 0, 0, 9, true, stage_bytes);
+  *img_bytes = img.size();
+  *nchunks = (int)tab.size();
+  if (img.size() > out_bytes) return fail(DYN_E_INVALID, "dyn_debug_pack_layer: image needs %zu bytes", img.size());
+  memcpy(out_img, img.data(), img.size());
+  return DYN_OK;
+}
+size_t debug_tile_image_off(long long row, int kgroup, int kgroups) { return fe::tile_image_off(row, kgroup, kgroups); }
+
 }  // namespace dyn

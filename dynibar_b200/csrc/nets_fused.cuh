@@ -51,13 +51,12 @@ struct ViewFusedArgs {
   long long* dbg;    // optional: clock64() phase timestamps of block 0 (profiling builds/tests only)
 };
 
-// ---- MotionMLP (motion_fused.cu) ----
+// ---- MotionMLP (motion_wg.cu) ----
 struct MotionFusedArgs {
   const float* x;  // [N, ldx] xyz (+ time column when time_is_column)
   int ldx, time_is_column;
   float time;
   long long N;
-  int S, n_last;   // zero the last n_last samples of each S-sample ray (S = 0: never)
   float* coeff;    // [N, ncoef]
   int ncoef;
   const float* params;
@@ -116,9 +115,9 @@ int debug_pack_layer(const float* W, const float* bias, int N, int Kw, int Npad,
                      float scale, int stage_bytes, void* out_img, size_t out_bytes, size_t* img_bytes,
                      int* nchunks);
 size_t debug_tile_image_off(long long row, int kgroup, int kgroups);
-size_t motion_fused_bytes();
-int motion_fused_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
-int launch_motion_fused(const dyn_net* n, MotionFusedArgs& a, cudaStream_t st);
+size_t motion_wg_bytes();
+int motion_wg_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
+int launch_motion_wg(const dyn_net* n, MotionFusedArgs& a, cudaStream_t st);
 
 // the point stages and the static blending head (chains_wg.cu): accumulators in registers, two 64-row
 // warpgroups per CTA

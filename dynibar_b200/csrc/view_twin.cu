@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
   __shared__ __align__(16) FusedChunk s_tab[kMaxChunks];
   stage_chunks(s_tab, a.chunks, a.nchunks);
 
-  if (tid == 0) init_barriers(bar0, /*pp=*/false, /*arrivals=*/128, RING);
+  if (tid == 0) init_barriers(bar0, /*arrivals=*/256, RING);
   {
     const float* prm = a.params;
     for (int i = tid; i < 256; i += blockDim.x) {  // camera matrices: lanes index them by view
@@ -143,10 +143,10 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
   const int n_iter = (int)((n_rows + ROWS - 1) / ROWS);
 
   if (warp == W_PROD) {
-    if ((tid & 31) == 0) producer_loop<false, RING, kTwinStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
+    if ((tid & 31) == 0) producer_loop<RING, kTwinStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
   } else if (warp >= W_ISSUE) {
-    issuer_loop<false, RING, kTwinStage>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base, kTwinATile,
-                                         a.dbg ? a.dbg + 128 : nullptr);
+    issuer_loop<RING, kTwinStage>(s_tab, a.nchunks, n_iter, smem, ring, bar0, tmem_base,
+                                  a.dbg ? a.dbg + 128 : nullptr);
   } else {
     const int tw = tid >> 7, t = tid & 127;  // twin index, row of the tile
     uint8_t* arow = smem + (t >> 3) * 128 + (t & 7) * 16;
@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
         }
         fence_proxy_async_smem();
         tc_fence_before_sync();
-        mbar_arrive(bar_aready(bar0, 0, RING));
+        mbar_arrive(bar_aready(bar0, RING));
       }
 
       TS();  // 1: after F1 operand + arrive
@@ -354,13 +354,13 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
       TS();  // 2: after gather
       if (ST) {
         // ---- F1 epilogue: this twin's 128 of the 256 columns ----
-        mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+        mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
         TS();  // 3: F1 acc ready
         tc_fence_after_sync();
         elu_log2_block_to_A<128>(arow, tacc, 128 * tw);
         fence_proxy_async_smem();
         tc_fence_before_sync();
-        mbar_arrive(bar_aready(bar0, 0, RING));
+        mbar_arrive(bar_aready(bar0, RING));
         TS();  // 4: F1 epilogue done
         // ---- F2: src_feat (35 of 48 columns) * ref_feat; twin 0 keeps 0..17, twin 1 keeps 18..34.
         //      The per-ray reference feature is loaded BEFORE the wait (its L2 latency hides behind the MMA) ----
@@ -370,7 +370,7 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
 #pragma unroll
           for (int i = 0; i < 18; ++i) rfv[i] = (tw == 0 || i < 17) ? __ldg(rf + i) : 0.f;
         }
-        mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+        mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
         TS();  // 5: F2 acc ready
         tc_fence_after_sync();
         float s48[48];
@@ -436,23 +436,23 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
       }
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, 0, RING));
+      mbar_arrive(bar_aready(bar0, RING));
 
       TS();  // 6: pool1 done + arrive
       // ---- F3: ELU(base_fc.0), this twin's 128 columns ----
-      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 7: F3 acc ready
       tc_fence_after_sync();
       elu_log2_block_to_A<128>(arow, tacc, 128 * tw);
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, 0, RING));
+      mbar_arrive(bar_aready(bar0, RING));
 
       const int c0 = 64 * tw;  // this twin's columns of the 128-wide layers
       TS();  // 8: F3 epilogue done
       // ---- F4: x = ELU(base_fc.2) -> TMEM [128,256); A = x (the pooling weight w1 of vis_fc.0's input is applied
       //      to the accumulator in the next epilogue: W (w1 x) = w1 (W x)); bias folded, accumulator on the exp2 scale ----
-      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 9: F4 acc ready
       tc_fence_after_sync();
 #pragma unroll 1
@@ -475,11 +475,11 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
       tmem_wait_st();
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, 0, RING));
+      mbar_arrive(bar_aready(bar0, RING));
 
       TS();  // 10: F4 epilogue done
       // ---- F5: h = ELU(vis_fc.0) -> A; partial visibility logit ----
-      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 11: F5 acc ready
       tc_fence_after_sync();
       {
@@ -501,11 +501,11 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
       }
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, 0, RING));
+      mbar_arrive(bar_aready(bar0, RING));
 
       TS();  // 12: F5 epilogue done
       // ---- F6: x += ELU(vis_fc.2[:128]); A = x * vis1 ----
-      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 13: F6 acc ready
       tc_fence_after_sync();
       // both twins arrived on a_ready before this MMA ran: the partial logits are visible
@@ -538,12 +538,12 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
       tmem_wait_st();
       fence_proxy_async_smem();
       tc_fence_before_sync();
-      mbar_arrive(bar_aready(bar0, 0, RING));
+      mbar_arrive(bar_aready(bar0, RING));
 
       TS();  // 14: F6 epilogue done
       if (it + (int)gridDim.x < n_iter) fetch_point(it + (int)gridDim.x);  // next iteration's point
       // ---- F7: vis2 = sigmoid(vis_fc2.2 . ELU(vis_fc2.0)) * mask ----
-      mbar_wait(bar_acc(bar0, 0, RING), acc_cnt & 1); ++acc_cnt;
+      mbar_wait(bar_acc(bar0, RING), acc_cnt & 1); ++acc_cnt;
       TS();  // 15: F7 acc ready
       tc_fence_after_sync();
       {

@@ -105,7 +105,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
   const int n_iter = (int)((n_rows + 127) / 128);
   if (wg == 2) {
     setmaxnreg_dec<kProducerRegs>();
-    if (tid == 256) producer_loop<false, kWgRing, kWgStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
+    if (tid == 256) producer_loop<kWgRing, kWgStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();

@@ -1,4 +1,4 @@
-// Warpgroup engine of the Hopper fused kernels (view_wg.cu, chains_wg.cu): one persistent CTA per SM with two
+// Warpgroup engine of the Hopper fused kernels (view_wg.cu, chains_wg.cu, motion_wg.cu): one persistent CTA per SM with two
 // consumer warpgroups and a producer warpgroup.  Each consumer warpgroup owns 64 rows of the CTA's 128-row
 // iteration and issues its own wgmmas, one instruction per k-step for the whole layer width; the accumulators
 // stay in registers, and a hidden layer's output, packed to bf16 pairs, is the register A operand of the next
@@ -26,7 +26,7 @@ constexpr int kWgStage = 16384;
 // 2 x 128 x 232 + 128 x 40 <= 64 K
 constexpr int kWgThreads = 3 * 128;
 constexpr int kConsumerRegs = 232, kProducerRegs = 40;
-constexpr int kWgMaxChunks = 32;
+constexpr int kWgMaxChunks = 72;  // the MotionMLP's image has 68 chunks
 
 // k-steps per weight chunk of a layer N wide (one ring stage; at most 8, as fe::append_block cuts them)
 __host__ __device__ constexpr int wg_chunk_ksteps(int N) { return kWgStage / (N * 32) < 8 ? kWgStage / (N * 32) : 8; }
@@ -99,7 +99,29 @@ __device__ __forceinline__ void layer_rs(float* acc, const uint32_t (&af)[KS][4]
   layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) { WgmmaRS<N>::mma(d, af[ks], bd, sc); });
   layer_finish<N>(acc, rg);
 }
+// One layer whose first KR k-steps take A from register fragments and the rest from a 64-row operand tile.
+template <int N, int KS, int KR>
+__device__ __forceinline__ void layer_rs_ss(float* acc, const uint32_t (*af)[4], uint32_t tile64, Ring& rg) {
+  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
+    if (ks < KR) WgmmaRS<N>::mma(d, af[ks < KR ? ks : 0], bd, sc);
+    else Wgmma<N, 0, 0>::mma(d, smem_desc(tile64 + (ks - KR) * 2048u, 1024u, 128u), bd, sc);
+  });
+  layer_finish<N>(acc, rg);
+}
 
+// ReLU(acc + bias[column]) in place, N columns of fragment layout (q = lane % 4)
+template <int N>
+__device__ __forceinline__ void bias_relu(float* acc, const float* bias, int q) {
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      acc[4 * j + 2 * h] = fmaxf(acc[4 * j + 2 * h] + b.x, 0.f);
+      acc[4 * j + 2 * h + 1] = fmaxf(acc[4 * j + 2 * h + 1] + b.y, 0.f);
+    }
+  }
+}
 // ELU(acc + bias[column]) in place, N columns of fragment layout (q = lane % 4)
 template <int N>
 __device__ __forceinline__ void bias_elu(float* acc, const float* bias, int q) {
