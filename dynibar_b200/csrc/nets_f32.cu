@@ -13,6 +13,8 @@
 #include "fused_engine.cuh"
 
 extern "C" long long* view_dbg_ptr();
+// the profiling buffer of dyn_debug_set_view_timestamps: static net [0, 616), dynamic net [616, 1232)
+constexpr int kViewDbgPerNet = 616;
 
 namespace dyn {
 
@@ -1185,6 +1187,7 @@ int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, 
     va.ref_feat = nullptr; va.dfeat = d.small;
     va.G = d.G; va.nvalid = d.t.nvalid; va.mask_proj = mask_out + p0 * V; va.mask_eff = nullptr;
     va.X = nullptr; va.vis2 = nullptr; va.ray_diff = nullptr; va.rgb_in = nullptr;
+    va.dbg = view_dbg_ptr() ? view_dbg_ptr() + kViewDbgPerNet : nullptr;
     RUN(launch_view_fused(n, va, V, st));
     if (g_view_cap_on) RUN(capture_view_outputs(va, p0, P, V, st));
     {

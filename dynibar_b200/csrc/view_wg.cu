@@ -9,11 +9,14 @@
 //
 // Built on the warpgroup engine (wg_engine.cuh): each consumer warpgroup owns 64 rows (view slots) of the CTA's
 // 128-row iteration, accumulators stay in registers, and only the two front-end operands (positional encodings,
-// pooled features) go through shared memory.  While one warpgroup runs an epilogue, the other's wgmmas keep the
-// tensor cores busy.  A point's view slots are 8 or 16 aligned rows of one warp's 16-row slab, so sums over its
+// pooled features) go through shared memory.  The two issue their layers in turn, so while one warpgroup runs an
+// epilogue, the other's wgmmas keep the tensor cores busy.  A point's view slots are 8 or 16 aligned rows of one warp's 16-row slab, so sums over its
 // views are shuffles over the row lanes (wg_engine.cuh: views_sum).
-// The front end (projection, gather, first pooling of the gathered channels) runs with two threads per row,
-// as in view_twin.cu: warps 0-1 of a warpgroup ("twin 0") and 2-3 ("twin 1") each take half of the channels.
+// The front end (projection, gather, first pooling of the gathered channels, positional encodings) runs on a
+// warpgroup of its own, for consumer 0's rows and then consumer 1's, with two threads per row as in view_twin.cu:
+// warps 0-1 ("twin 0") and 2-3 ("twin 1") each take half of the channels.  A full / empty mbarrier pair per
+// consumer hands over its operand tiles and per-row pooling weights and masks: the consumer frees them once
+// base_fc.0 has retired, so the front end of its next iteration runs behind its remaining layers.
 #include "geometry.cuh"
 #include "nets.cuh"
 #include "wg_engine.cuh"
@@ -26,15 +29,63 @@ using namespace wg;
 
 namespace {
 
-// per warpgroup: positional-encoding operand (112 columns) | pooled operand of base_fc.0 (240 columns), 64 rows
+// per consumer warpgroup: positional-encoding operand (112 columns) | pooled operand of base_fc.0 (240 columns),
+// 64 rows
 constexpr int kPeBytes = 14 * 1024, kPoolBytes = 30 * 1024, kWgATile = kPeBytes + kPoolBytes;
 // constants (floats): biases in true units; W6V = row 128 of vis_fc.2 (visibility logit), W8 = vis_fc2.2;
-// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; W1 / MK = per-row pooling weight and mask of each warpgroup
+// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; W1 / MK = per-row pooling weight and mask of each consumer
 constexpr int C_B1 = 0, C_B2 = 256, C_B3 = 304, C_B4 = 560, C_B5 = 688, C_B6 = 816, C_W6V = 944, C_B7 = 1072,
               C_W8 = 1200, C_MISC = 1328, C_DFEAT = 1332, C_CAMS = 1372, C_W1 = 1628, C_MK = 1756;
 constexpr int kWgConst = 1884;
-constexpr int kWgSmem = kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 4 /* align */ + 16 * 8;
+// mbarriers: the weight ring's full / empty pairs, then per consumer its operand tiles' full and empty
+constexpr int kViewBars = 2 * kWgRing + 4;
+constexpr int kWgSmem = kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 4 /* align */ + kViewBars * 8;
 static_assert(kWgSmem + kWgMaxChunks * 16 <= 227 * 1024, "shared memory of one CTA");
+// warpgroups 0, 1: consumers; 2: front end; 3: weight producer.  setmaxnreg splits the 64 K registers:
+// 2 x 128 x 208 + 128 x 72 + 128 x 24 = 64 K.  The consumers' peak is a 256-wide epilogue (128 accumulators,
+// then 64 A-fragment registers).
+constexpr int kViewThreads = 4 * 128;
+constexpr int kViewConsumerRegs = 208, kViewFrontRegs = 72, kViewProducerRegs = 24;
+
+// Phase profile of block 0 (dyn_debug_set_view_timestamps).  Thread 0 of each warpgroup charges the cycles since
+// its previous mark to one phase, less the weight-ring waits in between, which go to PH_WEIGHTS; the counters sit in
+// shared memory while the kernel runs and are copied to dbg[32 wg + phase] at its end.  tools/view_phases.py reads
+// them; the indices are its table.
+enum Phase {
+  PH_FRONT, PH_BAR, PH_WEIGHTS, PH_F1, PH_F1_EPI, PH_F2, PH_F2_EPI, PH_F3, PH_F3_EPI, PH_F4, PH_F4_EPI, PH_F5,
+  PH_F5_EPI, PH_F6, PH_F6_EPI, PH_F7, PH_F7_EPI, PH_POOL2, PH_HANDOFF,
+  PH_T = 28, PH_W = 29, PH_ITERS = 30, PH_LIFE = 31  // last mark, weight waits at the last mark, iterations, lifetime
+};
+constexpr int kPhaseSlots = 32;
+__shared__ long long s_phase[3][kPhaseSlots];  // consumers 0, 1, front end
+struct PhaseClock {
+  const ViewFusedArgs& a;  // profiling when a.dbg is set: thread 0 of each warpgroup of block 0
+  int wg;
+  __device__ __forceinline__ bool on() const { return a.dbg != nullptr && blockIdx.x == 0 && (threadIdx.x & 127) == 0; }
+  __device__ __forceinline__ long long* c() const { return s_phase[wg]; }
+  __device__ __forceinline__ void start() {
+    if (!on()) return;
+    for (int i = 0; i < kPhaseSlots; ++i) c()[i] = 0;
+    c()[PH_T] = c()[PH_LIFE] = clock64();
+  }
+  __device__ __forceinline__ void mark(int ph, long long waits) {
+    if (!on()) return;
+    long long* s = c();
+    const long long now = clock64();
+    s[ph] += now - s[PH_T] - (waits - s[PH_W]);
+    s[PH_WEIGHTS] += waits - s[PH_W];
+    s[PH_T] = now;
+    s[PH_W] = waits;
+  }
+  __device__ __forceinline__ void iteration() {
+    if (on()) ++c()[PH_ITERS];
+  }
+  __device__ __forceinline__ void finish() {
+    if (!on()) return;
+    c()[PH_LIFE] = clock64() - c()[PH_LIFE];
+    for (int i = 0; i < kPhaseSlots; ++i) a.dbg[kPhaseSlots * wg + i] = c()[i];
+  }
+};
 
 // 11 values of one PE component: [x, cos(2^k x) k=0..4, sin(2^k x) k=0..4]
 __device__ __forceinline__ void pe_comp(float x, float* o) {
@@ -50,14 +101,241 @@ __device__ __forceinline__ void pe_comp(float x, float* o) {
   }
 }
 
+// layer_ss<256, KS> as two m64n128k16 wgmmas per k-step, columns 0..127 into acc[0..63] and 128..255 into
+// acc[64..127] (the fragment layout of one N = 256 wgmma): a single m64n256k16 needs more registers than the
+// 128 a 512-thread CTA may launch with.  Rows 128..255 of a weight chunk's k-step start 16 core matrices (2048
+// bytes) after rows 0..127.
+template <int KS>
+__device__ __forceinline__ void layer_ss256(float* acc, uint32_t a_tile, Ring& rg) {
+  layer_issue<256, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
+    const uint64_t ad = smem_desc(a_tile + ks * 2048u, 1024u, 128u);
+    Wgmma<128, 0, 0>::mma(d, ad, bd, sc);
+    Wgmma<128, 0, 0>::mma(d + 64, ad, bd + (2048u >> 4), sc);
+  });
+}
+
+// layer_rs without its layer_finish
+template <int N, int KS>
+__device__ __forceinline__ void layer_rs_issue(float* acc, const uint32_t (&af)[KS][4], Ring& rg) {
+  layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) { WgmmaRS<N>::mma(d, af[ks], bd, sc); });
+}
+
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // columns (col, col + 1) of row r of a 64-row operand tile (col even)
 __device__ __forceinline__ void store2_64(uint8_t* tile, int r, int col, float x, float y) {
   *reinterpret_cast<uint32_t*>(tile + (col >> 3) * 1024 + (r >> 3) * 128 + (r & 7) * 16 + (col & 7) * 2) =
       pack_bf16x2(x, y);
 }
 
+// The front end of the 64 rows from row0 on, row layout (t = thread of the front-end warpgroup: twin tw = t / 64 of
+// row t % 64): projection, masks, gather, first pooling into columns 0..119 of pool_tile, [static] positional
+// encodings into pe_tile; each row's pooling weight and mask into s_w1 / s_mk; the per-(point, view) outputs.
 template <int VP, bool ST>
-__global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_constant__ ViewFusedArgs a) {
+__device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* cst, int t, long long row0,
+                                          uint8_t* pe_tile, uint8_t* pool_tile, float* s_w1, float* s_mk) {
+  const int tw = t >> 6, r = t & 63, v = r & (VP - 1);
+  uint8_t* arow_pe = pe_tile + (r >> 3) * 128 + (r & 7) * 16;
+  uint8_t* arow_pool = pool_tile + (r >> 3) * 128 + (r & 7) * 16;
+  const float wh = a.w_img, hh = a.h_img;
+  const bool want_rgb = (tw == 0) || (ST && a.mask_rgb);
+
+  const long long pl = (row0 + r) / VP;
+  const bool pt_ok = pl < a.P;
+  const bool valid = pt_ok && v < a.V;
+  const long long m = pl * a.V + v;
+  float p3[3] = {0.f, 0.f, 0.f};
+  if (pt_ok) { p3[0] = a.pts[pl * 3]; p3[1] = a.pts[pl * 3 + 1]; p3[2] = a.pts[pl * 3 + 2]; }
+  float q3[3] = {p3[0], p3[1], p3[2]};
+  if (!ST && valid) {
+    const float* qq = a.pts_seq + ((long long)v * a.seq_stride + pl) * 3;
+    q3[0] = qq[0]; q3[1] = qq[1]; q3[2] = qq[2];
+  }
+
+  const int vc = valid ? v : 0;
+  const float* cam = cst + C_CAMS + 16 * vc;
+  float pu, pv;
+  bool front;
+  project_point(cam, q3[0], q3[1], q3[2], pu, pv, front);
+  const bool inb = (pu <= wh - 1.f) && (pu >= 0.f) && (pv <= hh - 1.f) && (pv >= 0.f);
+  const float mask_proj = (valid && inb && front) ? 1.f : 0.f;
+
+  // ---- gather: this twin's 16 bf16 feature channels (+ RGB) at the 4 bilinear taps, two taps per round ----
+  float chv[24];
+#pragma unroll
+  for (int i = 0; i < 24; ++i) chv[i] = 0.f;
+  float rgb[3] = {0.f, 0.f, 0.f};
+  {
+    const float gx = 2.f * pu / (wh - 1.f) - 1.f, gy = 2.f * pv / (hh - 1.f) - 1.f;
+    const float fx = (gx + 1.f) * 0.5f * (float)(a.w - 1), fy = (gy + 1.f) * 0.5f * (float)(a.h - 1);
+    const float x0f = floorf(fx), y0f = floorf(fy);
+    const int x0 = (int)x0f, y0 = (int)y0f;
+    const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
+    const uint16_t* base = a.feat_bf + (long long)vc * a.h * a.w * kC + 16 * tw;
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy) {
+      uint4 tf[4];
+      float tw4[2];
+#pragma unroll
+      for (int dx = 0; dx < 2; ++dx) {
+        // out-of-range taps (and padding rows) load a clamped texel with weight 0
+        const int xi = x0 + dx, yi = y0 + dy;
+        const bool in = valid && xi >= 0 && xi < a.w && yi >= 0 && yi < a.h;
+        tw4[dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
+        const int xc = min(max(xi, 0), a.w - 1), yc = min(max(yi, 0), a.h - 1);
+        const uint4* tp = reinterpret_cast<const uint4*>(base + ((long long)yc * a.w + xc) * kC);
+        tf[2 * dx] = __ldg(tp);
+        tf[2 * dx + 1] = __ldg(tp + 1);
+      }
+#pragma unroll
+      for (int dx = 0; dx < 2; ++dx) {
+#pragma unroll
+        for (int hlf = 0; hlf < 2; ++hlf) {
+          const uint4 qv = tf[2 * dx + hlf];
+          const uint32_t u[4] = {qv.x, qv.y, qv.z, qv.w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float lo = __uint_as_float(u[j] << 16), hi = __uint_as_float(u[j] & 0xffff0000u);
+            if (tw == 0) {
+              chv[3 + 8 * hlf + 2 * j] += lo * tw4[dx];  // twin 0 keeps rgb in slots 0..2
+              chv[3 + 8 * hlf + 2 * j + 1] += hi * tw4[dx];
+            } else {
+              chv[8 * hlf + 2 * j] += lo * tw4[dx]; chv[8 * hlf + 2 * j + 1] += hi * tw4[dx];
+            }
+          }
+        }
+      }
+    }
+    if (want_rgb) {
+      const float fx = (gx + 1.f) * 0.5f * (float)(a.W - 1), fy = (gy + 1.f) * 0.5f * (float)(a.H - 1);
+      const float x0f = floorf(fx), y0f = floorf(fy);
+      const int x0 = (int)x0f, y0 = (int)y0f;
+      const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
+      const float* base = a.rgba + (long long)vc * a.H * a.W * 4;
+      float4 tr[4];
+      float twr[4];
+#pragma unroll
+      for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 2; ++dx) {
+          const int xi = x0 + dx, yi = y0 + dy;
+          const bool in = valid && xi >= 0 && xi < a.W && yi >= 0 && yi < a.H;
+          twr[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
+          const int xc = min(max(xi, 0), a.W - 1), yc = min(max(yi, 0), a.H - 1);
+          tr[2 * dy + dx] = __ldg(reinterpret_cast<const float4*>(base + ((long long)yc * a.W + xc) * 4));
+        }
+#pragma unroll
+      for (int tp = 0; tp < 4; ++tp) {
+        rgb[0] += tr[tp].x * twr[tp]; rgb[1] += tr[tp].y * twr[tp]; rgb[2] += tr[tp].z * twr[tp];
+      }
+    }
+  }
+
+  float rd[4];
+  {
+    float a0 = a.cams.tgt[0] - p3[0], a1 = a.cams.tgt[1] - p3[1], a2 = a.cams.tgt[2] - p3[2];
+    normalize3(a0, a1, a2);
+    float b0 = cam[12] - q3[0], b1 = cam[13] - q3[1], b2 = cam[14] - q3[2];
+    normalize3(b0, b1, b2);
+    rd[0] = a0 - b0; rd[1] = a1 - b1; rd[2] = a2 - b2;
+    rd[3] = a0 * b0 + a1 * b1 + a2 * b2;
+    normalize3(rd[0], rd[1], rd[2]);
+  }
+
+  float mask = mask_proj;
+  if (ST && a.mask_rgb) mask *= ((rgb[0] + rgb[1] + rgb[2]) > 1e-3f) ? 1.f : 0.f;
+  if (tw == 0) {
+    chv[0] = rgb[0]; chv[1] = rgb[1]; chv[2] = rgb[2];
+    if (valid) {
+      a.mask_proj[m] = mask_proj;
+      if (ST) {
+        a.mask_eff[m] = mask;
+        reinterpret_cast<float4*>(a.ray_diff)[m] = make_float4(rd[0], rd[1], rd[2], rd[3]);
+        a.rgb_in[m * 3] = rgb[0]; a.rgb_in[m * 3 + 1] = rgb[1]; a.rgb_in[m * 3 + 2] = rgb[2];
+      }
+    }
+  }
+  if (!ST) {  // dynamic: + time feature on this twin's channels (mlp_network.py:244-247)
+    const int c0 = tw == 0 ? 0 : 19, nc = tw == 0 ? 19 : 16;
+#pragma unroll
+    for (int i = 0; i < 19; ++i)
+      if (i < nc) chv[i] = valid ? chv[i] + cst[C_DFEAT + c0 + i] : 0.f;
+  }
+
+  // ---- pooling weights (both twins) ----
+  float w1;
+  if (ST && a.anti_alias) {
+    const float e = ex2f(cst[C_MISC + 2] * (rd[3] - 1.f) * 1.4426950408889634f);
+    const float emin = group_min<VP>(valid ? e : INFINITY);
+    w1 = valid ? (e - emin) * mask : 0.f;
+  } else {
+    w1 = mask;
+  }
+  w1 = w1 / (group_sum<VP>(w1) + 1e-8f);
+  if (tw == 0) { s_w1[r] = w1; s_mk[r] = mask; }
+
+  // ---- first pooling of the gathered channels (row layout): per twin groups of
+  //      [mean8 | var8 | feat8], twin 0 at columns 0..71 (3 groups), twin 1 at 72..119 (2 groups) ----
+#pragma unroll
+  for (int g = 0; g < 3; ++g) {
+    if (tw == 1 && g == 2) break;
+    float o[24];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float fv = chv[8 * g + j];
+      const float s1 = group_sum<VP>(w1 * fv);
+      const float d = fv - s1;
+      const float s2 = group_sum<VP>(w1 * d * d);
+      o[j] = s1; o[8 + j] = s2; o[16 + j] = fv;
+    }
+    const int cb = 72 * tw + 24 * g;
+    store8_64(arow_pool, cb, o);
+    store8_64(arow_pool, cb + 8, o + 8);
+    store8_64(arow_pool, cb + 16, o + 16);
+  }
+  if (!ST && tw == 1) {  // dynamic: K padding 120..127
+    const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    store8_64(arow_pool, 120, z);
+  }
+
+  if (ST) {
+    // ---- ray_dir_fc.0 operand: component-major PE, 56 columns per twin (layout in view_wg_build) ----
+    float pl6[6];
+    {
+      const float ox = cam[12], oy = cam[13], oz = cam[14];
+      float dx = p3[0] - ox, dy = p3[1] - oy, dz = p3[2] - oz;
+      normalize3(dx, dy, dz);
+      pl6[0] = dx; pl6[1] = dy; pl6[2] = dz;
+      pl6[3] = oy * dz - oz * dy;
+      pl6[4] = oz * dx - ox * dz;
+      pl6[5] = ox * dy - oy * dx;
+    }
+    // each 8-column group is stored as soon as it is complete (short live ranges)
+    float xin[56];
+    if (tw == 0) {
+      pe_comp(p3[0], xin);         store8_64(arow_pe, 0, xin);
+      pe_comp(p3[1], xin + 11);    store8_64(arow_pe, 8, xin + 8);
+      pe_comp(p3[2], xin + 22);    store8_64(arow_pe, 16, xin + 16); store8_64(arow_pe, 24, xin + 24);
+      pe_comp(pl6[0], xin + 33);   store8_64(arow_pe, 32, xin + 32);
+      pe_comp(pl6[1], xin + 44);   xin[55] = 0.f;
+      store8_64(arow_pe, 40, xin + 40);  store8_64(arow_pe, 48, xin + 48);
+    } else {
+      pe_comp(pl6[2], xin);        store8_64(arow_pe, 56, xin);
+      pe_comp(pl6[3], xin + 11);   store8_64(arow_pe, 64, xin + 8);
+      pe_comp(pl6[4], xin + 22);   store8_64(arow_pe, 72, xin + 16); store8_64(arow_pe, 80, xin + 24);
+      pe_comp(pl6[5], xin + 33);   store8_64(arow_pe, 88, xin + 32);
+      xin[44] = rd[0]; xin[45] = rd[1]; xin[46] = rd[2]; xin[47] = rd[3];
+#pragma unroll
+      for (int i = 48; i < 56; ++i) xin[i] = 0.f;
+      store8_64(arow_pe, 96, xin + 40);  store8_64(arow_pe, 104, xin + 48);
+    }
+  }
+}
+
+template <int VP, bool ST>
+__global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_constant__ ViewFusedArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem;
   uint8_t* atiles = smem + kWgRing * kWgStage;
@@ -67,11 +345,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
   const int tid = threadIdx.x, lane = tid & 31;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);  // warpgroup index, uniform to the compiler
   const uint32_t bar0 = smem_u32(bars);
+  // consumer c's operand tiles: filled by the front end (128 arrivals), free again (4 warps arrive)
+  const uint32_t tiles_full = bar0 + 8u * (2 * kWgRing), tiles_empty = tiles_full + 16u;
   stage_chunks(s_tab, a.chunks, a.nchunks);
   if (tid == 0) {
     for (int i = 0; i < kWgRing; ++i) {
       mbar_init(bar0 + 8u * i, 1);
       mbar_init(bar0 + 8u * (kWgRing + i), 8);
+    }
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(tiles_full + 8u * c, 128);
+      mbar_init(tiles_empty + 8u * c, 4);
     }
     mbar_fence_init();
   }
@@ -103,259 +387,90 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
 
   const long long n_rows = a.P * VP;
   const int n_iter = (int)((n_rows + 127) / 128);
-  if (wg == 2) {
-    setmaxnreg_dec<kProducerRegs>();
-    if (tid == 256) producer_loop<kWgRing, kWgStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
+  const int t = tid & 127;
+  if (wg == 3) {
+    setmaxnreg_dec<kViewProducerRegs>();
+    if (t == 0) producer_loop<kWgRing, kWgStage>(s_tab, a.nchunks, a.wimg, n_iter, ring, bar0);
     return;
   }
-  setmaxnreg_inc<kConsumerRegs>();
+  if (wg == 2) {
+    setmaxnreg_dec<kViewFrontRegs>();
+    PhaseClock pc{a, 2};
+    pc.start();
+    uint32_t k = 0;  // iterations handed over to each consumer so far
+    for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++k) {
+#pragma unroll 1
+      for (int c = 0; c < 2; ++c) {
+        if (k > 0) mbar_wait(tiles_empty + 8u * c, (k - 1) & 1);
+        pc.mark(PH_HANDOFF, 0);
+        front_end<VP, ST>(a, cst, t, (long long)it * 128 + 64 * c, atiles + c * kWgATile,
+                          atiles + c * kWgATile + kPeBytes, cst + C_W1 + 64 * c, cst + C_MK + 64 * c);
+        fence_proxy_async_smem();
+        mbar_arrive(tiles_full + 8u * c);
+        pc.mark(PH_FRONT, 0);
+      }
+      pc.iteration();
+    }
+    pc.finish();
+    return;
+  }
+  setmaxnreg_inc<kViewConsumerRegs>();
 
-  const int t = tid & 127, ww = t >> 5, q = lane & 3;
-  uint8_t* pe_tile = atiles + wg * kWgATile;
-  uint8_t* pool_tile = pe_tile + kPeBytes;
-  const uint32_t pe_addr = smem_u32(pe_tile), pool_addr = smem_u32(pool_tile);
-  float* s_w1 = cst + C_W1 + 64 * wg;
-  float* s_mk = cst + C_MK + 64 * wg;
-  // row layout (front end): twin tw of row r
-  const int tw = t >> 6, r = t & 63, v = r & (VP - 1);
-  uint8_t* arow_pe = pe_tile + (r >> 3) * 128 + (r & 7) * 16;
-  uint8_t* arow_pool = pool_tile + (r >> 3) * 128 + (r & 7) * 16;
+  const int ww = t >> 5, q = lane & 3;
+  uint8_t* pool_tile = atiles + wg * kWgATile + kPeBytes;
+  const uint32_t pe_addr = smem_u32(atiles + wg * kWgATile), pool_addr = smem_u32(pool_tile);
+  const float* s_w1 = cst + C_W1 + 64 * wg;
+  const float* s_mk = cst + C_MK + 64 * wg;
   // fragment layout: rows fr[h] of the half-tile
   const int fr[2] = {16 * ww + (lane >> 2), 16 * ww + (lane >> 2) + 8};
 
-  const bool prof = a.dbg != nullptr && blockIdx.x == 0 && t == 0;
-  Ring rg{ring, bar0, 0u, prof, 0};
-  int dbg_n = 0;
-  const long long t_begin = prof ? clock64() : 0;
-#define TS()                                                          \
-  do {                                                                \
-    if (prof && dbg_n < 64) a.dbg[wg * 64 + dbg_n++] = clock64();     \
-  } while (0)
+  PhaseClock pc{a, wg};
+  Ring rg{ring, bar0, 0u, pc.on(), 0};
+  pc.start();
+#define TS(ph) pc.mark(ph, rg.wait_cycles)
+  // The consumers issue their layers in turn (named barrier 3 + w: warpgroup w's turn, both warpgroups count), so
+  // one warpgroup's epilogue runs while the tensor cores work on the other's layer.  A warpgroup keeps the turn
+  // until its layer is issued, all chunks but the last retired.  Consumer 0 starts; consumer 1 does not pass the
+  // turn after its very last layer.
+  auto in_turn = [&](auto issue, bool pass) {
+    named_bar_sync(3 + wg, 256);
+    TS(PH_BAR);
+    issue();
+    if (pass) named_bar_arrive(4 - wg, 256);
+  };
+  if (wg == 1) named_bar_arrive(3, 256);
 
-  const float wh = a.w_img, hh = a.h_img;
-  const bool want_rgb = (tw == 0) || (ST && a.mask_rgb);
-
-  for (int it = blockIdx.x; it < n_iter; it += gridDim.x) {
+  uint32_t k = 0;  // iterations of this warpgroup so far
+  for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++k) {
     const long long row0 = (long long)it * 128 + 64 * wg;  // first row of this warpgroup
-    // ---- front end, row layout ----
-    const long long pl = (row0 + r) / VP;
-    const bool pt_ok = pl < a.P;
-    const bool valid = pt_ok && v < a.V;
-    const long long m = pl * a.V + v;
-    float p3[3] = {0.f, 0.f, 0.f};
-    if (pt_ok) { p3[0] = a.pts[pl * 3]; p3[1] = a.pts[pl * 3 + 1]; p3[2] = a.pts[pl * 3 + 2]; }
-    float q3[3] = {p3[0], p3[1], p3[2]};
-    if (!ST && valid) {
-      const float* qq = a.pts_seq + ((long long)v * a.seq_stride + pl) * 3;
-      q3[0] = qq[0]; q3[1] = qq[1]; q3[2] = qq[2];
-    }
-    // the previous iteration's wgmmas of every warp have retired before the operand tiles are rewritten
-    named_bar_sync(1 + wg, 128);
-    TS();  // 0: iteration start
-
-    const int vc = valid ? v : 0;
-    const float* cam = cst + C_CAMS + 16 * vc;
-    float pu, pv;
-    bool front;
-    project_point(cam, q3[0], q3[1], q3[2], pu, pv, front);
-    const bool inb = (pu <= wh - 1.f) && (pu >= 0.f) && (pv <= hh - 1.f) && (pv >= 0.f);
-    const float mask_proj = (valid && inb && front) ? 1.f : 0.f;
-
-    // ---- gather: this twin's 16 bf16 feature channels (+ RGB) at the 4 bilinear taps ----
-    float chv[24];
-#pragma unroll
-    for (int i = 0; i < 24; ++i) chv[i] = 0.f;
-    float rgb[3] = {0.f, 0.f, 0.f};
-    {
-      const float gx = 2.f * pu / (wh - 1.f) - 1.f, gy = 2.f * pv / (hh - 1.f) - 1.f;
-      uint4 tf[8];
-      float4 tr[4];
-      float tw4[4], twr[4];
-      {
-        const float fx = (gx + 1.f) * 0.5f * (float)(a.w - 1), fy = (gy + 1.f) * 0.5f * (float)(a.h - 1);
-        const float x0f = floorf(fx), y0f = floorf(fy);
-        const int x0 = (int)x0f, y0 = (int)y0f;
-        const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
-        const uint16_t* base = a.feat_bf + (long long)vc * a.h * a.w * kC + 16 * tw;
-#pragma unroll
-        for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-          for (int dx = 0; dx < 2; ++dx) {
-            // out-of-range taps (and padding rows) load a clamped texel with weight 0
-            const int xi = x0 + dx, yi = y0 + dy;
-            const bool in = valid && xi >= 0 && xi < a.w && yi >= 0 && yi < a.h;
-            tw4[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
-            const int xc = min(max(xi, 0), a.w - 1), yc = min(max(yi, 0), a.h - 1);
-            const uint4* tp = reinterpret_cast<const uint4*>(base + ((long long)yc * a.w + xc) * kC);
-            tf[2 * (2 * dy + dx)] = __ldg(tp);
-            tf[2 * (2 * dy + dx) + 1] = __ldg(tp + 1);
-          }
-      }
-      if (want_rgb) {
-        const float fx = (gx + 1.f) * 0.5f * (float)(a.W - 1), fy = (gy + 1.f) * 0.5f * (float)(a.H - 1);
-        const float x0f = floorf(fx), y0f = floorf(fy);
-        const int x0 = (int)x0f, y0 = (int)y0f;
-        const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
-        const float* base = a.rgba + (long long)vc * a.H * a.W * 4;
-#pragma unroll
-        for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-          for (int dx = 0; dx < 2; ++dx) {
-            const int xi = x0 + dx, yi = y0 + dy;
-            const bool in = valid && xi >= 0 && xi < a.W && yi >= 0 && yi < a.H;
-            twr[2 * dy + dx] = in ? (dx ? ax : bx) * (dy ? ay : by) : 0.f;
-            const int xc = min(max(xi, 0), a.W - 1), yc = min(max(yi, 0), a.H - 1);
-            tr[2 * dy + dx] = __ldg(reinterpret_cast<const float4*>(base + ((long long)yc * a.W + xc) * 4));
-          }
-      }
-#pragma unroll
-      for (int tp = 0; tp < 4; ++tp) {
-#pragma unroll
-        for (int hlf = 0; hlf < 2; ++hlf) {
-          const uint4 qv = tf[2 * tp + hlf];
-          const uint32_t u[4] = {qv.x, qv.y, qv.z, qv.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float lo = __uint_as_float(u[j] << 16), hi = __uint_as_float(u[j] & 0xffff0000u);
-            if (tw == 0) {
-              chv[3 + 8 * hlf + 2 * j] += lo * tw4[tp];  // twin 0 keeps rgb in slots 0..2
-              chv[3 + 8 * hlf + 2 * j + 1] += hi * tw4[tp];
-            } else {
-              chv[8 * hlf + 2 * j] += lo * tw4[tp]; chv[8 * hlf + 2 * j + 1] += hi * tw4[tp];
-            }
-          }
-        }
-      }
-      if (want_rgb) {
-#pragma unroll
-        for (int tp = 0; tp < 4; ++tp) {
-          rgb[0] += tr[tp].x * twr[tp]; rgb[1] += tr[tp].y * twr[tp]; rgb[2] += tr[tp].z * twr[tp];
-        }
-      }
-    }
-
-    float rd[4];
-    {
-      float a0 = a.cams.tgt[0] - p3[0], a1 = a.cams.tgt[1] - p3[1], a2 = a.cams.tgt[2] - p3[2];
-      normalize3(a0, a1, a2);
-      float b0 = cam[12] - q3[0], b1 = cam[13] - q3[1], b2 = cam[14] - q3[2];
-      normalize3(b0, b1, b2);
-      rd[0] = a0 - b0; rd[1] = a1 - b1; rd[2] = a2 - b2;
-      rd[3] = a0 * b0 + a1 * b1 + a2 * b2;
-      normalize3(rd[0], rd[1], rd[2]);
-    }
-
-    float mask = mask_proj;
-    if (ST && a.mask_rgb) mask *= ((rgb[0] + rgb[1] + rgb[2]) > 1e-3f) ? 1.f : 0.f;
-    if (tw == 0) {
-      chv[0] = rgb[0]; chv[1] = rgb[1]; chv[2] = rgb[2];
-      if (valid) {
-        a.mask_proj[m] = mask_proj;
-        if (ST) {
-          a.mask_eff[m] = mask;
-          reinterpret_cast<float4*>(a.ray_diff)[m] = make_float4(rd[0], rd[1], rd[2], rd[3]);
-          a.rgb_in[m * 3] = rgb[0]; a.rgb_in[m * 3 + 1] = rgb[1]; a.rgb_in[m * 3 + 2] = rgb[2];
-        }
-      }
-    }
-    if (!ST) {  // dynamic: + time feature on this twin's channels (mlp_network.py:244-247)
-      const int c0 = tw == 0 ? 0 : 19, nc = tw == 0 ? 19 : 16;
-#pragma unroll
-      for (int i = 0; i < 19; ++i)
-        if (i < nc) chv[i] = valid ? chv[i] + cst[C_DFEAT + c0 + i] : 0.f;
-    }
-
-    // ---- pooling weights (both twins) ----
-    float w1;
-    if (ST && a.anti_alias) {
-      const float e = ex2f(cst[C_MISC + 2] * (rd[3] - 1.f) * 1.4426950408889634f);
-      const float emin = group_min<VP>(valid ? e : INFINITY);
-      w1 = valid ? (e - emin) * mask : 0.f;
-    } else {
-      w1 = mask;
-    }
-    w1 = w1 / (group_sum<VP>(w1) + 1e-8f);
-    if (tw == 0) { s_w1[r] = w1; s_mk[r] = mask; }
-
-    // ---- first pooling of the gathered channels (row layout): per twin groups of
-    //      [mean8 | var8 | feat8], twin 0 at columns 0..71 (3 groups), twin 1 at 72..119 (2 groups) ----
-#pragma unroll
-    for (int g = 0; g < 3; ++g) {
-      if (tw == 1 && g == 2) break;
-      float o[24];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float fv = chv[8 * g + j];
-        const float s1 = group_sum<VP>(w1 * fv);
-        const float d = fv - s1;
-        const float s2 = group_sum<VP>(w1 * d * d);
-        o[j] = s1; o[8 + j] = s2; o[16 + j] = fv;
-      }
-      const int cb = 72 * tw + 24 * g;
-      store8_64(arow_pool, cb, o);
-      store8_64(arow_pool, cb + 8, o + 8);
-      store8_64(arow_pool, cb + 16, o + 16);
-    }
-    if (!ST && tw == 1) {  // dynamic: K padding 120..127
-      const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      store8_64(arow_pool, 120, z);
-    }
+    mbar_wait(tiles_full + 8u * wg, k & 1);
+    TS(PH_HANDOFF);
+    // the rows' pooling weights and masks stay in registers: the front end rewrites them once base_fc.0 has retired
+    const float w1r[2] = {s_w1[fr[0]], s_w1[fr[1]]}, mk[2] = {s_mk[fr[0]], s_mk[fr[1]]};
 
     float acc[128];  // accumulators of the 256-wide layers (the first 64 / 24 for the narrower ones)
     if (ST) {
-      // ---- ray_dir_fc.0 operand: component-major PE, 56 columns per twin (layout in view_wg_build) ----
-      float pl6[6];
-      {
-        const float ox = cam[12], oy = cam[13], oz = cam[14];
-        float dx = p3[0] - ox, dy = p3[1] - oy, dz = p3[2] - oz;
-        normalize3(dx, dy, dz);
-        pl6[0] = dx; pl6[1] = dy; pl6[2] = dz;
-        pl6[3] = oy * dz - oz * dy;
-        pl6[4] = oz * dx - ox * dz;
-        pl6[5] = ox * dy - oy * dx;
-      }
-      // each 8-column group is stored as soon as it is complete (short live ranges)
-      float xin[56];
-      if (tw == 0) {
-        pe_comp(p3[0], xin);         store8_64(arow_pe, 0, xin);
-        pe_comp(p3[1], xin + 11);    store8_64(arow_pe, 8, xin + 8);
-        pe_comp(p3[2], xin + 22);    store8_64(arow_pe, 16, xin + 16); store8_64(arow_pe, 24, xin + 24);
-        pe_comp(pl6[0], xin + 33);   store8_64(arow_pe, 32, xin + 32);
-        pe_comp(pl6[1], xin + 44);   xin[55] = 0.f;
-        store8_64(arow_pe, 40, xin + 40);  store8_64(arow_pe, 48, xin + 48);
-      } else {
-        pe_comp(pl6[2], xin);        store8_64(arow_pe, 56, xin);
-        pe_comp(pl6[3], xin + 11);   store8_64(arow_pe, 64, xin + 8);
-        pe_comp(pl6[4], xin + 22);   store8_64(arow_pe, 72, xin + 16); store8_64(arow_pe, 80, xin + 24);
-        pe_comp(pl6[5], xin + 33);   store8_64(arow_pe, 88, xin + 32);
-        xin[44] = rd[0]; xin[45] = rd[1]; xin[46] = rd[2]; xin[47] = rd[3];
-#pragma unroll
-        for (int i = 48; i < 56; ++i) xin[i] = 0.f;
-        store8_64(arow_pe, 96, xin + 40);  store8_64(arow_pe, 104, xin + 48);
-      }
-      fence_proxy_async_smem();
-      named_bar_sync(1 + wg, 128);
-      TS();  // 1: F1 issue
-      layer_ss<256, 7>(acc, pe_addr, rg);
+      in_turn([&] { layer_ss256<7>(acc, pe_addr, rg); }, true);
       layer_finish<256>(acc, rg);
-      TS();  // 2: F1 done
+      TS(PH_F1);
       // ---- F1 epilogue -> ray_dir_fc.2 (register A) ----
       {
         uint32_t af[16][4];
         bias_elu<256>(acc, cst + C_B1, q);
         to_afrag<16>(acc, af);
-        layer_rs<48, 16>(acc, af, rg);
+        TS(PH_F1_EPI);
+        in_turn([&] { layer_rs_issue<48, 16>(acc, af, rg); }, true);
+        layer_finish<48>(acc, rg);
       }
-      TS();  // 3: F2 done
+      TS(PH_F2);
       // ---- src_feat * ref_feat (35 channels, fragment columns j < 5) and their pooling over views:
       //      mean at column 120 + n, var at 160 + n, feat at 200 + n ----
-      float f[2][10], w1h[2];
+      float f[2][10];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long prow = (row0 + fr[h]) / VP;
         const bool ok = prow < a.P && ((fr[h] & (VP - 1)) < a.V);
         const float* rf = a.ref_feat + (ok ? prow / a.S : 0) * kF;
-        w1h[h] = s_w1[fr[h]];
 #pragma unroll
         for (int j = 0; j < 5; ++j)
 #pragma unroll
@@ -370,11 +485,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int i = 2 * j + e;
-          float tv[2] = {w1h[0] * f[0][i], w1h[1] * f[1][i]}, s1[2], s2[2];
+          float tv[2] = {w1r[0] * f[0][i], w1r[1] * f[1][i]}, s1[2], s2[2];
           views_sum<VP>(tv, s1);
           const float d0 = f[0][i] - s1[0], d1 = f[1][i] - s1[1];
-          tv[0] = w1h[0] * d0 * d0;
-          tv[1] = w1h[1] * d1 * d1;
+          tv[0] = w1r[0] * d0 * d0;
+          tv[1] = w1r[1] * d1 * d1;
           views_sum<VP>(tv, s2);
           mu[0][e] = s1[0]; mu[1][e] = s1[1]; va[0][e] = s2[0]; va[1][e] = s2[1];
         }
@@ -386,21 +501,28 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
           store2_64(pool_tile, fr[h], 200 + n, f[h][2 * j], f[h][2 * j + 1]);
         }
       }
+      TS(PH_F2_EPI);
+      // every warp's columns 120..239 are in place before base_fc.0 reads them
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);
+      TS(PH_BAR);
     }
-    fence_proxy_async_smem();
-    named_bar_sync(1 + wg, 128);
-    TS();  // 4: F3 issue
-    layer_ss<256, ST ? 15 : 8>(acc, pool_addr, rg);
+    in_turn([&] { layer_ss256<ST ? 15 : 8>(acc, pool_addr, rg); }, true);
     layer_finish<256>(acc, rg);
-    TS();  // 5: F3 done
+    // both operand tiles and the rows' pooling weights / masks are free for the next iteration's front end
+    __syncwarp();
+    if (lane == 0) mbar_arrive(tiles_empty + 8u * wg);
+    TS(PH_F3);
     // ---- base_fc.0 epilogue -> base_fc.2 (register A) ----
     {
       uint32_t af[16][4];
       bias_elu<256>(acc, cst + C_B3, q);
       to_afrag<16>(acc, af);
-      layer_rs<128, 16>(acc, af, rg);
+      TS(PH_F3_EPI);
+      in_turn([&] { layer_rs_issue<128, 16>(acc, af, rg); }, true);
+      layer_finish<128>(acc, rg);
     }
-    TS();  // 6: F4 done
+    TS(PH_F4);
     // ---- x = ELU(base_fc.2) (fp32 residual); vis_fc.0 on bf16(x): its row scale w1 applies to the accumulator ----
     float x[64];
     bias_elu<128>(acc, cst + C_B4, q);
@@ -409,11 +531,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
     {
       uint32_t af[8][4];
       to_afrag<8>(x, af);
-      layer_rs<128, 8>(acc, af, rg);
+      TS(PH_F4_EPI);
+      in_turn([&] { layer_rs_issue<128, 8>(acc, af, rg); }, true);
+      layer_finish<128>(acc, rg);
     }
-    TS();  // 7: F5 done
+    TS(PH_F5);
     // ---- h = ELU(w1 (W x) + b) and the row's visibility logit (quad sum) -> vis_fc.2 ----
-    const float w1r[2] = {s_w1[fr[0]], s_w1[fr[1]]}, mk[2] = {s_mk[fr[0]], s_mk[fr[1]]};
     float part[2] = {0.f, 0.f};
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -433,9 +556,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
     {
       uint32_t af[8][4];
       to_afrag<8>(acc, af);
-      layer_rs<128, 8>(acc, af, rg);
+      TS(PH_F5_EPI);
+      in_turn([&] { layer_rs_issue<128, 8>(acc, af, rg); }, true);
+      layer_finish<128>(acc, rg);
     }
-    TS();  // 8: F6 done
+    TS(PH_F6);
     // ---- x += ELU(vis_fc.2); bf16(x) is vis_fc2.0's operand (vis1 applies to its accumulator) and, for the
     //      static net, the blending head's input (X tile image, rows = view slots) ----
     float vis1[2];
@@ -455,9 +580,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
           for (int k = 0; k < 4; ++k)  // af[s][k]: row fr[k & 1], 8-column group 2 s + (k >> 1)
             *reinterpret_cast<uint32_t*>(xo + tile_image_off(row0 + fr[k & 1], 2 * s + (k >> 1), 16) + 4 * q) = af[s][k];
       }
-      layer_rs<128, 8>(acc, af, rg);
+      TS(PH_F6_EPI);
+      in_turn([&] { layer_rs_issue<128, 8>(acc, af, rg); }, wg == 0 || it + (int)gridDim.x < n_iter);
+      layer_finish<128>(acc, rg);
     }
-    TS();  // 9: F7 done
+    TS(PH_F7);
     // ---- vis2 = sigmoid(vis_fc2.2 . ELU(vis1 (W x) + b)) * mask ----
     float p7[2] = {0.f, 0.f};
 #pragma unroll
@@ -478,6 +605,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
       const int vh = fr[h] & (VP - 1);
       if (ST && q == 0 && prow < a.P && vh < a.V) a.vis2[prow * a.V + vh] = vis2[h];
     }
+    TS(PH_F7_EPI);
 
     // ---- second pooling: mean / second moment of x over the point's views, reduce-scattered over the row lanes:
     //      afterwards lane l holds columns 8 j0 + 2 q + {0, 1} and 8 (j0 + 1) + 2 q + {0, 1} ----
@@ -534,13 +662,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) view_wg_kernel(const __grid_con
         }
       }
     }
-    TS();  // 10: outputs done
+    TS(PH_POOL2);
+    pc.iteration();
   }
 #undef TS
-  if (prof) {
-    a.dbg[128 + wg] = clock64() - t_begin;  // warpgroup lifetime
-    a.dbg[130 + wg] = rg.wait_cycles;                // cycles waiting for weight chunks
-  }
+  pc.finish();
 }
 
 }  // namespace
@@ -633,11 +759,11 @@ int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
   const bool st_net = n->kind == DYN_NET_STATIC;
   ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
   if (st_net) {
-    if (VP == 8) view_wg_kernel<8, true><<<grid, kWgThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, true><<<grid, kWgThreads, kWgSmem, st>>>(a);
+    if (VP == 8) view_wg_kernel<8, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
   } else {
-    if (VP == 8) view_wg_kernel<8, false><<<grid, kWgThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, false><<<grid, kWgThreads, kWgSmem, st>>>(a);
+    if (VP == 8) view_wg_kernel<8, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
   }
   DYN_LAUNCH_CHECK();
   return DYN_OK;

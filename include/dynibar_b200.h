@@ -405,10 +405,16 @@ size_t dyn_debug_tile_image_off(long long row, int kgroup, int kgroups);
  * with DYN_E_INVALID. */
 void dyn_debug_set_view_kernel(int which);
 
-/* profiling hook: when set, block 0 of the fused static per-view kernel writes clock64()
- * phase timestamps into dev_buf (zeroed, >= 616 int64): the twin-warp kernels [2 twins][64] and
- * the MMA warpgroup's totals from index 128; the warpgroup kernel [2 warpgroups][64] at its layer
- * boundaries, then per warpgroup its lifetime ([128 + wg]) and the cycles it waited for weights ([130 + wg]). */
+/* profiling hook: when set, block 0 of each fused per-view kernel launch writes clock64() data into
+ * dev_buf (zeroed, >= 1232 int64): the static net's launches into [0, 616), the dynamic net's into
+ * [616, 1232); a later launch of the same net overwrites an earlier one.  Within a net's part:
+ *   warpgroup kernel: per warpgroup w (0, 1: consumers, 2: front end), 32 counters at [32 w, 32 w + 32):
+ *     the cycles of every phase accumulated over all of block 0's iterations (index = enum Phase in
+ *     csrc/view_wg.cu: front end, named-barrier waits, weight-ring waits, each layer's issue-to-finish and
+ *     each epilogue, second pooling and outputs, waits at the front-end handoff), [32 w + 30] its
+ *     iterations, [32 w + 31] its lifetime;
+ *   twin-warp kernel: timestamps [2 twins][64] and the MMA warpgroup's totals from index 128.
+ * tools/view_phases.py prints the warpgroup kernel's counters as shares of the lifetime. */
 void dyn_debug_set_view_timestamps(long long* dev_buf);
 
 /* unit-test hook: while any pointer is set, every dyn_net_static_fused / dyn_net_dynamic_fused call copies the
