@@ -49,6 +49,8 @@ SIGNATURES = {
     "dyn_occlusion_weights": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "dyn_project_gather": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
                                 _vp, _vp, _vp, _vp, _vp]),
+    "dyn_project_gather_mc": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
+                                   _vp, _vp, _vp, _vp, _vp]),
     "dyn_compute_projections": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "dyn_compute_angle": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     "dyn_plucker_ref": (_i, [_vp, _vp, _i, _vp, _vp]),
@@ -61,6 +63,8 @@ SIGNATURES = {
     "dyn_rgbs_rgba": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "dyn_net_static_fused": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i,
                                   _i, _vp, _vp, _vp, _sz, _vp]),
+    "dyn_net_static_fused_mc": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i,
+                                     _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "dyn_net_dynamic_fused": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _i,
                                    _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "dyn_composite": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),

@@ -273,13 +273,25 @@ int dyn_net_static_fused(dyn_net_t net, const float* pts, const float* ray_o, co
                          const void* feat_cl, int R, int S, int V, int H, int W, int C, int h, int w,
                          float* raw, float* mask_out, void* workspace, size_t workspace_bytes,
                          void* stream) {
+  return dyn_net_static_fused_mc(net, pts, ray_o, ray_d, query_cam, 1, nullptr, src_rgbs, src_cams, feat_cl, R, S,
+                                 V, H, W, C, h, w, raw, mask_out, workspace, workspace_bytes, stream);
+}
+
+int dyn_net_static_fused_mc(dyn_net_t net, const float* pts, const float* ray_o, const float* ray_d,
+                            const float* query_cams, int K, const int* query_idx, const float* src_rgbs,
+                            const float* src_cams, const void* feat_cl, int R, int S, int V, int H, int W, int C,
+                            int h, int w, float* raw, float* mask_out, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+  if (K < 1 || K > kMaxTargets) return fail(DYN_E_INVALID, "target camera count K = %d outside 1..%d", K, kMaxTargets);
+  if (K > 1 && query_idx == nullptr) return fail(DYN_E_INVALID, "K = %d target cameras need a per-ray camera index", K);
   if (R == 0) return DYN_OK;  // empty batch: nothing to do (pointers may be null)
-  DYN_CHECK_ARG(net && net->kind == DYN_NET_STATIC && pts && ray_o && ray_d && query_cam && src_rgbs);
+  DYN_CHECK_ARG(net && net->kind == DYN_NET_STATIC && pts && ray_o && ray_d && query_cams && src_rgbs);
   DYN_CHECK_ARG(src_cams && feat_cl && raw && mask_out && workspace && C == kC);
   DYN_CHECK_ARG(R >= 0 && S >= 1 && V >= 1 && V <= 16);
   if (R == 0) return DYN_OK;
-  return net_static_fused(net, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, feat_cl, R, S, V, H, W,
-                          h, w, raw, mask_out, workspace, workspace_bytes, (cudaStream_t)stream);
+  return net_static_fused(net, pts, ray_o, ray_d, query_cams, K, K > 1 ? query_idx : nullptr, src_rgbs, src_cams,
+                          feat_cl, R, S, V, H, W, h, w, raw, mask_out, workspace, workspace_bytes,
+                          (cudaStream_t)stream);
 }
 
 int dyn_net_dynamic_fused(dyn_net_t net, const float* pts, const float* pts_seq, const float* ray_dir,

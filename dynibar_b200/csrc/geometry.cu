@@ -202,11 +202,12 @@ __global__ void rgb_to_rgba_kernel(const float* __restrict__ in, float4* __restr
 // with coalesced 16-byte stores.
 // Bilinear, zero padding, align_corners=True, coordinates normalised by the
 // SOURCE IMAGE size for both maps (projection.py:22-30, :143-158).
+// tgt_idx [R] (multi-camera launches, else null): ray r's target camera centre is cams.tgts[tgt_idx[r]].
 __global__ void __launch_bounds__(256)
 project_gather_kernel(const float* __restrict__ xyz_st, const float* __restrict__ xyz,
                       const float* __restrict__ rgbs, const float* __restrict__ feat_cl,
-                      const __grid_constant__ ViewCams cams, int V, long long N /* R*S */, int H,
-                      int W, int h, int w, float* __restrict__ rgb_feat,
+                      const __grid_constant__ ViewCams cams, const int* __restrict__ tgt_idx, int S, int V,
+                      long long N /* R*S */, int H, int W, int h, int w, float* __restrict__ rgb_feat,
                       float* __restrict__ ray_diff, float* __restrict__ mask) {
   // A block owns 256 consecutive (point, view) pairs.  Phase 1: every thread projects ONE pair (all lanes
   // busy; coalesced mask / ray_diff stores) and leaves the sampling position in shared memory.  Phase 2:
@@ -240,7 +241,8 @@ project_gather_kernel(const float* __restrict__ xyz_st, const float* __restrict_
       const bool inb = (u <= cams.w_img - 1.f) && (u >= 0.f) && (vv <= cams.h_img - 1.f) && (vv >= 0.f);
       mask[gid] = (inb && front) ? 1.f : 0.f;
       // compute_angle, projection.py:61-101
-      float a0 = cams.tgt[0] - sx, a1 = cams.tgt[1] - sy, a2 = cams.tgt[2] - sz;
+      const float* tgt = tgt_idx != nullptr ? cams.tgts[tgt_idx[pt / S]] : cams.tgt;
+      float a0 = tgt[0] - sx, a1 = tgt[1] - sy, a2 = tgt[2] - sz;
       normalize3(a0, a1, a2);
       float b0 = cams.center[v][0] - x, b1 = cams.center[v][1] - y, b2 = cams.center[v][2] - z;
       normalize3(b0, b1, b2);
@@ -543,15 +545,17 @@ static int fetch_cams(const float* cams, int V, float* host, cudaStream_t st) {
 }
 
 int build_view_cams(const float* src_cams, int V, const float* query_cam, cudaStream_t st,
-                    ViewCams* vc) {
-  DYN_CHECK_ARG(V >= 1 && V <= kMaxViews);
-  static thread_local float host[34 * (kMaxViews + 1)];
+                    ViewCams* vc, int n_query) {
+  DYN_CHECK_ARG(V >= 1 && V <= kMaxViews && n_query >= 1 && n_query <= kMaxTargets);
+  static thread_local float host[34 * (kMaxViews + kMaxTargets)];
   int rc = fetch_cams(src_cams, V, host, st);
   if (rc) return rc;
   if (query_cam != nullptr) {
-    rc = fetch_cams(query_cam, 1, host + 34 * V, st);
+    rc = fetch_cams(query_cam, n_query, host + 34 * V, st);
     if (rc) return rc;
     for (int i = 0; i < 3; ++i) vc->tgt[i] = host[34 * V + 18 + i * 4 + 3];
+    for (int k = 0; k < n_query; ++k)
+      for (int i = 0; i < 3; ++i) vc->tgts[k][i] = host[34 * (V + k) + 18 + i * 4 + 3];
   }
   vc->h_img = host[0];
   vc->w_img = host[1];
@@ -721,14 +725,24 @@ int dyn_project_gather(const float* xyz_st, const float* xyz, const float* query
                        const float* src_rgbs, const float* src_cams, const float* featmaps, int V,
                        int R, int S, int H, int W, int C, int h, int w, float* feat_cl_ws,
                        float* rgb_feat, float* ray_diff, float* mask, void* stream) {
+  return dyn_project_gather_mc(xyz_st, xyz, query_cam, 1, nullptr, src_rgbs, src_cams, featmaps, V, R, S, H, W, C,
+                               h, w, feat_cl_ws, rgb_feat, ray_diff, mask, stream);
+}
+
+int dyn_project_gather_mc(const float* xyz_st, const float* xyz, const float* query_cams, int K,
+                          const int* query_idx, const float* src_rgbs, const float* src_cams,
+                          const float* featmaps, int V, int R, int S, int H, int W, int C, int h, int w,
+                          float* feat_cl_ws, float* rgb_feat, float* ray_diff, float* mask, void* stream) {
+  if (K < 1 || K > kMaxTargets) return fail(DYN_E_INVALID, "target camera count K = %d outside 1..%d", K, kMaxTargets);
+  if (K > 1 && query_idx == nullptr) return fail(DYN_E_INVALID, "K = %d target cameras need a per-ray camera index", K);
   if (R == 0) return DYN_OK;  // empty batch: nothing to do (pointers may be null)
-  DYN_CHECK_ARG(xyz_st && query_cam && src_rgbs && src_cams && featmaps && feat_cl_ws);
+  DYN_CHECK_ARG(xyz_st && query_cams && src_rgbs && src_cams && featmaps && feat_cl_ws);
   DYN_CHECK_ARG(rgb_feat && ray_diff && mask);
-  DYN_CHECK_ARG(C == kC && V >= 1 && V <= kMaxViews && H > 1 && W > 1 && h > 1 && w > 1);
+  DYN_CHECK_ARG(C == kC && V >= 1 && V <= kMaxViews && H > 1 && W > 1 && h > 1 && w > 1 && (K == 1 || S >= 1));
   if (R == 0) return DYN_OK;
   cudaStream_t st = (cudaStream_t)stream;
   ViewCams vc;
-  int rc = build_view_cams(src_cams, V, query_cam, st, &vc);
+  int rc = build_view_cams(src_cams, V, query_cams, st, &vc, K);
   if (rc) return rc;
   dim3 tb(32, 8), tg(cdiv(h * w, 32), cdiv(C, 32), V);
   to_channels_last_kernel<<<tg, tb, 0, st>>>(featmaps, feat_cl_ws, C, h * w);
@@ -736,8 +750,8 @@ int dyn_project_gather(const float* xyz_st, const float* xyz, const float* query
   long long N = (long long)R * S;
   ProfScope prof(PROF_GATHER, st);
   project_gather_kernel<<<cdiv(N * V, 256), 256, 0, st>>>(xyz_st, xyz, src_rgbs, feat_cl_ws, vc,
-                                                            V, N, H, W, h, w, rgb_feat, ray_diff,
-                                                            mask);
+                                                            K > 1 ? query_idx : nullptr, S, V, N, H, W, h,
+                                                            w, rgb_feat, ray_diff, mask);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }

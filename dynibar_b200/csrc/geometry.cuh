@@ -5,11 +5,15 @@
 
 namespace dyn {
 
+// target cameras of one multi-camera launch (dyn_net_static_fused_mc, dyn_project_gather_mc)
+constexpr int kMaxTargets = 16;
+
 struct ViewCams {
   float P[kMaxViews][12];   // rows 0..2 of K * inv(c2w)  (projection.py:46-48)
   float center[kMaxViews][3];  // c2w[:3,3]
   float tgt[3];             // target camera centre
   float h_img, w_img;       // train_cameras[0][:2] (projection.py:136)
+  float tgts[kMaxTargets][3];  // multi-camera launches: centre of target camera k (tgts[0] == tgt)
 };
 
 __device__ __forceinline__ void project_point(const float* P, float x, float y, float z, float& u,
@@ -24,8 +28,9 @@ __device__ __forceinline__ void project_point(const float* P, float x, float y, 
 }
 
 
+// query_cam: n_query target cameras [n_query,34] (n_query <= kMaxTargets) or null
 int build_view_cams(const float* src_cams, int V, const float* query_cam, cudaStream_t st,
-                    ViewCams* vc);
+                    ViewCams* vc, int n_query = 1);
 int launch_to_channels_last(const float* featmaps, float* out, int V, int C, int hw, cudaStream_t st);
 int launch_to_channels_last_bf16(const float* featmaps, void* out, int V, int C, int hw, cudaStream_t st);
 int launch_rgb_to_rgba(const float* rgbs, float* out, long long npix, cudaStream_t st);

@@ -22,10 +22,11 @@ int motion_f32(const dyn_net* n, const float* x, int ldx, bool time_is_column, f
                float* coeff, void* ws, size_t ws_bytes, int prec, cudaStream_t st);
 // fused DYN_PREC_BF16 path (per-view stage = nets_fused.cu)
 size_t net_fused_workspace(int kind, int R, int S, int V);
+// query_cams [K,34]; query_idx [R] (device) = target camera of each ray, null for one camera
 int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, const float* ray_d,
-                     const float* query_cam, const float* src_rgbs, const float* src_cams,
-                     const void* feat_cl, int R, int S, int V, int H, int W, int h, int w, float* raw,
-                     float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st);
+                     const float* query_cams, int K, const int* query_idx, const float* src_rgbs,
+                     const float* src_cams, const void* feat_cl, int R, int S, int V, int H, int W, int h,
+                     int w, float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st);
 int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, const float* ray_dir,
                       const float* query_cam, const float* src_rgbs, const float* src_cams,
                       const void* feat_cl, float time, int R, int S, int V, int H, int W, int h, int w,

@@ -1109,9 +1109,9 @@ static int capture_view_outputs(const ViewFusedArgs& va, long long p0, long long
 
 static int fill_view_args(ViewFusedArgs* a, const float* query_cam, const float* src_rgbs,
                           const float* src_cams, const void* feat_cl, int V, int S, int H, int W,
-                          int h, int w, cudaStream_t st) {
+                          int h, int w, cudaStream_t st, int n_query = 1) {
   memset(a, 0, sizeof(*a));
-  RUN(build_view_cams(src_cams, V, query_cam, st, &a->cams));
+  RUN(build_view_cams(src_cams, V, query_cam, st, &a->cams, n_query));
   a->h_img = a->cams.h_img; a->w_img = a->cams.w_img;
   a->rgba = src_rgbs; a->feat_bf = reinterpret_cast<const uint16_t*>(feat_cl);
   a->H = H; a->W = W; a->h = h; a->w = w; a->V = V; a->S = S;
@@ -1119,14 +1119,14 @@ static int fill_view_args(ViewFusedArgs* a, const float* query_cam, const float*
 }
 
 int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, const float* ray_d,
-                     const float* query_cam, const float* src_rgbs, const float* src_cams,
-                     const void* feat_cl, int R_all, int S, int V, int H, int W, int h, int w,
-                     float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+                     const float* query_cams, int K, const int* query_idx, const float* src_rgbs,
+                     const float* src_cams, const void* feat_cl, int R_all, int S, int V, int H, int W, int h,
+                     int w, float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st) {
   const StaticLayout& L = n->sl;
   const int prec = DYN_PREC_BF16;
   RUN(check_attention_samples(S, true));
   ViewFusedArgs va{};
-  RUN(fill_view_args(&va, query_cam, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st));
+  RUN(fill_view_args(&va, query_cams, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st, K));
   const int RC = net_rows_per_chunk(S, V);
   for (int r0 = 0; r0 < R_all; r0 += RC) {
     const int R = (R_all - r0) < RC ? (R_all - r0) : RC;
@@ -1140,6 +1140,7 @@ int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, con
     RUN(launch_pe(d.refpl, 6, 6, 0, 0.f, 5, false, R, d.refpe, st));
     RUN(launch_linear(L1(n, L.ref_feat, d.refpe, d.reff, R, ACT_NONE), st));
     va.pts = pts + p0 * 3; va.pts_seq = nullptr; va.P = P;
+    va.tgt_idx = query_idx != nullptr ? query_idx + r0 : nullptr;
     va.ref_feat = d.reff; va.dfeat = nullptr;
     va.G = d.G; va.nvalid = d.t.nvalid; va.mask_proj = mask_out + p0 * V; va.mask_eff = d.meff;
     va.X = d.X; va.vis2 = d.vis2; va.ray_diff = d.rd; va.rgb_in = d.rgbin;

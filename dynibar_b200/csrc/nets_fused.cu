@@ -38,7 +38,11 @@ int launch_view_fused(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st
     a.anti_alias = 0; a.mask_rgb = 0;
   }
   switch (g_view_kernel < 0 ? kDefaultViewKernel : g_view_kernel) {
-    case 0: return launch_view_twin(n, a, V, st);
+    case 0:
+      if (a.tgt_idx != nullptr)
+        return fail(DYN_E_INVALID, "the twin-warp per-view kernel (view_twin.cu) has no multi-camera form: "
+                                   "select the warpgroup kernel (dyn_debug_set_view_kernel(-1))");
+      return launch_view_twin(n, a, V, st);
     case 1: return fail(DYN_E_INVALID, "per-view kernel 1 (the quad-schedule kernel) has been removed");
     case 2:
     case 3:

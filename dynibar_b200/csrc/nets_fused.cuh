@@ -49,6 +49,7 @@ struct ViewFusedArgs {
   float* ray_diff;   // static [P*V,4]
   float* rgb_in;     // static [P*V,3] gathered source colours
   long long* dbg;    // optional: clock64() phase timestamps of block 0 (profiling builds/tests only)
+  const int* tgt_idx;  // static, multi-camera launches: [R] target camera of each ray (cams.tgts), else null
 };
 
 // ---- MotionMLP (motion_wg.cu) ----

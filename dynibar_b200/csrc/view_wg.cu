@@ -33,10 +33,11 @@ namespace {
 // 64 rows
 constexpr int kPeBytes = 14 * 1024, kPoolBytes = 30 * 1024, kWgATile = kPeBytes + kPoolBytes;
 // constants (floats): biases in true units; W6V = row 128 of vis_fc.2 (visibility logit), W8 = vis_fc2.2;
-// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; W1 / MK = per-row pooling weight and mask of each consumer
+// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; W1 / MK = per-row pooling weight and mask of each consumer;
+// TGT = the target camera centres of a multi-camera launch (3 floats each)
 constexpr int C_B1 = 0, C_B2 = 256, C_B3 = 304, C_B4 = 560, C_B5 = 688, C_B6 = 816, C_W6V = 944, C_B7 = 1072,
-              C_W8 = 1200, C_MISC = 1328, C_DFEAT = 1332, C_CAMS = 1372, C_W1 = 1628, C_MK = 1756;
-constexpr int kWgConst = 1884;
+              C_W8 = 1200, C_MISC = 1328, C_DFEAT = 1332, C_CAMS = 1372, C_W1 = 1628, C_MK = 1756, C_TGT = 1884;
+constexpr int kWgConst = C_TGT + 3 * kMaxTargets;
 // mbarriers: the weight ring's full / empty pairs, then per consumer its operand tiles' full and empty
 constexpr int kViewBars = 2 * kWgRing + 4;
 constexpr int kWgSmem = kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 4 /* align */ + kViewBars * 8;
@@ -133,7 +134,8 @@ __device__ __forceinline__ void store2_64(uint8_t* tile, int r, int col, float x
 // The front end of the 64 rows from row0 on, row layout (t = thread of the front-end warpgroup: twin tw = t / 64 of
 // row t % 64): projection, masks, gather, first pooling into columns 0..119 of pool_tile, [static] positional
 // encodings into pe_tile; each row's pooling weight and mask into s_w1 / s_mk; the per-(point, view) outputs.
-template <int VP, bool ST>
+// MC (static, multi-camera launch): the target camera centre of the row's ray is cst[C_TGT + 3 a.tgt_idx[ray]].
+template <int VP, bool ST, bool MC>
 __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* cst, int t, long long row0,
                                           uint8_t* pe_tile, uint8_t* pool_tile, float* s_w1, float* s_mk) {
   const int tw = t >> 6, r = t & 63, v = r & (VP - 1);
@@ -235,7 +237,9 @@ __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* c
 
   float rd[4];
   {
-    float a0 = a.cams.tgt[0] - p3[0], a1 = a.cams.tgt[1] - p3[1], a2 = a.cams.tgt[2] - p3[2];
+    const float* tgt = a.cams.tgt;
+    if (MC) tgt = cst + C_TGT + 3 * (pt_ok ? a.tgt_idx[(int)pl / a.S] : 0);
+    float a0 = tgt[0] - p3[0], a1 = tgt[1] - p3[1], a2 = tgt[2] - p3[2];
     normalize3(a0, a1, a2);
     float b0 = cam[12] - q3[0], b1 = cam[13] - q3[1], b2 = cam[14] - q3[2];
     normalize3(b0, b1, b2);
@@ -334,8 +338,9 @@ __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* c
   }
 }
 
-template <int VP, bool ST>
+template <int VP, bool ST, bool MC>
 __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_constant__ ViewFusedArgs a) {
+  static_assert(ST || !MC, "multi-camera launches are static-net only");
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem;
   uint8_t* atiles = smem + kWgRing * kWgStage;
@@ -382,6 +387,7 @@ __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_c
       cst[C_MISC + 1] = prm[a.o_b8];
       cst[C_MISC + 2] = (ST && a.o_s >= 0) ? fabsf(prm[a.o_s]) : 0.f;
     }
+    if (MC && tid < 3 * kMaxTargets) cst[C_TGT + tid] = a.cams.tgts[tid / 3][tid % 3];
   }
   __syncthreads();
 
@@ -403,7 +409,7 @@ __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_c
       for (int c = 0; c < 2; ++c) {
         if (k > 0) mbar_wait(tiles_empty + 8u * c, (k - 1) & 1);
         pc.mark(PH_HANDOFF, 0);
-        front_end<VP, ST>(a, cst, t, (long long)it * 128 + 64 * c, atiles + c * kWgATile,
+        front_end<VP, ST, MC>(a, cst, t, (long long)it * 128 + 64 * c, atiles + c * kWgATile,
                           atiles + c * kWgATile + kPeBytes, cst + C_W1 + 64 * c, cst + C_MK + 64 * c);
         fence_proxy_async_smem();
         mbar_arrive(tiles_full + 8u * c);
@@ -747,23 +753,29 @@ int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
     int dev = 0;
     DYN_CUDA(cudaGetDevice(&dev));
     DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-#define PREP_WG(VPV, STV) \
-    DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem))
-    PREP_WG(8, true); PREP_WG(16, true); PREP_WG(8, false); PREP_WG(16, false);
+#define PREP_WG(VPV, STV, MCV) \
+    DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV, MCV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem))
+    PREP_WG(8, true, false); PREP_WG(16, true, false); PREP_WG(8, false, false); PREP_WG(16, false, false);
+    PREP_WG(8, true, true); PREP_WG(16, true, true);
 #undef PREP_WG
   }
+  const bool st_net = n->kind == DYN_NET_STATIC;
+  const bool mc = a.tgt_idx != nullptr;
+  if (mc && !st_net) return fail(DYN_E_INVALID, "multi-camera per-view launches are for the static net only");
   const int VP = V <= 8 ? 8 : 16;
   const long long n_iter = (a.P * VP + 127) / 128;
   const int grid = (int)(n_iter < sms ? n_iter : sms);
   if (grid == 0) return DYN_OK;
-  const bool st_net = n->kind == DYN_NET_STATIC;
   ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
-  if (st_net) {
-    if (VP == 8) view_wg_kernel<8, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+  if (st_net && mc) {
+    if (VP == 8) view_wg_kernel<8, true, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, true, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+  } else if (st_net) {
+    if (VP == 8) view_wg_kernel<8, true, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, true, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
   } else {
-    if (VP == 8) view_wg_kernel<8, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    if (VP == 8) view_wg_kernel<8, false, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, false, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
   }
   DYN_LAUNCH_CHECK();
   return DYN_OK;

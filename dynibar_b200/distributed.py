@@ -15,7 +15,7 @@ Backend-agnostic (`nccl` on GPUs; the host logic is tested with `gloo`).
 import torch
 import torch.distributed as dist
 
-_RAY_KEYS_1 = ("ray_o", "ray_d", "uv_grid", "rgb", "disp", "motion_mask", "static_mask")
+_RAY_KEYS_1 = ("ray_o", "ray_d", "uv_grid", "rgb", "disp", "motion_mask", "static_mask", "camera_index")
 
 
 def shard_bounds(n_rays, rank, world):

@@ -69,8 +69,10 @@ class Projector(object):
     return project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmaps)
 
 
-def project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmaps):
-  """`xyz` may be None: every view then uses xyz_st (static branch)."""
+def project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmaps, camera_index=None):
+  """`xyz` may be None: every view then uses xyz_st (static branch).  With `camera_index` ([R] int32 on the
+  device) query_camera is [K,34] and ray r's view-direction term (ray_diff) uses camera camera_index[r]; the
+  kernel trusts the values to lie in [0, K)."""
   R, S = xyz_st.shape[:2]
   V = train_cameras.shape[1]
   _, _, H, W, _ = train_imgs.shape
@@ -84,9 +86,16 @@ def project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmap
   ws = _lib.workspace.get(fm.numel() * 4, dev, slot=1)
   A = Args()
   with torch.cuda.device(dev):
-    check(lib.dyn_project_gather(
-        A(xyz_st), A(xyz),
-        A.host(query_camera), A(train_imgs), A.host(train_cameras), ptr(fm),
-        V, R, S, H, W, Cc, h, w, ws.data_ptr(), ptr(rgb_feat), ptr(ray_diff), ptr(mask),
-        stream()))
+    if camera_index is None:
+      check(lib.dyn_project_gather(
+          A(xyz_st), A(xyz),
+          A.host(query_camera), A(train_imgs), A.host(train_cameras), ptr(fm),
+          V, R, S, H, W, Cc, h, w, ws.data_ptr(), ptr(rgb_feat), ptr(ray_diff), ptr(mask),
+          stream()))
+    else:
+      assert camera_index.shape == (R,)
+      check(lib.dyn_project_gather_mc(
+          A(xyz_st), A(xyz), A.host(query_camera), query_camera.shape[0], A(camera_index, torch.int32),
+          A(train_imgs), A.host(train_cameras), ptr(fm), V, R, S, H, W, Cc, h, w, ws.data_ptr(),
+          ptr(rgb_feat), ptr(ray_diff), ptr(mask), stream()))
   return rgb_feat, ray_diff, mask

@@ -354,9 +354,11 @@ def source_rgba(src_rgbs):
   return _frame_cache.get("rgba", src_rgbs, _pack_rgba)
 
 
-def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, feat_cl):
+def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, feat_cl, camera_index=None):
   """Projector.compute_with_motions + DynibarStatic.forward fused
-  (projection.py:103-176 + mlp_network.py:423-527) -> raw [R,S,4], mask [R,S,V,1]."""
+  (projection.py:103-176 + mlp_network.py:423-527) -> raw [R,S,4], mask [R,S,V,1].
+  With `camera_index` ([R] int32, device) query_cam is [K,34] and ray r is seen from camera camera_index[r]
+  (values trusted to lie in [0, K))."""
   dev = dev_of(pts)
   net = _weights.packed_of(module, dev)
   R, S = pts.shape[:2]
@@ -369,10 +371,18 @@ def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, f
   ws = _lib.workspace.get(nbytes, dev)
   A = Args()
   with torch.cuda.device(dev):
-    check(lib.dyn_net_static_fused(net.handle, A(pts), A(ray_o), A(ray_d), A.host(query_cam),
-                                   ptr(source_rgba(src_rgbs)), A.host(src_cams),
-                                   ptr(feat_cl, torch.bfloat16), R, S, V, H, W, Cc, h, w, ptr(raw),
-                                   ptr(mask), ws.data_ptr(), nbytes, stream()))
+    if camera_index is None:
+      check(lib.dyn_net_static_fused(net.handle, A(pts), A(ray_o), A(ray_d), A.host(query_cam),
+                                     ptr(source_rgba(src_rgbs)), A.host(src_cams),
+                                     ptr(feat_cl, torch.bfloat16), R, S, V, H, W, Cc, h, w, ptr(raw),
+                                     ptr(mask), ws.data_ptr(), nbytes, stream()))
+    else:
+      assert camera_index.shape == (R,)
+      check(lib.dyn_net_static_fused_mc(net.handle, A(pts), A(ray_o), A(ray_d), A.host(query_cam),
+                                        query_cam.shape[0], A(camera_index, torch.int32),
+                                        ptr(source_rgba(src_rgbs)), A.host(src_cams),
+                                        ptr(feat_cl, torch.bfloat16), R, S, V, H, W, Cc, h, w, ptr(raw),
+                                        ptr(mask), ws.data_ptr(), nbytes, stream()))
   return raw, mask
 
 
@@ -497,6 +507,28 @@ def compute_optical_flow(outputs_coarse, raw_pts_3d_seq, src_cameras, uv_grid):
 # ---------------------------------------------------------------------------
 
 _HOST_KEYS = ("camera", "src_cameras", "static_src_cameras", "anchor_src_cameras", "depth_range")
+MAX_CAMERAS = 16  # target cameras of one multi-camera ray batch (csrc/geometry.cuh: kMaxTargets)
+
+
+def camera_count(ray_batch):
+  """Number K of target cameras of a ray batch: `camera` [K,34].  A multi-camera batch (K > 1, see
+  sample_ray.stack_ray_batches) carries `camera_index` [R] int32 naming each ray's row of `camera`."""
+  cam = ray_batch["camera"]
+  K = cam.shape[0] if cam.dim() == 2 else 1
+  if K > 1:
+    if K > MAX_CAMERAS:
+      raise ValueError("multi-camera ray batch: %d target cameras, at most %d" % (K, MAX_CAMERAS))
+    ci = ray_batch.get("camera_index")
+    if ci is None or ci.dtype != torch.int32 or ci.shape != ray_batch["ray_o"].shape[:1]:
+      raise ValueError("multi-camera ray batch (%d target cameras) needs camera_index: int32 [R]" % K)
+  return K
+
+
+def _refuse_multi_camera(ray_batch, what):
+  if camera_count(ray_batch) > 1:
+    raise NotImplementedError(
+        "%s renders one target camera per time step; multi-camera ray batches (batched target cameras) are "
+        "for render_rays_mv / render_image.render_multi_image_nvi" % what)
 
 
 def _with_host_copies(ray_batch, model, basis_names):
@@ -520,6 +552,10 @@ def _render_pass(ray_batch, feat_dy, feat_st, pts, z, s, t, frame_idx, offsets, 
   """One coarse-or-fine evaluation at the reference time
   (render_ray.py:455-597 == :672-782 == :951-1096)."""
   cam, ray_o, ray_d = ray_batch["camera"], ray_batch["ray_o"], ray_batch["ray_d"]
+  # multi-camera batch: only the static branch's ray_diff reads the target camera (the dynamic net discards
+  # ray_diff, mlp_network.py:236-316), so the dynamic calls keep one camera
+  cam_idx = ray_batch.get("camera_index")
+  cam_dy = cam if cam_idx is None else cam[0:1]
   ref_plucker = compute_ref_plucker_coordinate(ray_o, ray_d)  # [d_hat, o x d_hat]
   ray_dir = ref_plucker[:, :3]  # == F.normalize(ray_d) (render_ray.py:455)
   coeff = motion_coefficients(motion, pts, t)
@@ -529,16 +565,16 @@ def _render_pass(ray_batch, feat_dy, feat_st, pts, z, s, t, frame_idx, offsets, 
   if fused:
     # gather + per-view MLP chain + pooling in one tensor-core kernel per branch: the
     # [R,S,V,35] gather output and the per-view activations never reach HBM
-    raw_dy, m_dy = net_dynamic_fused(net_dy, pts, seq, ray_dir, cam, ray_batch["src_rgbs"],
+    raw_dy, m_dy = net_dynamic_fused(net_dy, pts, seq, ray_dir, cam_dy, ray_batch["src_rgbs"],
                                      ray_batch["src_cameras"], featmaps_channels_last(feat_dy), t)
     raw_st, m_st = net_static_fused(net_st, pts, ray_o, ray_d, cam, ray_batch["static_src_rgbs"],
                                     ray_batch["static_src_cameras"],
-                                    featmaps_channels_last(feat_st))
+                                    featmaps_channels_last(feat_st), cam_idx)
   else:
-    f_dy, _, m_dy = project_gather(pts, seq, cam, ray_batch["src_rgbs"], ray_batch["src_cameras"],
+    f_dy, _, m_dy = project_gather(pts, seq, cam_dy, ray_batch["src_rgbs"], ray_batch["src_cameras"],
                                    feat_dy)
     f_st, rd_st, m_st = project_gather(pts, None, cam, ray_batch["static_src_rgbs"],
-                                       ray_batch["static_src_cameras"], feat_st)
+                                       ray_batch["static_src_cameras"], feat_st, cam_idx)
     raw_dy = net_dynamic_forward(net_dy, pts, f_dy, ray_dir, m_dy, t)
     raw_st = net_static_forward(net_st, pts, ref_plucker,
                                 compute_src_plucker_coordinate(pts, ray_batch["static_src_cameras"]),
@@ -568,8 +604,12 @@ def render_rays_mv(frame_idx, time_embedding, time_offset, ray_batch, model, pro
   (render_ray.py:600-867).  Extra keyword-only inputs `jitter` / `u` carry the
   random draws of :119 / :34 when det=False (drawn with torch.rand if None).
   Returns the reference's dict: outputs_coarse_ref, outputs_fine_ref,
-  outputs_fine_ref_dy, outputs_fine_anchor(None), outputs_fine_anchor_dy(None)."""
+  outputs_fine_ref_dy, outputs_fine_anchor(None), outputs_fine_anchor_dy(None).
+  `ray_batch` may be a multi-camera batch (sample_ray.stack_ray_batches): the rays of K target cameras
+  of one time step, ray r seen from camera[camera_index[r]]; the index values are not checked here
+  (render_image.render_multi_image_nvi checks them once per frame)."""
   assert N_importance > 0  # render_ray.py:787
+  camera_count(ray_batch)
   _refuse_training(model, coarse_featmaps, fine_featmaps)
   with torch.no_grad(), precision_scope(precision):
     t = _scalar(time_embedding[0].float())
@@ -603,6 +643,7 @@ def render_rays_mono(frame_idx, time_embedding, time_offset, ray_batch, model, f
   cross-time branch (:1099-1270) when is_train=True.  With gradients enabled and parameters / feature
   maps that require grad the differentiable fp32 training path runs (`_render_mono_train`); otherwise
   the forward-only kernels (fused tensor-core path in bf16 mode) under no_grad."""
+  _refuse_multi_camera(ray_batch, "render_rays_mono (and its training path)")
   if _wants_grad(model, featmaps):
     with precision_scope(precision):
       return _render_mono_train_chunked(frame_idx, time_embedding, time_offset, ray_batch, model, featmaps,

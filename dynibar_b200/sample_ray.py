@@ -140,3 +140,65 @@ class RaySamplerSingleImage(object):
     for k in self._passthrough:
       ret[k] = self._dev(getattr(self, k))
     return ret
+
+
+# what the target cameras of one time step share (eval_nvidia.py:305-378: DynamicVideoDataset builds the
+# source views from render_idx only)
+_FRAME_KEYS = ("src_cameras", "static_src_cameras", "depth_range", "src_rgbs", "static_src_rgbs")
+_RAY_KEYS = ("ray_o", "ray_d", "uv_grid", "rgb", "disp", "motion_mask", "static_mask")
+_CAMERA_KEYS = ("camera", "render_camera", "anchor_camera")
+
+
+def _same(a, b):
+  if a is b:
+    return True
+  if a is None or b is None:
+    return False
+  return a.shape == b.shape and a.device == b.device and torch.equal(a, b)
+
+
+def _stack(batches, k, dim):
+  vals = [b.get(k) for b in batches]
+  if all(v is None for v in vals):
+    return None
+  if any(v is None for v in vals):
+    raise ValueError("stack_ray_batches: '%s' is missing from some of the batches" % k)
+  return torch.cat(vals, dim)
+
+
+def stack_ray_batches(batches):
+  """K `get_all()` batches of the target cameras of ONE time step -> (multi-camera batch, per-camera ray
+  counts, (H, W) of the target images).
+
+  The multi-camera batch is an ordinary ray batch whose `camera` is [K,34] and whose per-ray tensors are the
+  K batches' concatenated in order; `camera_index` (int32 [R], on the rays' device) names each ray's row of
+  `camera`.  Per-frame tensors (source views, depth range) are shared: they must be the same in every batch
+  (same tensor or equal values), otherwise ValueError.  render_image.render_multi_image_nvi renders it and
+  splits the outputs back with the counts."""
+  K = len(batches)
+  if not 1 <= K <= 16:
+    raise ValueError("stack_ray_batches: %d batches, 1..16 target cameras per batch" % K)
+  first = batches[0]
+  for i, b in enumerate(batches[1:], 1):
+    for k in _FRAME_KEYS:
+      if not _same(first.get(k), b.get(k)):
+        raise ValueError("stack_ray_batches: batch %d does not share '%s' with batch 0 (the target cameras "
+                         "of one time step see the same source views and depth range)" % (i, k))
+  cams = [b["camera"] for b in batches]
+  if any(c.dim() != 2 or c.shape[0] != 1 for c in cams):
+    raise ValueError("stack_ray_batches: every batch has one target camera [1,34]")
+  hw = {(int(c[0, 0]), int(c[0, 1])) for c in cams}
+  if len(hw) != 1:
+    raise ValueError("stack_ray_batches: the target cameras have different image sizes %s" % sorted(hw))
+  out = dict(first)
+  for k in _CAMERA_KEYS + _RAY_KEYS:
+    if k in first:
+      out[k] = _stack(batches, k, 0)
+  for k in ("flows", "masks"):  # [n_views, R, c]
+    if k in first:
+      out[k] = _stack(batches, k, 1)
+  counts = [b["ray_o"].shape[0] for b in batches]
+  dev = first["ray_o"].device
+  out["camera_index"] = torch.repeat_interleave(torch.arange(K, dtype=torch.int32),
+                                                torch.tensor(counts)).to(dev)
+  return out, counts, hw.pop()

@@ -148,6 +148,18 @@ int dyn_project_gather(const float* xyz_st, const float* xyz,
                        int R, int S, int H, int W, int C, int h, int w,
                        float* feat_cl_ws, float* rgb_feat, float* ray_diff,
                        float* mask, void* stream);
+/* Multi-camera form of dyn_project_gather: the rays of K target cameras of one time step in one call.
+ * query_cams [K,34] (host or device, read like query_cam), 1 <= K <= 16; query_idx [R] (device, int32):
+ * ray r belongs to target camera query_idx[r], whose centre enters its ray_diff.  query_idx may be NULL
+ * only when K = 1 (it is ignored then: the call is dyn_project_gather).  The kernel trusts the index
+ * values: the caller keeps them in [0, K).  K and query_idx are checked before any CUDA call. */
+int dyn_project_gather_mc(const float* xyz_st, const float* xyz,
+                          const float* query_cams, int K, const int* query_idx,
+                          const float* src_rgbs, const float* src_cams,
+                          const float* featmaps, int V, int R, int S, int H,
+                          int W, int C, int h, int w, float* feat_cl_ws,
+                          float* rgb_feat, float* ray_diff, float* mask,
+                          void* stream);
 /* compute_projections only (projection.py:32-59): pix [V,N,2], front [V,N] u8 */
 int dyn_compute_projections(const float* xyz, const float* src_cams, int V,
                             int N, float* pix, uint8_t* front, void* stream);
@@ -204,6 +216,18 @@ int dyn_net_static_fused(dyn_net_t net, const float* pts, const float* ray_o,
                          int W, int C, int h, int w, float* raw,
                          float* mask_out, void* workspace,
                          size_t workspace_bytes, void* stream);
+/* Multi-camera form of dyn_net_static_fused: query_cams [K,34] and query_idx [R] as for
+ * dyn_project_gather_mc (1 <= K <= 16, query_idx non-NULL when K > 1, values trusted to lie in [0, K);
+ * K = 1 is dyn_net_static_fused).  Only the view-direction term of ray_diff reads the target camera.
+ * Runs on the warpgroup per-view kernel only: with the twin-warp kernel selected
+ * (dyn_debug_set_view_kernel(0)) a call with K > 1 fails with DYN_E_INVALID. */
+int dyn_net_static_fused_mc(dyn_net_t net, const float* pts, const float* ray_o,
+                            const float* ray_d, const float* query_cams, int K,
+                            const int* query_idx, const float* src_rgba,
+                            const float* src_cams, const void* feat_cl, int R,
+                            int S, int V, int H, int W, int C, int h, int w,
+                            float* raw, float* mask_out, void* workspace,
+                            size_t workspace_bytes, void* stream);
 int dyn_net_dynamic_fused(dyn_net_t net, const float* pts, const float* pts_seq,
                           const float* ray_dir, const float* query_cam,
                           const float* src_rgba, const float* src_cams,
