@@ -48,31 +48,6 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
-// accumulator memory of the fused tensor-core kernels that keep it in global memory (tc.cuh): a slot for each of
-// two resident CTAs per SM
-tc::AccPool acc_pool() {
-  static tc::AccPool pool[64] = {};
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ||
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
-    fail(DYN_E_CUDA, "acc_pool: no current CUDA device");
-    return tc::AccPool{};
-  }
-  if (pool[dev].mem == nullptr) {
-    const int slots = 2 * sms;
-    const size_t bytes = (size_t)slots * tc::kAccCtaFloats * sizeof(float);
-    void* p = nullptr;
-    cudaError_t e = cudaMalloc(&p, bytes + slots * sizeof(int));
-    if (e == cudaSuccess) e = cudaMemset((char*)p + bytes, 0, slots * sizeof(int));
-    if (e != cudaSuccess) {
-      if (p) cudaFree(p);
-      fail(DYN_E_CUDA, "acc_pool: %s", cudaGetErrorString(e));
-      return tc::AccPool{};
-    }
-    pool[dev] = tc::AccPool{(float*)p, (int*)((char*)p + bytes), slots};
-  }
-  return pool[dev];
-}
 
 }  // namespace dyn
 
@@ -311,7 +286,7 @@ int dyn_net_dynamic_fused(dyn_net_t net, const float* pts, const float* pts_seq,
 int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid, const float* pts,
                           const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
                           float* O, float* out_a, float* out_b, float* posenc_ws, void* stream) {
-  DYN_CHECK_ARG(net && net->kind != DYN_NET_MOTION && G && nvalid && g2 && out_a && posenc_ws);
+  DYN_CHECK_ARG(net && net->kind != DYN_NET_MOTION && G && nvalid && out_a && posenc_ws);
   DYN_CHECK_ARG(R >= 0 && S >= 1);
   return debug_point_chain(net, G, nvalid, pts, ray_dir, R, S, g2, Q, K, V, O, out_a, out_b, posenc_ws,
                            (cudaStream_t)stream);

@@ -121,9 +121,10 @@ struct dyn_net {
   dyn::MotionLayout ml;
   // MotionMLP in one fused kernel (motion_wg.cu): full-width weight chunks in consumption order; motion net only
   dyn::ChainImage motion;
-  // row-local chains of the aggregation nets (chains_wg.cu): [0] point stage 1, [1] point stage 2,
-  // [2] static blending head
-  dyn::ChainImage chain[3];
+  // row-local chains of the aggregation nets (chains_wg.cu): [0] the per-point stage, the point1 layers (its
+  // first point1_chunks chunks) then the point2 layers; [1] static blending head
+  dyn::ChainImage chain[2];
+  int point1_chunks;
   // twin-warp per-view stage (view_twin.cu): weight images in its column layout
   dyn::ChainImage twin;
   // warpgroup per-view stage (view_wg.cu): full-width weight chunks in consumption order

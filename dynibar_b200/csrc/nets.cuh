@@ -41,10 +41,6 @@ int debug_rgb_head(const dyn_net* n, const float* X, const float* vis2, const fl
                    cudaStream_t st);
 void set_view_capture(float* G, float* nvalid, float* X, float* vis2, float* mask_eff, float* ray_diff,
                       float* rgb_in);
-// tensor-core ray-transformer attention (attention_tc.cu); S must divide 128
-bool attention_tc_supported(int S);
-int launch_attention_tc(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __nv_bfloat16* V,
-                        const float* nvalid, long long P, int S, __nv_bfloat16* O, cudaStream_t st);
 int zero_last_samples(float* coeff, int R, int S, int width, cudaStream_t st);
 // training slice of the MotionMLP (motion_train.cu); embedding hooks live in nets_f32.cu
 int motion_embed(const float* xyzt, long long N, float* x0, cudaStream_t st);

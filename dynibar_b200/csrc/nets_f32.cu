@@ -449,7 +449,7 @@ static int check_simt_attention(int S) {
 // divides 128, everything else (and every S of the staged path) runs on a SIMT kernel.  Every entry point that
 // reaches an attention launch (the nets, the test hooks) checks this once, before it launches anything.
 static int check_attention_samples(int S, bool fused) {
-  if (fused) return attention_tc_supported(S) ? DYN_OK : check_simt_attention<true>(S);
+  if (fused) return point_fused_supported(S) ? DYN_OK : check_simt_attention<true>(S);
   return check_simt_attention<false>(S);
 }
 
@@ -875,11 +875,12 @@ size_t net_fused_workspace(int kind, int R, int S, int V) {
   return fused_alloc(b, kind == DYN_NET_STATIC, R < rc ? R : rc, S, V, &d);
 }
 
-// ray-transformer attention of the fused path on bf16 tile images (16 k-groups): the tensor-core kernels when S
-// divides 128, else the SIMT kernel (one block per ray)
+// ray-transformer attention of the fused path on bf16 tile images (16 k-groups): the fused stage's tensor-core
+// attention when S divides 128 (the test hook; the product path runs it inside point_fused_wg_kernel), else the
+// SIMT kernel (one block per ray)
 static int run_attention_fused(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __nv_bfloat16* V,
                                const float* nvalid, long long P, int R, int S, __nv_bfloat16* O, cudaStream_t st) {
-  if (attention_tc_supported(S)) return launch_attention_tc(Q, K, V, nvalid, P, S, O, st);
+  if (point_fused_supported(S)) return launch_attention_wg(Q, K, V, nvalid, P, S, O, st);
   const int threads = ((S + 31) / 32) * 32;  // S <= the kernel's block limit (check_attention_samples at entry)
   const size_t smem = (size_t)2 * S * 32 * sizeof(float);
   if (smem > 48 * 1024)
@@ -890,11 +891,12 @@ static int run_attention_fused(const __nv_bfloat16* Q, const __nv_bfloat16* K, c
   return DYN_OK;
 }
 
-// per-point stage on the fused chains: point1 (geometry_fc, Q|K|V) -> ray-transformer
-// attention -> point2 (fc + LayerNorm + heads);
+// per-point stage on the fused chains: point1 (geometry_fc, Q|K|V) -> ray-transformer attention -> point2 (fc +
+// LayerNorm + heads).  When S divides 128 that is one kernel (capture: it also stores g2, Q, K, V and O);
+// otherwise point1, the SIMT attention and point2 exchange them through the workspace.
 // G, Q, K, V, O are bf16 tile images, g2 / GW use the fp32 tile layout (fused_engine.cuh)
 static int run_point_fused(const dyn_net* n, const float* G, long long P, int R, int S, bool dynamic,
-                           float* posenc_tab, TrunkBufs& t, Point2Args& p2, cudaStream_t st) {
+                           float* posenc_tab, TrunkBufs& t, Point2Args& p2, cudaStream_t st, bool capture = false) {
   Point1Args p1;
   memset(&p1, 0, sizeof(p1));
   // Q, K, V, O travel between the point kernels as bf16 rows (they are tensor-core operands)
@@ -909,9 +911,10 @@ static int run_point_fused(const dyn_net* n, const float* G, long long P, int R,
     DYN_LAUNCH_CHECK();
     p1.posenc = posenc_tab;
   }
+  p2.O = Ob; p2.g2 = t.G2; p2.nvalid = t.nvalid; p2.P = P; p2.S = S;
+  if (point_fused_supported(S)) return launch_point_fused_wg(n, p1, p2, capture ? Ob : nullptr, st);
   RUN(launch_point1_wg(n, p1, st));
   RUN(run_attention_fused(Qb, Kb, Vb, t.nvalid, P, R, S, Ob, st));
-  p2.O = Ob; p2.g2 = t.G2; p2.nvalid = t.nvalid; p2.P = P; p2.S = S;
   return launch_point2_wg(n, p2, st);
 }
 
@@ -979,8 +982,9 @@ static int image_rows_out(const void* img, long long P, float* dst, cudaStream_t
   return DYN_OK;
 }
 
-// The per-point fused stage on caller-provided G / nvalid; Q, K, V, O (any may be NULL) receive the bf16 values
-// the kernels exchanged.
+// The per-point fused stage on caller-provided G / nvalid; g2 and Q, K, V, O (any may be NULL) receive the values
+// the kernels exchanged.  With all five NULL and S dividing 128 it runs the product kernel, which stores none of
+// them.
 int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, const float* pts,
                       const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
                       float* O, float* out_a, float* out_b, float* posenc_ws, cudaStream_t st) {
@@ -1004,9 +1008,12 @@ int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, con
   const bool dynamic = n->kind == DYN_NET_DYNAMIC;
   if (dynamic) { p2.pts = pts; p2.ray_dir = ray_dir; p2.raw = out_a; }
   else { p2.GW = buf[5]; p2.sigma = out_b; }
-  int rc = run_point_fused(n, reinterpret_cast<const float*>(gimg), P, R, S, dynamic, posenc_ws, t, p2, st);
+  // the capturing instantiation when the caller wants any of the exchanged values, else the product kernel
+  const bool capture = g2 || Q || K || V || O;
+  int rc = run_point_fused(n, reinterpret_cast<const float*>(gimg), P, R, S, dynamic, posenc_ws, t, p2, st, capture);
   if (rc == DYN_OK) {
-    tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[0]), P, g2);
+    if (g2)
+      tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[0]), P, g2);
     if (!dynamic)
       tile_f32_to_rows_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(reinterpret_cast<const uint8_t*>(buf[5]), P, out_a);
     const float* img[4] = {t.Q, t.K, t.V, t.O};

@@ -100,6 +100,14 @@ struct Point2Args {
   int nchunks;
 };
 
+// the whole per-point stage in one kernel (S dividing 128): point1's inputs and point2's outputs; p1.g2, p1.Q,
+// p1.K, p1.V and O are written only by the capture instantiation the test hooks run
+struct PointFusedArgs {
+  Point1Args p1;
+  Point2Args p2;
+  __nv_bfloat16* O;
+};
+
 struct RgbHeadArgs {
   const float *X /* bf16 tile image, 16 k-groups, rows = view slots (point * VP + view) */, *vis2, *ray_diff, *mask_eff, *rgb_in, *GW, *sigma;
   long long P;
@@ -126,6 +134,14 @@ size_t chain_wg_bytes(int kind);
 int chain_wg_build(dyn_net* n, const float* host_params, void* dst_dev, size_t dst_bytes, cudaStream_t st);
 int launch_point1_wg(const dyn_net* n, Point1Args& a, cudaStream_t st);
 int launch_point2_wg(const dyn_net* n, Point2Args& a, cudaStream_t st);
+// point1 -> attention -> point2 as one kernel, for S dividing 128 (point_fused_supported); with O_capture, g2, Q,
+// K, V (p1's pointers) and O are stored as well
+bool point_fused_supported(int S);
+int launch_point_fused_wg(const dyn_net* n, const Point1Args& p1, const Point2Args& p2, __nv_bfloat16* O_capture,
+                          cudaStream_t st);
+// the fused stage's attention alone on bf16 tile images (16 k-groups), S dividing 128
+int launch_attention_wg(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __nv_bfloat16* V, const float* nvalid,
+                        long long P, int S, __nv_bfloat16* O, cudaStream_t st);
 int launch_rgbhead_wg(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st);
 
 // twin-warp per-view stage (view_twin.cu)

@@ -9,12 +9,11 @@
 //   with SBO = 128 (row groups packed back to back) and LBO = rows*16.
 // One wgmma consumes K = 16 (two core matrices along K) for 64 rows of A.
 //
-// Accumulator memory: a 128-lane x (up to) 512-column fp32 array per CTA, laid out [column / 4][lane][4].
-// The MMA warpgroup stores each finished 128 x N block there from its wgmma registers; the row threads read
-// their row (lane = row of the 128-row tile) in blocks of 8 - 32 columns and may use columns as scratch.
-// One-tile kernels keep it in shared memory (256 columns, 128 KB), the others in their slice of a
-// device buffer (acc_pool, indexed by blockIdx.x), which stays L2-resident.  The writer stores before
-// arriving on an mbarrier and the reader loads after waiting on it (release / acquire at CTA scope).
+// Accumulator memory: a 128-lane x 256-column fp32 array per CTA in shared memory (128 KB), laid out
+// [column / 4][lane][4], used by the twin-warp per-view kernel (view_twin.cu).  The MMA warpgroup stores each
+// finished 128 x N block there from its wgmma registers; the row threads read their row (lane = row of the
+// 128-row tile) in blocks of 8 - 32 columns and may use columns as scratch.  The writer stores before arriving on
+// an mbarrier and the reader loads after waiting on it (release / acquire at CTA scope).
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -212,21 +211,21 @@ struct Wgmma<256, TA, TB> {
   }
 };
 
-// D[64 x N] (+)= A[64 x 16] * B[16 x N] with A in registers (the bf16x2 fragment of WgmmaRsFrag below) and
-// B K-major in shared memory.
-template <int N>
+// D[64 x N] (+)= A[64 x 16] * B[16 x N] with A in registers (the bf16x2 fragment of acc_to_afrag below) and
+// B in shared memory, K-major (TB = 0) or MN-major (TB = 1: N = 32 only, the attention's P V).
+template <int N, int TB = 0>
 struct WgmmaRS;
-template <>
-struct WgmmaRS<32> {
+template <int TB>
+struct WgmmaRS<32, TB> {
   static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
         "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
-        "}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        "}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
           "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
   }
 };
 
@@ -348,19 +347,9 @@ __device__ __forceinline__ bool elect_one() {
 // ---- accumulator memory, addressed TMEM-style ----------------------------------------
 // tmem_alloc binds the CTA's accumulator memory and writes its base address (lane << 16 | column) to a
 // shared-memory slot; loads and stores complete in program order, so tmem_wait_* and tc_fence_* only keep
-// the compiler from moving accumulator accesses across them.  A slot of the device pool belongs to one CTA
-// from its tmem_alloc to its tmem_dealloc, so launches on several streams of a device can share the pool.
-constexpr int kAccCols = 512;
-constexpr size_t kAccCtaFloats = (size_t)kAccCols * 128;
+// the compiler from moving accumulator accesses across them.
 constexpr int kAccSmemBytes = 256 * 128 * 4;  // a one-tile kernel's accumulator memory in shared memory
-struct AccPool {
-  float* mem;  // slots x kAccCtaFloats
-  int* busy;   // slots flags: 1 = claimed
-  int slots;
-};
-static __device__ AccPool g_acc_pool;  // this translation unit's copy of acc_pool(): set by bind_acc_pool()
-static __shared__ float* s_acc;        // this CTA's accumulator memory (shared or global)
-static __shared__ int s_acc_slot;      // its pool slot, -1 in shared memory
+static __shared__ float* s_acc;               // this CTA's accumulator memory
 
 __device__ __forceinline__ void compiler_fence() { asm volatile("" ::: "memory"); }
 __device__ __forceinline__ void tc_fence_before_sync() { compiler_fence(); }
@@ -368,36 +357,14 @@ __device__ __forceinline__ void tc_fence_after_sync() { compiler_fence(); }
 __device__ __forceinline__ void tmem_wait_ld() { compiler_fence(); }
 __device__ __forceinline__ void tmem_wait_st() { compiler_fence(); }
 
-// called by one warp before the CTA's first __syncthreads: base address 0, memory = a free slot of the
-// device pool (ncols <= kAccCols; waits while every slot is held by a running CTA) ...
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  (void)ncols;
-  if ((threadIdx.x & 31) == 0) {
-    int s = (int)(blockIdx.x % g_acc_pool.slots);
-    while (atomicCAS(g_acc_pool.busy + s, 0, 1) != 0) s = (s + 1) % g_acc_pool.slots;
-    __threadfence();
-    s_acc_slot = s;
-    s_acc = g_acc_pool.mem + (size_t)s * kAccCtaFloats;
-    asm volatile("st.shared.u32 [%0], %1;" ::"r"(dst_smem), "r"(0u) : "memory");
-  }
-}
-// ... or kAccSmemBytes of shared memory at `region` (one 128-row tile, 256 columns)
+// called by one warp before the CTA's first __syncthreads: base address 0, memory = kAccSmemBytes of shared
+// memory at `region` (one 128-row tile, 256 columns)
 __device__ __forceinline__ void tmem_alloc_smem(uint32_t dst_smem, void* region) {
   if ((threadIdx.x & 31) == 0) {
-    s_acc_slot = -1;
     s_acc = reinterpret_cast<float*>(region);
     asm volatile("st.shared.u32 [%0], %1;" ::"r"(dst_smem), "r"(0u) : "memory");
   }
 }
-// called by one warp after the CTA's last __syncthreads
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  (void)taddr; (void)ncols;
-  if ((threadIdx.x & 31) == 0 && s_acc_slot >= 0) {
-    __threadfence();
-    atomicExch(g_acc_pool.busy + s_acc_slot, 0);
-  }
-}
-
 __device__ __forceinline__ float* acc_cta() { return s_acc; }
 __device__ __forceinline__ uint32_t tmem_addr(uint32_t base, uint32_t lane, uint32_t col) {
   return base + (lane << 16) + col;
@@ -491,24 +458,5 @@ __host__ __device__ constexpr uint32_t tile_off(uint32_t rows, uint32_t r, uint3
 }
 
 }  // namespace tc
-
-// Host: the accumulator-memory pool of the current device (allocated and zeroed on first use, kept for the life
-// of the process; a first launch inside a stream capture fails: that set-up is not capturable).
-tc::AccPool acc_pool();
-
-// Points this translation unit's g_acc_pool at the current device's pool.
-static inline int bind_acc_pool() {
-  static float* bound[64] = {};  // what this translation unit's symbol holds, per device
-  int dev = 0;
-  DYN_CUDA(cudaGetDevice(&dev));
-  const tc::AccPool p = acc_pool();
-  if (p.mem == nullptr) return DYN_E_CUDA;
-  if (dev < 0 || dev >= 64) return fail(DYN_E_INVALID, "device index %d out of range", dev);
-  if (bound[dev] != p.mem) {
-    DYN_CUDA(cudaMemcpyToSymbol(tc::g_acc_pool, &p, sizeof(p)));
-    bound[dev] = p.mem;
-  }
-  return DYN_OK;
-}
 
 }  // namespace dyn

@@ -637,11 +637,6 @@ __global__ void __launch_bounds__(kTwinThreads, 1) view_twin_kernel(const __grid
     }
 #undef TS
   }
-  __syncthreads();
-  if (warp == W_ISSUE) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 256);
-  }
 }
 
 }  // namespace

@@ -37,32 +37,34 @@ __device__ __forceinline__ void store8_64(uint8_t* arow, int c0, const float* v)
       make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
 }
 
-// The weight ring as one consumer warpgroup sees it: chunk `cnt` sits in slot cnt % kWgRing.
-struct Ring {
+// The weight ring as one consumer warpgroup sees it: chunk `cnt` sits in slot cnt % RING.
+template <int RING>
+struct RingN {
   uint8_t* base;
-  uint32_t bar0;  // [0, kWgRing) full, [kWgRing, 2 kWgRing) empty
+  uint32_t bar0;  // [0, RING) full, [RING, 2 RING) empty
   uint32_t cnt;
   bool prof;
   long long wait_cycles;  // profiling: cycles spent waiting for weights
   __device__ __forceinline__ uint32_t wait_full(uint32_t c) {
-    const uint32_t st = c % kWgRing;
+    const uint32_t st = c % RING;
     const long long t0 = prof ? clock64() : 0;
-    mbar_wait(bar0 + 8u * st, (c / kWgRing) & 1);
+    mbar_wait(bar0 + 8u * st, (c / RING) & 1);
     if (prof) wait_cycles += clock64() - t0;
     return smem_u32(base + st * kWgStage);
   }
   // this warp's wgmmas that read chunk c have retired (the empty barrier counts 4 warps x 2 warpgroups)
   __device__ __forceinline__ void release(uint32_t c) {
     __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (kWgRing + c % kWgRing));
+    if ((threadIdx.x & 31) == 0) mbar_arrive(bar0 + 8u * (RING + c % RING));
   }
 };
+using Ring = RingN<kWgRing>;
 
 // Issues one layer, D[64 x N] = A[64 x 16 KS] W^T, chunk by chunk as the weights arrive; each chunk's slot is
 // released as soon as the next chunk's wgmmas are committed and its own have retired.  The last chunk stays in
 // flight: layer_finish waits for it.  mma(acc, kstep, b_desc, scale_d) issues one k-step.
-template <int N, int KS, class Mma>
-__device__ __forceinline__ void layer_issue(float* acc, Ring& rg, Mma mma) {
+template <int N, int KS, class RG, class Mma>
+__device__ __forceinline__ void layer_issue(float* acc, RG& rg, Mma mma) {
   constexpr int KC = wg_chunk_ksteps(N), NCH = (KS + KC - 1) / KC;
   fence_regs<N / 2>(acc);
   wgmma_fence();
@@ -80,28 +82,28 @@ __device__ __forceinline__ void layer_issue(float* acc, Ring& rg, Mma mma) {
   }
   rg.cnt += NCH;
 }
-template <int N>
-__device__ __forceinline__ void layer_finish(float* acc, Ring& rg) {
+template <int N, class RG>
+__device__ __forceinline__ void layer_finish(float* acc, RG& rg) {
   wgmma_wait<0>();
   fence_regs<N / 2>(acc);
   rg.release(rg.cnt - 1);
 }
 
 // A from a K-major operand tile of ROWS rows (this warpgroup's 64 rows start at a_tile)
-template <int N, int KS, int ROWS = 64>
-__device__ __forceinline__ void layer_ss(float* acc, uint32_t a_tile, Ring& rg) {
+template <int N, int KS, int ROWS = 64, class RG>
+__device__ __forceinline__ void layer_ss(float* acc, uint32_t a_tile, RG& rg) {
   layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
     Wgmma<N, 0, 0>::mma(d, smem_desc(a_tile + ks * (ROWS * 32u), ROWS * 16u, 128u), bd, sc);
   });
 }
-template <int N, int KS>
-__device__ __forceinline__ void layer_rs(float* acc, const uint32_t (&af)[KS][4], Ring& rg) {
+template <int N, int KS, class RG>
+__device__ __forceinline__ void layer_rs(float* acc, const uint32_t (&af)[KS][4], RG& rg) {
   layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) { WgmmaRS<N>::mma(d, af[ks], bd, sc); });
   layer_finish<N>(acc, rg);
 }
 // One layer whose first KR k-steps take A from register fragments and the rest from a 64-row operand tile.
-template <int N, int KS, int KR>
-__device__ __forceinline__ void layer_rs_ss(float* acc, const uint32_t (*af)[4], uint32_t tile64, Ring& rg) {
+template <int N, int KS, int KR, class RG>
+__device__ __forceinline__ void layer_rs_ss(float* acc, const uint32_t (*af)[4], uint32_t tile64, RG& rg) {
   layer_issue<N, KS>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
     if (ks < KR) WgmmaRS<N>::mma(d, af[ks < KR ? ks : 0], bd, sc);
     else Wgmma<N, 0, 0>::mma(d, smem_desc(tile64 + (ks - KR) * 2048u, 1024u, 128u), bd, sc);

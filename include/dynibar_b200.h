@@ -383,7 +383,8 @@ int dyn_encoder_forward(const float* params, size_t n_params, const float* image
  * -> heads; mlp_network.py:283-315 / :496-506) on caller-provided pooled
  * features G [R*S, 272] (257 used) and nvalid [R*S].  Outputs g2 [R*S,128] (plain
  * fp32 rows); Q, K, V, O [R*S,128]: the bf16 values the kernels exchanged, as fp32 rows
- * (each may be NULL: not written); dynamic net: out_a = raw [R*S,4]; static net:
+ * (each may be NULL: not written; when S divides 128 and all five are NULL, the product
+ * kernel runs instead of its capturing twin); dynamic net: out_a = raw [R*S,4]; static net:
  * out_a = per-point part of rgb_fc.0 [R*S,128], out_b = masked sigma [R*S].
  * posenc_ws: S*128 floats of scratch. */
 int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid,
