@@ -95,6 +95,10 @@ SIGNATURES = {
     "dyn_traj_combine": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "dyn_traj_combine_backward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "dyn_flow_backward": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "dyn_traj_combine_grad_d_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dyn_traj_combine_grad_d": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "dyn_expected_scene_flow": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
+    "dyn_expected_scene_flow_backward": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "dyn_debug_tc_grad_w": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "dyn_debug_tc_grad_in": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _vp, _sz, _vp]),
     "dyn_debug_tc_grad_in_scratch_bytes": (_sz, []),

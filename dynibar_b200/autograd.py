@@ -15,8 +15,10 @@ of the path, so that `render_ray.render_rays_mono(..., is_train=True)` is differ
                         :423-527) incl. the ray transformer: gradients w.r.t. every parameter, the gathered
                         rgb_feat and (dynamic) the sample points (csrc/nets_train.cu, fp32).
   * `composite_vanilla` raw2outputs_vanilla (render_ray.py:134-211).
-  * `traj_combine`      compute_traj_pts and the displacements built from it (render_ray.py:361-369, :462-500).
+  * `traj_combine`      compute_traj_pts and the displacements built from it (render_ray.py:361-369, :462-500),
+                        including the gradient w.r.t. the trajectory-basis rows.
   * `optical_flow`      compute_optical_flow (render_ray.py:333-358).
+  * `expected_scene_flow`  exp_sf of the mv fine pass (render_ray.py:585-595).
 
 tests/test_backward_gpu.py and tests/test_train_gpu.py check them -- and the whole training forward/backward --
 against torch autograd through the oracle's restatement of the same functions.
@@ -323,26 +325,71 @@ class _TrajCombine(torch.autograd.Function):
       check(lib.dyn_traj_combine(ptr(c), ptr(Dd), ptr(b) if b is not None else None, n, nb, R * S, ptr(out),
                                  stream()))
     ctx.D, ctx.dims = Dd, (n, nb, R, S)
+    ctx.coeff = c if ctx.needs_input_grad[1] else None
     return out
 
   @staticmethod
   def backward(ctx, g):
     n, nb, R, S = ctx.dims
     go = f32c(g)
-    need_c, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[2]
-    if not (need_c or need_b):
-      return None, None, None
+    need_c, need_d, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
     g_c = torch.empty(R, S, 3 * nb, device=go.device) if need_c else None
+    g_d = torch.empty(n, nb, device=go.device) if need_d else None
     g_b = torch.empty(R, S, 3, device=go.device) if need_b else None
     with torch.cuda.device(go.device):
-      check(lib.dyn_traj_combine_backward(ptr(go), ptr(ctx.D), n, nb, R * S, ptr(g_c) if need_c else None,
-                                          ptr(g_b) if need_b else None, stream()))
-    return g_c, None, g_b
+      if need_c or need_b:
+        check(lib.dyn_traj_combine_backward(ptr(go), ptr(ctx.D), n, nb, R * S, ptr(g_c) if need_c else None,
+                                            ptr(g_b) if need_b else None, stream()))
+      if need_d:
+        from dynibar_b200 import _lib
+        nbytes = int(lib.dyn_traj_combine_grad_d_workspace_bytes(n, nb, R * S))
+        ws = _lib.workspace.get(nbytes, go.device, slot=4)
+        check(lib.dyn_traj_combine_grad_d(ptr(go), ptr(ctx.coeff), n, nb, R * S, ptr(g_d), ws.data_ptr(), nbytes,
+                                          stream()))
+    ctx.coeff = None
+    return g_c, g_d, g_b
 
 
 def traj_combine(coeff, D, base=None):
-  """out[i] = (base or 0) + sum_k coeff[..., axis * nb + k] * D[i, k] -> [n,R,S,3]; D [n,nb] on the device."""
+  """out[i] = (base or 0) + sum_k coeff[..., axis * nb + k] * D[i, k] -> [n,R,S,3]; D [n,nb] on the device.  When D
+  requires grad (rows built from a trainable trajectory basis) its gradient is the deterministic reduction of
+  dyn_traj_combine_grad_d."""
   return _TrajCombine.apply(coeff, D, base)
+
+
+class _ExpectedSceneFlow(torch.autograd.Function):
+  @staticmethod
+  def forward(ctx, weights, sf):
+    dev = dev_of(weights)
+    R, S = weights.shape
+    w, s = f32c(weights), f32c(sf)
+    assert s.shape == (2, R, S, 3), s.shape
+    out = torch.empty(R, 3, device=dev)
+    with torch.cuda.device(dev):
+      check(lib.dyn_expected_scene_flow(ptr(w), ptr(s), R, S, ptr(out), stream()))
+    ctx.save_for_backward(w, s)
+    return out
+
+  @staticmethod
+  def backward(ctx, g):
+    w, s = ctx.saved_tensors
+    R, S = w.shape
+    g_w = torch.empty_like(w) if ctx.needs_input_grad[0] else None
+    g_s = torch.empty_like(s) if ctx.needs_input_grad[1] else None
+    if g_w is None and g_s is None:
+      return None, None
+    with torch.cuda.device(w.device):
+      check(lib.dyn_expected_scene_flow_backward(ptr(w), ptr(s), ptr(f32c(g)), R, S,
+                                                 ptr(g_w) if g_w is not None else None,
+                                                 ptr(g_s) if g_s is not None else None, stream()))
+    return g_w, g_s
+
+
+def expected_scene_flow(weights, sf):
+  """Differentiable exp_sf of the mv fine pass (render_ray.py:585-595): weights [R,S], sf [2,R,S,3] =
+  (traj(f+2) - traj(f), traj(f-2) - traj(f)) -> [R,3] = max(sum_s w sf[0], sum_s w sf[1]); ties split the gradient
+  in half like torch.max."""
+  return _ExpectedSceneFlow.apply(weights, sf)
 
 
 class _OpticalFlow(torch.autograd.Function):

@@ -6,6 +6,9 @@
 //                                 gathered rgb_feat w.r.t. the source feature maps (F.grid_sample backward,
 //                                 bilinear, zero padding, align_corners=True) and w.r.t. the (motion-displaced)
 //                                 sample points through the projection
+//   dyn_traj_combine_grad_d      gradient of the trajectory displacements w.r.t. the trajectory-basis rows
+//                                 (deterministic two-stage reduction over all points)
+//   dyn_expected_scene_flow      exp_sf of the mv fine pass (render_ray.py:585-595), forward and backward
 //
 // fp32 throughout; one warp per ray for the compositing scan (reverse multiplicative scan for the
 // transmittance), atomicAdd scatter for the feature-map gradient.  The MLP / ray-transformer backward is not
@@ -233,6 +236,129 @@ __global__ void traj_combine_bwd_kernel(const float* __restrict__ g_out, const f
     for (int k = 0; k < nb; ++k) g_coeff[p * 3 * nb + a * nb + k] = gc[k];
 }
 
+// Gradient of traj_combine w.r.t. the basis-difference rows: gD[i, k] = sum_p sum_a g_out[i, p, a] coeff[p, a nb + k],
+// a reduction over all P points.  Stage 1: block b owns points [b kGdPts, (b + 1) kGdPts) and writes its partial sums
+// partial[b, i, k]; stage 2 adds the partials of every block in block order.  Each thread, lane and warp always covers
+// the same points in the same order, so the result does not depend on scheduling (no float atomics): two calls on the
+// same inputs give the same bits.
+constexpr int kGdThreads = 256;
+constexpr int kGdPts = 1024;  // points per block (4 per thread)
+
+__global__ void __launch_bounds__(kGdThreads) traj_grad_d_partial_kernel(const float* __restrict__ g_out,
+                                                                       const float* __restrict__ coeff, int n, int nb,
+                                                                       long long P, float* __restrict__ partial) {
+  __shared__ float red[kGdThreads / 32][8];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long p0 = (long long)blockIdx.x * kGdPts;
+  const long long p1 = min(P, p0 + kGdPts);
+  for (int i = 0; i < n; ++i) {
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (long long p = p0 + tid; p < p1; p += kGdThreads) {
+      const float* g = g_out + ((long long)i * P + p) * 3;
+      const float* c = coeff + p * 3 * nb;
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        const float ga = g[a];
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          if (k < nb) acc[k] = fmaf(ga, c[a * nb + k], acc[k]);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = warp_sum_b(acc[k]);
+    if (lane == 0)
+#pragma unroll
+      for (int k = 0; k < 8; ++k) red[warp][k] = acc[k];
+    __syncthreads();
+    if (tid < nb) {
+      float s = 0.f;
+#pragma unroll
+      for (int w = 0; w < kGdThreads / 32; ++w) s += red[w][tid];
+      partial[((long long)blockIdx.x * n + i) * nb + tid] = s;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void traj_grad_d_sum_kernel(const float* __restrict__ partial, int blocks, int n, int nb,
+                                       float* __restrict__ g_D) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n * nb) return;
+  float s = 0.f;
+  for (int b = 0; b < blocks; ++b) s += partial[(long long)b * n * nb + j];
+  g_D[j] = s;
+}
+
+// Expected scene flow (render_ray.py:585-595): exp_sf[r, a] = max(sum_s w[r, s] sf[0, r, s, a],
+// sum_s w[r, s] sf[1, r, s, a]) with sf = (traj(f + k) - traj(f), traj(f - k) - traj(f)).  One warp per ray; forward
+// and backward form the two sums with the same code, so the backward sees the forward's ties.
+__device__ __forceinline__ void exp_sf_sums(const float* __restrict__ w, const float* __restrict__ sf, int r, int R,
+                                            int S, int lane, float ep[3], float em[3]) {
+  const long long N = (long long)R * S;
+  for (int a = 0; a < 3; ++a) ep[a] = em[a] = 0.f;
+  for (int s = lane; s < S; s += 32) {
+    const long long ps = (long long)r * S + s;
+    const float wv = w[ps];
+    const float* p = sf + ps * 3;
+    const float* m = sf + (N + ps) * 3;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      ep[a] = fmaf(wv, p[a], ep[a]);
+      em[a] = fmaf(wv, m[a], em[a]);
+    }
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    ep[a] = warp_sum_b(ep[a]);
+    em[a] = warp_sum_b(em[a]);
+  }
+}
+
+__global__ void exp_sf_kernel(const float* __restrict__ w, const float* __restrict__ sf, int R, int S,
+                              float* __restrict__ exp_sf) {
+  const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (r >= R) return;
+  float ep[3], em[3];
+  exp_sf_sums(w, sf, r, R, S, lane, ep, em);
+  if (lane < 3) exp_sf[r * 3 + lane] = fmaxf(ep[lane], em[lane]);
+}
+
+// torch.max(p, m) backward: the larger side takes the gradient; at a tie each side takes half of it.
+__global__ void exp_sf_bwd_kernel(const float* __restrict__ w, const float* __restrict__ sf,
+                                  const float* __restrict__ g_exp, int R, int S, float* __restrict__ g_w,
+                                  float* __restrict__ g_sf) {
+  const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (r >= R) return;
+  const long long N = (long long)R * S;
+  float ep[3], em[3], gp[3], gm[3];
+  exp_sf_sums(w, sf, r, R, S, lane, ep, em);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float g = g_exp[r * 3 + a];
+    gp[a] = ep[a] > em[a] ? g : (ep[a] == em[a] ? 0.5f * g : 0.f);
+    gm[a] = em[a] > ep[a] ? g : (ep[a] == em[a] ? 0.5f * g : 0.f);
+  }
+  for (int s = lane; s < S; s += 32) {
+    const long long ps = (long long)r * S + s;
+    const float* p = sf + ps * 3;
+    const float* m = sf + (N + ps) * 3;
+    if (g_w != nullptr)
+      g_w[ps] = gp[0] * p[0] + gp[1] * p[1] + gp[2] * p[2] + gm[0] * m[0] + gm[1] * m[1] + gm[2] * m[2];
+    if (g_sf != nullptr) {
+      const float wv = w[ps];
+      float* op = g_sf + ps * 3;
+      float* om = g_sf + (N + ps) * 3;
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        op[a] = wv * gp[a];
+        om[a] = wv * gm[a];
+      }
+    }
+  }
+}
+
 }  // namespace
 }  // namespace dyn
 
@@ -294,6 +420,50 @@ int dyn_traj_combine_backward(const float* g_out, const float* D, int n, int nb,
   DYN_CHECK_ARG(g_out && D && n >= 1 && nb >= 1 && nb <= 8 && P >= 0 && (g_coeff || g_base));
   traj_combine_bwd_kernel<<<cdiv((long long)P * 3, 256), 256, 0, (cudaStream_t)stream>>>(g_out, D, n, nb, P, g_coeff,
                                                                                        g_base);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+size_t dyn_traj_combine_grad_d_workspace_bytes(int n, int nb, int P) {
+  if (n <= 0 || nb <= 0 || P <= 0) return 0;
+  return (size_t)cdiv((long long)P, kGdPts) * n * nb * sizeof(float);
+}
+
+int dyn_traj_combine_grad_d(const float* g_out, const float* coeff, int n, int nb, int P, float* g_D, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  DYN_CHECK_ARG(g_D && n >= 1 && nb >= 1 && nb <= 8 && P >= 0);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (P == 0) {
+    DYN_CUDA(cudaMemsetAsync(g_D, 0, (size_t)n * nb * sizeof(float), st));
+    return DYN_OK;
+  }
+  DYN_CHECK_ARG(g_out && coeff && workspace);
+  if (workspace_bytes < dyn_traj_combine_grad_d_workspace_bytes(n, nb, P))
+    return fail(DYN_E_INVALID, "traj_combine_grad_d: workspace of %zu bytes, %zu needed", workspace_bytes,
+                dyn_traj_combine_grad_d_workspace_bytes(n, nb, P));
+  const int blocks = (int)cdiv((long long)P, kGdPts);
+  float* partial = (float*)workspace;
+  traj_grad_d_partial_kernel<<<blocks, kGdThreads, 0, st>>>(g_out, coeff, n, nb, P, partial);
+  DYN_LAUNCH_CHECK();
+  traj_grad_d_sum_kernel<<<cdiv((long long)n * nb, 128), 128, 0, st>>>(partial, blocks, n, nb, g_D);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+int dyn_expected_scene_flow(const float* weights, const float* sf, int R, int S, float* exp_sf, void* stream) {
+  if (R == 0) return DYN_OK;
+  DYN_CHECK_ARG(weights && sf && exp_sf && R > 0 && S >= 1);
+  exp_sf_kernel<<<cdiv((long long)R * 32, 256), 256, 0, (cudaStream_t)stream>>>(weights, sf, R, S, exp_sf);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+int dyn_expected_scene_flow_backward(const float* weights, const float* sf, const float* g_exp_sf, int R, int S,
+                                     float* g_weights, float* g_sf, void* stream) {
+  if (R == 0) return DYN_OK;
+  DYN_CHECK_ARG(weights && sf && g_exp_sf && (g_weights || g_sf) && R > 0 && S >= 1);
+  exp_sf_bwd_kernel<<<cdiv((long long)R * 32, 256), 256, 0, (cudaStream_t)stream>>>(weights, sf, g_exp_sf, R, S,
+                                                                                    g_weights, g_sf);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }

@@ -9,10 +9,11 @@ reference): `render_rays_mv` (render_ray.py:600), `render_rays_mono` (:870),
 All math runs in `csrc/` kernels through the C ABI (include/dynibar_b200.h);
 this file only allocates tensors and sequences calls.  `render_rays_mono` is
 differentiable (training, SURVEY 8(f) f2): when gradients are enabled and the
-model's parameters or the feature maps require grad it runs the training
-path (`_render_mono_train`, autograd Functions of dynibar_b200/autograd.py over
-the backward kernels).  `render_rays_mv` is the evaluation path (the reference
-calls it under no_grad) and refuses inputs that require grad.
+model's parameters, its trajectory basis or the feature maps require grad it runs
+the training path (`_render_mono_train`, autograd Functions of
+dynibar_b200/autograd.py over the backward kernels).  `render_rays_mv` trains its
+fine stage the same way (`_render_mv_train`) when a fine-stage tensor requires
+grad; its coarse pass always runs under no_grad, as in the reference.
 """
 
 from collections import OrderedDict
@@ -74,22 +75,35 @@ def _no_grad_only(*tensors):
 
 
 def _wants_grad(model, *featmaps):
-  """True when gradients are enabled and a parameter of the model or a feature map requires grad."""
+  """True when gradients are enabled and a parameter of the model, a tensor of the model (the trajectory basis) or a
+  feature map requires grad."""
   if not torch.is_grad_enabled():
     return False
   mods = [m for m in vars(model).values() if isinstance(m, torch.nn.Module)]
   live = any(p.requires_grad for m in mods for p in m.parameters())
+  live = live or any(torch.is_tensor(v) and v.requires_grad for v in vars(model).values())
   return live or any(torch.is_tensor(f) and f.requires_grad for fm in featmaps if fm is not None
                      for f in fm if f is not None)
 
 
-def _refuse_training(model, *featmaps):
-  """render_rays_mv runs under no_grad (evaluation path; forward-only fused kernels): a training loop that
-  called it would get detached outputs and fail late (or silently).  Fail loudly instead."""
-  if _wants_grad(model, *featmaps):
-    raise NotImplementedError(
-        "dynibar_b200.render_rays_mv is the evaluation path (forward-only fused kernels): parameters or "
-        "feature maps require grad; call under torch.no_grad() or freeze them (training = render_rays_mono)")
+_FINE_MODULES = ("net_fine_dy", "net_fine_st", "motion_mlp_fine")
+
+
+def _fine_stage_wants_grad(model, fine_featmaps):
+  """True when gradients are enabled and a tensor of render_rays_mv's fine stage requires grad: a parameter of
+  net_fine_dy / net_fine_st / motion_mlp_fine, trajectory_basis_fine, or the fine feature maps [0] / [2] (what
+  DynibarFF's optimiser updates, ibrnet/model.py:94-118).  The coarse stage never trains here: the reference runs
+  it under no_grad (render_ray.py:672)."""
+  if not torch.is_grad_enabled():
+    return False
+  mods = [getattr(model, k, None) for k in _FINE_MODULES]
+  if any(p.requires_grad for m in mods if m is not None for p in m.parameters()):
+    return True
+  basis = getattr(model, "trajectory_basis_fine", None)
+  if torch.is_tensor(basis) and basis.requires_grad:
+    return True
+  fm = fine_featmaps if fine_featmaps is not None else ()
+  return any(torch.is_tensor(f) and f.requires_grad for f in (fm[0], fm[2]) if f is not None)
 
 
 def _scalar(x):
@@ -607,10 +621,20 @@ def render_rays_mv(frame_idx, time_embedding, time_offset, ray_batch, model, pro
   outputs_fine_ref_dy, outputs_fine_anchor(None), outputs_fine_anchor_dy(None).
   `ray_batch` may be a multi-camera batch (sample_ray.stack_ray_batches): the rays of K target cameras
   of one time step, ray r seen from camera[camera_index[r]]; the index values are not checked here
-  (render_image.render_multi_image_nvi checks them once per frame)."""
+  (render_image.render_multi_image_nvi checks them once per frame).
+  With gradients enabled and a fine-stage tensor that requires grad (a parameter of net_fine_dy / net_fine_st /
+  motion_mlp_fine, trajectory_basis_fine, fine_featmaps[0] / [2]) the fine pass is differentiable
+  (`_render_mv_train`, single-camera batches only); the coarse pass never is, as in the reference."""
   assert N_importance > 0  # render_ray.py:787
-  camera_count(ray_batch)
-  _refuse_training(model, coarse_featmaps, fine_featmaps)
+  K = camera_count(ray_batch)
+  if _fine_stage_wants_grad(model, fine_featmaps):
+    if K > 1:
+      raise NotImplementedError(
+          "render_rays_mv trains on one target camera per call: multi-camera ray batches (batched target cameras) "
+          "are rendered by the forward path only; call under torch.no_grad() or freeze the fine stage")
+    with precision_scope(precision):
+      return _render_mv_train_chunked(frame_idx, time_embedding, time_offset, ray_batch, model, coarse_featmaps,
+                                      fine_featmaps, N_samples, args, inv_uniform, N_importance, det, jitter, u)
   with torch.no_grad(), precision_scope(precision):
     t = _scalar(time_embedding[0].float())
     offs = [int(o) for o in time_offset[0]]
@@ -741,6 +765,11 @@ def _render_mono_train_chunked(frame_idx, time_embedding, time_offset, ray_batch
     parts.append(_render_mono_train(frame_idx, time_embedding, time_offset, rb, model, featmaps, N_samples, args,
                                     inv_uniform, det, is_train, num_vv,
                                     None if jitter is None else jitter[lo:hi]))
+  return _cat_slices(parts)
+
+
+def _cat_slices(parts):
+  """Per-slice output dicts -> one dict, every tensor concatenated along its ray axis."""
   ret = {}
   for name, first in parts[0].items():
     if first is None:
@@ -751,18 +780,114 @@ def _render_mono_train_chunked(frame_idx, time_embedding, time_offset, ray_batch
   return ret
 
 
+def _keep_mask(S, dev):
+  """[1,S,1]: 0 on the last round(0.1 S) samples, whose motion coefficients the reference zeroes (:471-472)."""
+  keep = torch.ones(1, S, 1, device=dev)
+  n_last = int(round(S * 0.1))
+  if n_last > 0:
+    keep[:, S - n_last:] = 0.0
+  return keep
+
+
+def _basis_rows(basis, pairs, dev):
+  """D [n,nb] on `dev`, D[i] = basis[a_i] - basis[b_i]; a pair (None, None) is a zero row (these come last).  Row
+  indices wrap like the reference's (-1 = the last frame).  The model's basis tensor itself is indexed, so that a
+  basis that requires grad (trajectory_basis of DynibarMono, trajectory_basis_fine of DynibarFF) gets the gradient
+  of every row built from it.  Rows are selected with integer indices (views, no index tensor to copy to the
+  device), so building D never waits for the stream."""
+  real = [(a, b) for a, b in pairs if a is not None]
+  assert all(a is None for a, _ in pairs[len(real):]), pairs
+  bf = basis.to(device=dev, dtype=torch.float32)
+  zeros = bf.new_zeros(len(pairs) - len(real), bf.shape[1])
+  if not real:
+    return zeros
+  D = torch.stack([bf[a] for a, _ in real]) - torch.stack([bf[b] for _, b in real])
+  return torch.cat([D, zeros]) if zeros.shape[0] else D
+
+
+# ---------------------------------------------------------------------------
+# f2: differentiable fine stage of render_rays_mv (training step of DynibarFF)
+# ---------------------------------------------------------------------------
+def _render_mv_train_chunked(frame_idx, time_embedding, time_offset, ray_batch, model, coarse_featmaps, fine_featmaps,
+                             N_samples, args, inv_uniform, N_importance, det, jitter, u):
+  """Slices the rays so that no fine-stage network call exceeds TRAIN_ROWS_LIMIT rows (fine S = N_samples +
+  N_importance samples, max(V_dy, V_st) views) and concatenates the per-slice output dicts along their ray axis."""
+  R = ray_batch["ray_o"].shape[0]
+  vmax = max(ray_batch["src_cameras"].shape[1], ray_batch["static_src_cameras"].shape[1])
+  per = max(1, TRAIN_ROWS_LIMIT // ((N_samples + N_importance) * vmax))
+  call = lambda rb, jit, uu: _render_mv_train(frame_idx, time_embedding, time_offset, rb, model, coarse_featmaps,
+                                              fine_featmaps, N_samples, args, inv_uniform, N_importance, det, jit, uu)
+  if R <= per:
+    return call(ray_batch, jitter, u)
+  parts = []
+  for lo in range(0, R, per):
+    hi = min(R, lo + per)
+    rb = dict(ray_batch)
+    for k in ("ray_o", "ray_d", "uv_grid"):
+      rb[k] = ray_batch[k][lo:hi]
+    parts.append(call(rb, None if jitter is None else jitter[lo:hi], None if u is None else u[lo:hi]))
+  return _cat_slices(parts)
+
+
+def _render_mv_train(frame_idx, time_embedding, time_offset, ray_batch, model, coarse_featmaps, fine_featmaps,
+                     N_samples, args, inv_uniform, N_importance, det, jitter, u):
+  """render_rays_mv (render_ray.py:600-867) with a differentiable fine pass (fine_render_rays, :407-597).  The coarse
+  pass, the importance resampling and the fine points run under no_grad with the forward path's kernels, so
+  outputs_coarse_ref and the fine z_vals are those of the forward path (the reference detaches the coarse weights,
+  :789-791).  Every fine stage is a `torch.autograd.Function` (dynibar_b200/autograd.py); gradients reach
+  net_fine_dy / net_fine_st / motion_mlp_fine, fine_featmaps[0] / [2] and, when it requires grad,
+  trajectory_basis_fine.  render_flows covers every dynamic view and exp_sf is differentiable (:585-595)."""
+  from dynibar_b200 import autograd as ag
+  t = _scalar(time_embedding[0].float())
+  offs = [int(o) for o in time_offset[0]]
+  fidx = int(frame_idx[0])
+  rb, hb = _with_host_copies(ray_batch, model, ("trajectory_basis", "trajectory_basis_fine"))
+  with torch.no_grad():
+    pts, z, _ = sample_along_camera_ray(rb["ray_o"], rb["ray_d"], rb["depth_range"], N_samples, inv_uniform, det,
+                                        jitter)
+    out_c, _, _ = _render_pass(rb, coarse_featmaps[0], coarse_featmaps[2], pts, z, None, t, fidx, offs, 0,
+                               model.net_coarse_dy, model.net_coarse_st, model.motion_mlp, hb["trajectory_basis"],
+                               None, 2, want_extras=False)
+    zf = resample_depths(z, out_c["weights"], N_importance, inv_uniform, det, u)
+    pts_f, s = points_from_depths(rb["ray_o"], rb["ray_d"], zf, rb["depth_range"])
+    ref_plucker = compute_ref_plucker_coordinate(rb["ray_o"], rb["ray_d"])
+    src_plucker = compute_src_plucker_coordinate(pts_f, rb["static_src_cameras"])
+  ray_dir = ref_plucker[:, :3]
+  dev = dev_of(pts_f)
+  R, S = pts_f.shape[:2]
+  basis = model.trajectory_basis_fine
+  xyzt = torch.cat([pts_f, torch.full((R, S, 1), t, device=dev)], dim=-1)
+  coeff = ag.motion_mlp(model.motion_mlp_fine, xyzt) * _keep_mask(S, dev)      # :459-472
+  seq = ag.traj_combine(coeff, _basis_rows(basis, [(fidx + o, fidx) for o in offs], dev), pts_f)  # :479-497
+  cam = rb["camera"]
+  f_dy, _, m_dy = ag.project_gather(pts_f, seq, cam, rb["src_rgbs"], rb["src_cameras"], fine_featmaps[0])
+  f_st, rd_st, m_st = ag.project_gather(pts_f, None, cam, rb["static_src_rgbs"], rb["static_src_cameras"],
+                                        fine_featmaps[2])
+  raw_dy = ag.net_dynamic(model.net_fine_dy, pts_f, f_dy, ray_dir, m_dy, t)
+  raw_st = ag.net_static(model.net_fine_st, pts_f, ref_plucker, src_plucker, f_st, rd_st, m_st)
+  out = ag.composite(raw_dy, raw_st, zf, m_dy, m_st, 1, 1)
+  out_dy = ag.composite_vanilla(raw_dy, zf, m_dy, 1)
+  out["render_flows"] = ag.optical_flow(out["weights"], seq, rb["src_cameras"], rb["uv_grid"])
+  out["s_vals"] = s
+  sf = ag.traj_combine(coeff, _basis_rows(basis, [(fidx + 2, fidx), (fidx - 2, fidx)], dev))
+  out["exp_sf"] = ag.expected_scene_flow(out["weights"], sf)
+  return {"outputs_coarse": None, "outputs_fine": None, "outputs_coarse_ref": out_c, "outputs_fine_ref": out,
+          "outputs_fine_ref_dy": out_dy, "outputs_fine_anchor": None, "outputs_fine_anchor_dy": None}
+
+
 def _render_mono_train(frame_idx, time_embedding, time_offset, ray_batch, model, featmaps, N_samples, args,
                        inv_uniform, det, is_train, num_vv, jitter):
   """render_rays_mono (render_ray.py:870-1277) with autograd: the same sequence as the reference, every stage a
   `torch.autograd.Function` over the forward/backward kernels (dynibar_b200/autograd.py).  Gradients reach
-  the parameters of motion_mlp / net_coarse_dy / net_coarse_st and the feature maps.  torch itself only
+  the parameters of motion_mlp / net_coarse_dy / net_coarse_st, the feature maps and, when it requires grad,
+  trajectory_basis (through every displaced point: seq, sf_seq, pts_anchor, seq_a, pts_traj_ref).  torch itself only
   concatenates the time column, zeroes the last samples' coefficients, slices and detaches.  Precision (the
   library-wide setting / `precision=`): "bf16" runs the products of the three networks, forward and backward, on
   tensor cores (bf16 operands, fp32 accumulation, fp32 master weights and gradients); "fp32" = SIMT products."""
   from dynibar_b200 import autograd as ag
   t = _scalar(time_embedding[0].float())
   rb, hb = _with_host_copies(ray_batch, model, ("trajectory_basis",))
-  basis = hb["trajectory_basis"]  # host [T, nb]; rows indexed like the reference (negative indices wrap)
+  basis = hb["trajectory_basis"]  # host [T, nb] for the (detached) exp_sf kernel
   fidx = int(frame_idx[0])
   ref_offsets = [int(o) for o in time_offset[0]]
   with torch.no_grad():
@@ -773,14 +898,10 @@ def _render_mono_train(frame_idx, time_embedding, time_offset, ray_batch, model,
   ray_dir = ref_plucker[:, :3]
   dev = dev_of(pts)
   R, S = pts.shape[:2]
-  n_last = int(round(S * 0.1))
-  keep = torch.ones(1, S, 1, device=dev)
-  if n_last > 0:
-    keep[:, S - n_last:] = 0.0
-  zero = torch.zeros_like(basis[0])
+  keep = _keep_mask(S, dev)
 
-  def rows(pairs):  # D[i] = basis[a_i] - basis[b_i] (b = None: zero row), on the device
-    return torch.stack([basis[a] - basis[b] if a is not None else zero for a, b in pairs]).to(dev)
+  def rows(pairs):
+    return _basis_rows(model.trajectory_basis, pairs, dev)
 
   def coeffs(p, tt):  # model.motion_mlp(cat[p, t]) with the last samples zeroed (:957-958, :1126-1127)
     xyzt = torch.cat([p, torch.full((R, S, 1), tt, device=dev)], dim=-1)

@@ -359,6 +359,23 @@ int dyn_traj_combine_backward(const float* g_out, const float* D, int n, int nb,
 int dyn_flow_backward(const float* weights, const float* pts_seq, const float* src_cams, const float* g_flows,
                       int n_flow, int R, int S, float* g_weights, float* g_pts_seq, void* stream);
 
+/* Trainable trajectory basis (trajectory_basis / trajectory_basis_fine, ibrnet/model.py:94-118, :331-351):
+ * dyn_traj_combine_grad_d: the gradient of dyn_traj_combine w.r.t. its rows D, g_D[i,k] = sum_p sum_axis
+ *   g_out[i,p,axis] * coeff[p, axis*nb + k] -> g_D [n,nb] (DEVICE).  Autograd routes it to the basis rows each D row
+ *   was built from (render_ray.py:361-369, :462-500, :1101-1176).  A two-stage reduction over the P points through
+ *   `workspace` (dyn_traj_combine_grad_d_workspace_bytes(n, nb, P) bytes) without float atomics: the same inputs
+ *   always give the same bits.  nb <= 8.
+ * dyn_expected_scene_flow(_backward): exp_sf (render_ray.py:585-595, the mv fine pass, differentiable there):
+ *   sf [2,R,S,3] = (traj(f+k) - traj(f), traj(f-k) - traj(f)), weights [R,S] -> exp_sf [R,3] =
+ *   max(sum_s w*sf[0], sum_s w*sf[1]) per axis.  The backward writes g_weights [R,S] and / or g_sf [2,R,S,3] (either
+ *   may be NULL); at a tie each side takes half of the gradient, as torch.max(p, m) does. */
+size_t dyn_traj_combine_grad_d_workspace_bytes(int n, int nb, int P);
+int dyn_traj_combine_grad_d(const float* g_out, const float* coeff, int n, int nb, int P, float* g_D, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int dyn_expected_scene_flow(const float* weights, const float* sf, int R, int S, float* exp_sf, void* stream);
+int dyn_expected_scene_flow_backward(const float* weights, const float* sf, const float* g_exp_sf, int R, int S,
+                                     float* g_weights, float* g_sf, void* stream);
+
 /* Unit-test hooks of the tensor-core training products (csrc/train_tc.cu; bf16 operands, fp32 accumulation):
  * dyn_debug_tc_grad_w: dW[out,width] += dz[rows,out]^T (x[rows,width] * kscale[rows] or 1); out, width <= 256.
  * dyn_debug_tc_grad_in: din[rows,width] = dz[rows,out] W[out, 0:width] (W row-major with ldw columns). */
