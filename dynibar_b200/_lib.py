@@ -25,6 +25,33 @@ NET_DYNAMIC, NET_STATIC, NET_MOTION = 0, 1, 2
 
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
+# ---- the criterion's host structs (include/dynibar_b200.h: dyn_mono_loss*) -------------------------------
+LOSS_RGB_SLOTS, LOSS_TERMS, LOSS_OUT_FLOATS = 6, 15, 40
+LOSS_SLOT_COMPLEMENT_W0, LOSS_SLOT_TIMES_ONE_MINUS_RATIO = 1, 2
+
+
+class LossRgbSlot(C.Structure):
+  _fields_ = [("pred", _vp), ("mask", _vp), ("w0", _vp), ("w1", _vp), ("ld", _i), ("flags", _i)]
+
+
+class MonoLossInputs(C.Structure):
+  _fields_ = ([("rgb", LossRgbSlot * LOSS_RGB_SLOTS)] +
+              [(k, _vp) for k in ("gt_rgb", "depth", "gt_disp", "ray_mask", "flows", "gt_flows", "flow_masks",
+                                  "traj_ref", "traj_anchor", "occ_weights", "sf_seq", "weights_dy", "weights_st",
+                                  "dist_w", "s_vals", "dist_m", "dist_interval")] +
+              [(k, _i) for k in ("R", "S", "depth_ld", "n_flow", "K", "n_sf", "dist_ld", "dist_n")])
+
+
+class MonoLossWeights(C.Structure):
+  _fields_ = [("terms", C.c_uint), ("w", _f * LOSS_TERMS), ("rgb_eps", _f * LOSS_RGB_SLOTS)]
+
+
+class MonoLossGrads(C.Structure):
+  _fields_ = ([("rgb", _vp * LOSS_RGB_SLOTS)] +
+              [(k, _vp) for k in ("depth", "flows", "weights", "weights_dy", "weights_st", "traj_ref", "traj_anchor",
+                                  "sf_seq")])
+
+
 # name -> (restype, argtypes); mirrors include/dynibar_b200.h one to one
 SIGNATURES = {
     "dyn_version": (_i, []),
@@ -99,6 +126,10 @@ SIGNATURES = {
     "dyn_traj_combine_grad_d": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "dyn_expected_scene_flow": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "dyn_expected_scene_flow_backward": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "dyn_mono_loss_workspace_bytes": (_sz, [_i]),
+    "dyn_mono_loss": (_i, [C.POINTER(MonoLossInputs), C.POINTER(MonoLossWeights), _vp, _vp, _sz, _vp]),
+    "dyn_mono_loss_backward": (_i, [C.POINTER(MonoLossInputs), C.POINTER(MonoLossWeights), _vp, _vp,
+                                    C.POINTER(MonoLossGrads), _vp]),
     "dyn_debug_tc_grad_w": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "dyn_debug_tc_grad_in": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _vp, _sz, _vp]),
     "dyn_debug_tc_grad_in_scratch_bytes": (_sz, []),

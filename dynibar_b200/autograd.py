@@ -19,11 +19,14 @@ of the path, so that `render_ray.render_rays_mono(..., is_train=True)` is differ
                         including the gradient w.r.t. the trajectory-basis rows.
   * `optical_flow`      compute_optical_flow (render_ray.py:333-358).
   * `expected_scene_flow`  exp_sf of the mv fine pass (render_ray.py:585-595).
+  * `mono_loss`         the criterion of a DynibarMono step (train.py:187-196, :300-456): every loss term in one
+                        forward and one backward call (csrc/loss.cu); dynibar_b200/criterion.py is its interface.
 
 tests/test_backward_gpu.py and tests/test_train_gpu.py check them -- and the whole training forward/backward --
 against torch autograd through the oracle's restatement of the same functions.
 """
 
+import ctypes
 from collections import OrderedDict
 
 import torch
@@ -429,3 +432,108 @@ class _OpticalFlow(torch.autograd.Function):
 def optical_flow(weights, pts_seq, src_cameras, uv_grid):
   """Differentiable compute_optical_flow -> [n,R,2] for the n views of pts_seq."""
   return _OpticalFlow.apply(weights, pts_seq, src_cameras, uv_grid)
+
+
+# the differentiable inputs of the criterion, in the order _MonoLoss takes them, and the terms (bits of
+# dyn_mono_loss_weights.terms) through which each one is reached
+_LOSS_INPUTS = OrderedDict(
+    [("rgb%d" % k, 1 << k) for k in range(6)] +
+    [("depth", 1 << 6), ("flows", 1 << 7), ("weights", 1 << 13), ("weights_dy", (1 << 12) | (1 << 14)),
+     ("weights_st", 1 << 12), ("traj_ref", 1 << 8), ("traj_anchor", 1 << 8), ("sf_seq", 7 << 9)])
+
+
+def _rows(A, t, width):
+  """(pointer, row stride in floats) of a per-ray tensor [R,width] ([R] when width is 1); a column slice of a wider
+  row-major tensor (the outputs of `composite`) is read in place."""
+  c = t.detach()
+  if c.dtype != torch.float32:
+    c = c.to(torch.float32)
+  if c.dim() != (1 if width == 1 else 2) or (width > 1 and (c.shape[1] != width or c.stride(1) != 1)) \
+      or c.stride(0) < width:
+    c = c.reshape(-1, width).contiguous() if width > 1 else c.reshape(-1).contiguous()
+  dev_of(c)
+  A.keep.append(c)
+  return c.data_ptr(), c.stride(0)
+
+
+class _MonoLoss(torch.autograd.Function):
+  @staticmethod
+  def forward(ctx, weights, fixed, *diff):
+    from dynibar_b200 import _lib
+    x = dict(zip(_LOSS_INPUTS, diff))
+    R, S = int(fixed["R"]), int(fixed["S"])
+    A, inp = Args(), _lib.MonoLossInputs()
+    inp.R, inp.S = R, S
+    on = lambda k: (weights.terms >> k) & 1
+    for k in range(_lib.LOSS_RGB_SLOTS):
+      slot = fixed.get("slot%d" % k)
+      if slot is None:
+        continue
+      sl = inp.rgb[k]
+      if x["rgb%d" % k] is not None:
+        sl.pred, sl.ld = _rows(A, x["rgb%d" % k], 3)
+      sl.mask, sl.w0, sl.w1, sl.flags = A(slot.get("mask"), torch.bool), A(slot.get("w0")), A(slot.get("w1")), \
+          int(slot.get("flags", 0))
+    inp.gt_rgb = A(fixed.get("gt_rgb"))
+    if on(6):
+      inp.depth, inp.depth_ld = _rows(A, x["depth"], 1)
+      inp.gt_disp = A(fixed["gt_disp"])
+    inp.ray_mask = A(fixed.get("ray_mask"), torch.bool)
+    if on(7):
+      inp.flows, inp.gt_flows, inp.flow_masks = A(x["flows"]), A(fixed["gt_flows"]), A(fixed["flow_masks"])
+      inp.n_flow = int(x["flows"].shape[0])
+    if on(8):
+      inp.traj_ref, inp.traj_anchor, inp.occ_weights = A(x["traj_ref"]), A(x["traj_anchor"]), A(fixed["occ_weights"])
+      inp.K = int(x["traj_ref"].shape[0])
+    if on(9) or on(10) or on(11):
+      inp.sf_seq, inp.n_sf = A(x["sf_seq"]), int(x["sf_seq"].shape[0])
+    inp.weights_dy, inp.weights_st = A(x["weights_dy"]), A(x["weights_st"])
+    if on(13):
+      inp.dist_w, inp.dist_ld, inp.dist_n = A(x["weights"]), int(x["weights"].shape[1]), int(fixed["dist_n"])
+      inp.s_vals, inp.dist_m, inp.dist_interval = A(fixed.get("s_vals")), A(fixed.get("dist_m")), \
+          A(fixed.get("dist_interval"))
+    if not A.keep:
+      raise ValueError("dynibar_b200: the criterion was given no tensor")
+    dev = dev_of(A.keep[0])
+    out = torch.empty(_lib.LOSS_OUT_FLOATS, device=dev)
+    nbytes = int(lib.dyn_mono_loss_workspace_bytes(R))
+    ws = _lib.workspace.get(nbytes, dev, slot=5)
+    with torch.cuda.device(dev):
+      check(lib.dyn_mono_loss(ctypes.byref(inp), ctypes.byref(weights), ptr(out), ws.data_ptr(), nbytes, stream()))
+    ctx.inp, ctx.weights, ctx.keep, ctx.out = inp, weights, A, out
+    ctx.shapes = [(None if t is None else (t.shape, t.dtype)) for t in diff]
+    return out
+
+  @staticmethod
+  def backward(ctx, g_out):
+    from dynibar_b200 import _lib
+    dev = ctx.out.device
+    g = f32c(g_out)  # element 0 = d / d loss: read by the kernel from device memory
+    gr, grads = _lib.MonoLossGrads(), []
+    for i, (name, bits) in enumerate(_LOSS_INPUTS.items()):
+      t = None
+      if ctx.shapes[i] is not None and ctx.needs_input_grad[2 + i] and (ctx.weights.terms & bits):
+        t = torch.empty(ctx.shapes[i][0], device=dev)
+        if name.startswith("rgb"):
+          gr.rgb[int(name[3:])] = ptr(t)
+        else:
+          setattr(gr, name, ptr(t))
+      grads.append(t)
+    if any(t is not None for t in grads):
+      with torch.cuda.device(dev):
+        check(lib.dyn_mono_loss_backward(ctypes.byref(ctx.inp), ctypes.byref(ctx.weights), ptr(ctx.out), ptr(g),
+                                         ctypes.byref(gr), stream()))
+    grads = [t if t is None or t.dtype == ctx.shapes[i][1] else t.to(ctx.shapes[i][1]) for i, t in enumerate(grads)]
+    return (None, None) + tuple(grads)
+
+
+def mono_loss(term_weights, fixed, **inputs):
+  """The criterion kernels (csrc/loss.cu) as one differentiable call -> out [40] (include/dynibar_b200.h,
+  dyn_mono_loss): out[0] is the loss and the only differentiable element; out[1:9] are the logged scalars, out[9:24]
+  the unweighted components.  `term_weights`: a `_lib.MonoLossWeights`; `fixed`: R, S and the tensors that carry no
+  gradient (supervision, masks, occ_weights, s_vals; "slot<k>" = dict(mask, w0, w1, flags) of rgb slot k); `inputs`:
+  the differentiable tensors by the names of `_LOSS_INPUTS` (absent = None)."""
+  unknown = set(inputs) - set(_LOSS_INPUTS)
+  if unknown:
+    raise TypeError("mono_loss: unknown inputs %s" % sorted(unknown))
+  return _MonoLoss.apply(term_weights, fixed, *[inputs.get(k) for k in _LOSS_INPUTS])

@@ -376,6 +376,92 @@ int dyn_expected_scene_flow(const float* weights, const float* sf, int R, int S,
 int dyn_expected_scene_flow_backward(const float* weights, const float* sf, const float* g_exp_sf, int R, int S,
                                      float* g_weights, float* g_sf, void* stream);
 
+/* ---- f2: the monocular training criterion (train.py:187-196 and :300-456, ibrnet/criterion.py, utils.py:32-39) ----
+ * Every loss term of a DynibarMono step in one forward and one backward call (csrc/loss.cu).  A term is a bit of
+ * `terms` and an entry of `w`; a cleared bit is an absent term (its pointers may be NULL, it contributes 0 and its
+ * inputs get no gradient).  Term k, its component c_k = numerator / denominator, and what enters the loss:
+ *    0..5  Charbonnier of rgb slot k: sum_r m_r sum_c sqrt((pred - gt)^2 + 1e-6) / (3 sum_r m_r + rgb_eps[k]);
+ *          m_r = mask (bytes, 0 / non-0) * w0 (or 1 - w0 with flag 1) * w1 [* (1 - weights_ratio), flag 2],
+ *          each factor optional.  rgb_eps: 1e-6 for utils.img2charbonier, 1e-8 for compute_temporal_rgb_loss.
+ *          Slots 0-4 add up to rgb_loss (train.py:304-328), slot 5 is the static loss (:426-434, :187-196).
+ *    6     disparity :331-342: sum |1 / max(depth, 1e-2) - gt_disp| mask / (sum mask + 1e-8)
+ *    7     flow :345-351, criterion.py:83-85: L1 over [n_flow,R,2] under ray mask * flow_masks [n_flow,R]
+ *    8     trajectory cycle :359-371 over traj_ref / traj_anchor [K,R,S,3] weighted by occ_weights [R,S]
+ *    9-11  scene-flow regularisers :376-397 over sf_seq [n_sf,R,S,3]: mean |x|, mean (x[v] - x[v+1])^2 (give
+ *          w = w_reg / 2), mean |x[:, s+1] - x[:, s]|
+ *    12    entropy :400-413 of weights_ratio = sum_s weights_dy / max(sum_s weights_dy + sum_s weights_st, 1e-9)
+ *    13    distortion :416-423 on dist_w [R, dist_n] (rows dist_ld floats apart) with mid-points and intervals
+ *          either given (dist_m, dist_interval [R, dist_n]) or formed from s_vals [R, dist_n + 1]
+ *    14    :437-445 sum |sum_s weights_dy * m2| / sum (m2 + 1e-8), m2 = m of slot 5 where weights_ratio < 0.1;
+ *          joins slot 5 in static_loss
+ * loss = sum_k w[k] c_k.  `out` receives DYN_LOSS_OUT_FLOATS floats: [0..8] loss, flow_loss, disp_loss, rgb_loss,
+ * distortion_loss, entropy_loss, static_loss, cycle_loss, reg_loss (the weighted sums train.py:447-464 logs);
+ * [9 + k] c_k; [24 + k] w[k] / denominator_k, the table the backward reads.
+ * Two launches: one warp per ray writes a block's partial sums into `workspace`
+ * (dyn_mono_loss_workspace_bytes(R) bytes), one block then adds them in block order.  No float atomics: the same
+ * inputs give the same bits.  S >= 2; with term 9-11 n_sf >= 2; with term 13 dist_n <= 256.
+ * dyn_mono_loss_backward: `g_loss` is the DEVICE address of d/d loss, `out` the forward's output.  Every non-NULL
+ * pointer of `grads` is written exactly once per element in one launch (no zero-fill needed): rgb[k] [R,3],
+ * depth [R], flows [n_flow,R,2], weights [R,dist_ld] (columns >= dist_n get 0), weights_dy / weights_st [R,S],
+ * traj_ref / traj_anchor [K,R,S,3], sf_seq [n_sf,R,S,3].  The (1 - weights_ratio) factor and m2 carry no gradient
+ * (detached in the reference).  Both structs are HOST structs read before the call returns. */
+#define DYN_LOSS_RGB_SLOTS 6
+#define DYN_LOSS_TERMS 15
+#define DYN_LOSS_OUT_FLOATS 40
+#define DYN_LOSS_SLOT_COMPLEMENT_W0 1
+#define DYN_LOSS_SLOT_TIMES_ONE_MINUS_RATIO 2
+typedef struct {
+  const float* pred; /* [R,3], rows `ld` floats apart */
+  const uint8_t* mask; /* [R] or NULL */
+  const float* w0;   /* [R] or NULL */
+  const float* w1;   /* [R] or NULL */
+  int ld;
+  int flags;
+} dyn_loss_rgb_slot;
+typedef struct {
+  dyn_loss_rgb_slot rgb[DYN_LOSS_RGB_SLOTS];
+  const float* gt_rgb; /* [R,3] */
+  const float* depth;  /* [R], elements depth_ld floats apart */
+  const float* gt_disp;
+  const uint8_t* ray_mask; /* [R] or NULL: the mask of terms 6 and 7 */
+  const float* flows;
+  const float* gt_flows;
+  const float* flow_masks;
+  const float* traj_ref;
+  const float* traj_anchor;
+  const float* occ_weights;
+  const float* sf_seq;
+  const float* weights_dy;
+  const float* weights_st;
+  const float* dist_w;
+  const float* s_vals;
+  const float* dist_m;
+  const float* dist_interval;
+  int R, S, depth_ld, n_flow, K, n_sf, dist_ld, dist_n;
+} dyn_mono_loss_inputs;
+typedef struct {
+  unsigned terms;
+  float w[DYN_LOSS_TERMS];
+  float rgb_eps[DYN_LOSS_RGB_SLOTS];
+} dyn_mono_loss_weights;
+typedef struct {
+  float* rgb[DYN_LOSS_RGB_SLOTS];
+  float* depth;
+  float* flows;
+  float* weights;
+  float* weights_dy;
+  float* weights_st;
+  float* traj_ref;
+  float* traj_anchor;
+  float* sf_seq;
+} dyn_mono_loss_grads;
+size_t dyn_mono_loss_workspace_bytes(int R);
+int dyn_mono_loss(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host, float* out,
+                  void* workspace, size_t workspace_bytes, void* stream);
+int dyn_mono_loss_backward(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host,
+                           const float* out, const float* g_loss, const dyn_mono_loss_grads* grads_host,
+                           void* stream);
+
 /* Unit-test hooks of the tensor-core training products (csrc/train_tc.cu; bf16 operands, fp32 accumulation):
  * dyn_debug_tc_grad_w: dW[out,width] += dz[rows,out]^T (x[rows,width] * kscale[rows] or 1); out, width <= 256.
  * dyn_debug_tc_grad_in: din[rows,width] = dz[rows,out] W[out, 0:width] (W row-major with ldw columns). */
