@@ -13,7 +13,8 @@
 //
 // One persistent CTA per SM.  Per 128-row iteration a thread of the producer warpgroup lands the input tile (the
 // G, O or X tile image) with one bulk copy; both consumer warpgroups read their 64 rows of it as the A operand
-// of the first layer, and the tile is refilled for the next iteration as soon as both have retired that layer.
+// of the first layer, and the tile is refilled for the next iteration as soon as both have retired that layer
+// (the blending head instead keeps its weights resident and streams its X tiles through a ring).
 // Every later layer takes A from registers (the dynamic point2 also from two small per-warpgroup tiles of
 // positional encodings).  Each layer is one wgmma per k-step at its full width (N = 256, 128 or 64).
 //
@@ -726,77 +727,173 @@ __global__ void __launch_bounds__(256, 1) attention_wg_kernel(const uint8_t* __r
 // static colour-blending head (rows = (point, view slot), VP slots per point)
 // input tile = the X image the per-view kernel writes (16 k-groups); k-step 8 of rgb_fc.0 is a register
 // fragment holding [vis2, ray_diff(4), 0 x 11]
+// A streaming kernel: its whole weight image (5 chunks, 80 KB) stays in shared memory for the CTA's lifetime, and
+// one producer thread keeps kRhDepth iterations in flight, each an X tile plus the GW rows of its 128 / VP points;
+// every consumer thread loads the per-row scalars of its next iteration while it finishes the current one, so no
+// global load latency sits on the consumers' critical path.
 // ---------------------------------------------------------------------------
 constexpr int kRhTile = 16 * 2048;
+constexpr int kRhChunks = 5;  // rgb_fc.0: 3 chunks (4, 4, 1 k-steps), rgb_fc.2: 2 chunks (8, 1)
+constexpr int kRhDepth = 3;   // slots of the X / GW ring: 80 KB + 3 x 40.5 KB
+// GW of an iteration's points in a slot: 32 groups of 4 columns (the fp32 tile layout's groups), each group the 16 B
+// of every point, group stride padded by 16 B so that the two groups a warp's load touches fall in different banks
+template <int VP>
+__host__ __device__ constexpr int rh_gw_stride() { return (128 / VP) * 16 + 16; }
+constexpr int kRhGw = 32 * rh_gw_stride<8>();
 constexpr int C_RW4 = 0, C_RB4 = 64;  // ln 2 x rgb_fc.4 weights, its bias
 constexpr int kRhConst = 68;
-using RhSmem = ChainSmem<kRhTile, 0, kRhConst>;
+// shared memory: resident weights | X ring | GW ring | constants | barriers: weights landed, then full / empty per slot
+struct RhSmem {
+  static constexpr int kXOff = kRhChunks * kWgStage;
+  static constexpr int kGwOff = kXOff + kRhDepth * kRhTile;
+  static constexpr int kConstOff = kGwOff + kRhDepth * kRhGw;
+  static constexpr int kBarOff = (kConstOff + kRhConst * 4 + 7) & ~7;
+  static constexpr int kBytes = kBarOff + (1 + 2 * kRhDepth) * 8;
+  static_assert(kBytes <= 227 * 1024, "shared memory of one CTA");
+};
+__device__ __forceinline__ uint32_t rh_full(uint32_t bar0, uint32_t slot) { return bar0 + 8u * (1 + slot); }
+__device__ __forceinline__ uint32_t rh_empty(uint32_t bar0, uint32_t slot) {
+  return bar0 + 8u * (1 + kRhDepth + slot);
+}
+
+// This thread's two rows row0 + fr[h] of an iteration (row0 a multiple of VP): their point, whether it exists,
+// whether the view slot holds a view, and the per-view row index m = point * V + view.
+template <int VP>
+__device__ __forceinline__ void head_rows(const RgbHeadArgs& a, long long row0, const int* fr, long long* pl,
+                                          bool* pt_ok, bool* valid, long long* m) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int v = fr[h] & (VP - 1);
+    pl[h] = (row0 + fr[h]) / VP;
+    pt_ok[h] = pl[h] < a.P;
+    valid[h] = pt_ok[h] && v < a.V;
+    m[h] = pl[h] * a.V + v;
+  }
+}
+
+// What an iteration reads from global memory besides the X tile and GW, for this thread's two rows: vis2 and
+// ray_diff (operand columns 128..132 of rgb_fc.0; lane q holds columns 2 q, 2 q + 1), the masked-softmax inputs
+// and the density passed through to raw.
+struct HeadIn {
+  float vis[2];
+  float4 rd[2];
+  float mk[2], c3[2][3], sig[2];
+};
+// Issues the loads of HeadIn for the iteration whose rows start at row0; rows past the end read zeros.
+template <int VP>
+__device__ __forceinline__ void head_load(const RgbHeadArgs& a, long long row0, const int* fr, int q, HeadIn& in) {
+  long long pl[2], m[2];
+  bool pt_ok[2], valid[2];
+  head_rows<VP>(a, row0, fr, pl, pt_ok, valid, m);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    in.vis[h] = 0.f;
+    in.rd[h] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (valid[h] && q < 3) {
+      in.vis[h] = a.vis2[m[h]];
+      in.rd[h] = __ldg(reinterpret_cast<const float4*>(a.ray_diff) + m[h]);
+    }
+    in.mk[h] = 0.f;
+    in.c3[h][0] = in.c3[h][1] = in.c3[h][2] = 0.f;
+    if (valid[h]) {
+      in.mk[h] = a.mask_eff[m[h]];
+      in.c3[h][0] = a.rgb_in[m[h] * 3]; in.c3[h][1] = a.rgb_in[m[h] * 3 + 1]; in.c3[h][2] = a.rgb_in[m[h] * 3 + 2];
+    }
+    in.sig[h] = pt_ok[h] ? a.sigma[pl[h]] : 0.f;
+  }
+}
 
 template <int VP>
 __global__ void __launch_bounds__(kWgThreads, 1) rgbhead_wg_kernel(const __grid_constant__ RgbHeadArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(16) FusedChunk s_tab[kWgMaxChunks];
-  const uint32_t bar0 = chain_init(smem, RhSmem::kBarOff, s_tab, a.chunks, a.nchunks);
+  const uint32_t bar0 = smem_u32(smem + RhSmem::kBarOff);
   float* cst = reinterpret_cast<float*>(smem + RhSmem::kConstOff);
   const int tid = threadIdx.x, lane = tid & 31;
+  if (tid == 0) {
+    mbar_init(bar0, 1);
+    for (int s = 0; s < kRhDepth; ++s) {
+      mbar_init(rh_full(bar0, s), 1);
+      mbar_init(rh_empty(bar0, s), 8);  // 4 warps x 2 warpgroups
+    }
+    mbar_fence_init();
+  }
   for (int i = tid; i < 64; i += blockDim.x) cst[C_RW4 + i] = a.params[a.o_wrgb4 + i] * kLn2;
   if (tid == 0) cst[C_RB4] = a.params[a.o_brgb4];
   __syncthreads();
   const int n_iter = (int)((a.P * VP + 127) / 128);
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
   if (wg == 2) {
-    chain_producers(s_tab, a.nchunks, a.wimg, a.X, (uint32_t)kRhTile, n_iter, smem, bar0);
+    setmaxnreg_dec<kProducerRegs>();
+    if ((tid & 127) == 0) {
+      // the weight image, once
+      const uint8_t* w = reinterpret_cast<const uint8_t*>(a.wimg);
+      uint32_t bytes = 0;
+      for (int c = 0; c < kRhChunks; ++c) bytes += a.chunks[c].bytes;
+      mbar_arrive_expect_tx(bar0, bytes);
+      for (int c = 0; c < kRhChunks; ++c)
+        bulk_g2s(smem_u32(smem + c * kWgStage), w + a.chunks[c].off, a.chunks[c].bytes, bar0);
+      // per iteration the X tile and the GW rows of its points, into a slot as soon as both consumer warpgroups have
+      // released the slot's previous iteration.  GW is allocated in whole 128-point tiles, so the points of the last
+      // iteration that lie past the end can be read too; no output depends on them.
+      const uint8_t* x = reinterpret_cast<const uint8_t*>(a.X);
+      const uint8_t* gw = reinterpret_cast<const uint8_t*>(a.GW);
+      constexpr uint32_t kGwRow = (128 / VP) * 16;  // one group of the iteration's points
+      uint32_t k = 0;
+      for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++k) {
+        const uint32_t s = k % kRhDepth, full = rh_full(bar0, s);
+        if (k >= kRhDepth) mbar_wait(rh_empty(bar0, s), (k / kRhDepth - 1) & 1);
+        mbar_arrive_expect_tx(full, kRhTile + 32 * kGwRow);
+        bulk_g2s(smem_u32(smem + RhSmem::kXOff + s * kRhTile), x + (size_t)it * kRhTile, kRhTile, full);
+        const uint32_t gdst = smem_u32(smem + RhSmem::kGwOff + s * kRhGw);
+        const long long p0 = (long long)it * (128 / VP);
+        for (int g = 0; g < 32; ++g) bulk_g2s(gdst + g * rh_gw_stride<VP>(), gw + tile_f32_off(p0, g), kGwRow, full);
+      }
+    }
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
   const int q = lane & 3, ww = (tid & 127) >> 5;
   const int fr[2] = {16 * ww + (lane >> 2), 16 * ww + (lane >> 2) + 8};
-  Ring rg{smem, bar0, 0u, false, 0};
-  const uint32_t tile = smem_u32(smem + RhSmem::kTileOff) + 1024u * wg;
+  Resident rg{smem, 0u};
+  const uint32_t x0 = smem_u32(smem + RhSmem::kXOff) + 1024u * wg;  // this warpgroup's 64 rows of slot 0
+  const uint8_t* gw_slot = smem + RhSmem::kGwOff;
+  HeadIn in;
+  head_load<VP>(a, (long long)blockIdx.x * 128 + 64 * wg, fr, q, in);
+  mbar_wait(bar0, 0);  // the weights have landed
   uint32_t k = 0;
   for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++k) {
     const long long row0 = (long long)it * 128 + 64 * wg;  // a multiple of VP
     long long pl[2], m[2];
     bool pt_ok[2], valid[2];
+    head_rows<VP>(a, row0, fr, pl, pt_ok, valid, m);
     uint32_t a8[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int v = fr[h] & (VP - 1);
-      pl[h] = (row0 + fr[h]) / VP;
-      pt_ok[h] = pl[h] < a.P;
-      valid[h] = pt_ok[h] && v < a.V;
-      m[h] = pl[h] * a.V + v;
-      // operand columns 128..132: vis2, ray_diff (lane q holds columns 2 q, 2 q + 1)
-      float vis = 0.f;
-      float4 rd = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (valid[h] && q < 3) {
-        vis = a.vis2[m[h]];
-        rd = __ldg(reinterpret_cast<const float4*>(a.ray_diff) + m[h]);
-      }
-      a8[h] = q == 0 ? pack_bf16x2(vis, rd.x) : q == 1 ? pack_bf16x2(rd.y, rd.z) : pack_bf16x2(q == 2 ? rd.w : 0.f, 0.f);
+      const float4 rd = in.rd[h];
+      a8[h] = q == 0 ? pack_bf16x2(in.vis[h], rd.x) : q == 1 ? pack_bf16x2(rd.y, rd.z)
+                                                            : pack_bf16x2(q == 2 ? rd.w : 0.f, 0.f);
     }
+    const uint32_t s = k % kRhDepth, tile = x0 + s * kRhTile;
     float acc[64];
-    tile_wait(bar0, k);
+    mbar_wait(rh_full(bar0, s), (k / kRhDepth) & 1);
+    rg.cnt = 0;
     // rgb_fc.0, per-view part (weights x log2 e): accumulator on the exp2 scale
     layer_issue<128, 9>(acc, rg, [&](float* d, int ks, uint64_t bd, uint32_t sc) {
       if (ks < 8) Wgmma<128, 0, 0>::mma(d, smem_desc(tile + ks * 4096u, 2048u, 128u), bd, sc);
       else WgmmaRS<128>::mma(d, a8, bd, sc);
     });
-    // per-point part of rgb_fc.0 (GW, bias included) and the masked-softmax inputs: loaded behind the MMA
+    // per-point part of rgb_fc.0 (GW, bias included) of this thread's rows, read behind the MMA
     float2 gw[2][16];
-    float mk[2] = {0.f, 0.f}, c3[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const long long p = pt_ok[h] ? pl[h] : 0;
+      const uint8_t* g = gw_slot + s * kRhGw + ((64 * wg + fr[h]) / VP) * 16 + (q & 1) * 8;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) gw[h][j] = __ldg(f32_pair(a.GW, p, 8 * j + 2 * q));
-      if (valid[h]) {
-        mk[h] = a.mask_eff[m[h]];
-        c3[h][0] = a.rgb_in[m[h] * 3]; c3[h][1] = a.rgb_in[m[h] * 3 + 1]; c3[h][2] = a.rgb_in[m[h] * 3 + 2];
-      }
+      for (int j = 0; j < 16; ++j)
+        gw[h][j] = *reinterpret_cast<const float2*>(g + (2 * j + (q >> 1)) * rh_gw_stride<VP>());
     }
     layer_finish<128>(acc, rg);
-    tile_release(bar0);
+    __syncwarp();  // this warp's wgmmas that read the slot's X tile have retired, and its GW reads are done
+    if (lane == 0) mbar_arrive(rh_empty(bar0, s));
     uint32_t ah[9][4];
 #pragma unroll
     for (int j = 0; j < 16; ++j)
@@ -808,6 +905,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) rgbhead_wg_kernel(const __grid_
     to_afrag<8>(acc, *reinterpret_cast<uint32_t(*)[8][4]>(ah));
     bias_afrag(ah[8], 0, q);  // operand columns 128, 129
     layer_rs<64, 9>(acc, ah, rg);  // rgb_fc.2 (bias folded, exp2 scale) -> rgb_fc.4 logit
+    const float mk[2] = {in.mk[0], in.mk[1]}, sig[2] = {in.sig[0], in.sig[1]};
+    const float c3[2][3] = {{in.c3[0][0], in.c3[0][1], in.c3[0][2]}, {in.c3[1][0], in.c3[1][1], in.c3[1][2]}};
+    head_load<VP>(a, row0 + (long long)gridDim.x * 128, fr, q, in);  // the next iteration's inputs
     float lg[2] = {0.f, 0.f};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -844,7 +944,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) rgbhead_wg_kernel(const __grid_
 #pragma unroll
     for (int h = 0; h < (VP == 8 ? 2 : 1); ++h)
       if (lane == 0 && pt_ok[h])
-        reinterpret_cast<float4*>(a.raw)[pl[h]] = make_float4(b[0][h], b[1][h], b[2][h], a.sigma[pl[h]]);
+        reinterpret_cast<float4*>(a.raw)[pl[h]] = make_float4(b[0][h], b[1][h], b[2][h], sig[h]);
   }
 }
 
@@ -1055,6 +1155,9 @@ int launch_attention_wg(const __nv_bfloat16* Q, const __nv_bfloat16* K, const __
 
 int launch_rgbhead_wg(const dyn_net* n, RgbHeadArgs& a, cudaStream_t st) {
   if (!n->chain[1].img) return fail(DYN_E_INVALID, "static net has no blending-head images");
+  if (n->chain[1].nchunks != kRhChunks)
+    return fail(DYN_E_INVALID, "blending-head image has %d chunks, the kernel keeps %d resident", n->chain[1].nchunks,
+                kRhChunks);
   a.wimg = n->chain[1].img; a.chunks = n->chain[1].tab; a.nchunks = n->chain[1].nchunks;
   a.params = n->params;
   a.o_wrgb4 = n->sl.rgb4.w; a.o_brgb4 = n->sl.rgb4.b;

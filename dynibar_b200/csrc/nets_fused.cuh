@@ -108,6 +108,8 @@ struct PointFusedArgs {
   __nv_bfloat16* O;
 };
 
+// The blending head reads X in whole 128-row tiles and GW (fp32 tile layout) in whole 128-point tiles, so both
+// are allocated in whole tiles.
 struct RgbHeadArgs {
   const float *X /* bf16 tile image, 16 k-groups, rows = view slots (point * VP + view) */, *vis2, *ray_diff, *mask_eff, *rgb_in, *GW, *sigma;
   long long P;

@@ -60,6 +60,16 @@ struct RingN {
 };
 using Ring = RingN<kWgRing>;
 
+// A weight image resident in shared memory for the kernel's lifetime, landed once before the first iteration:
+// chunk c of an iteration sits in slot c, so there is nothing to wait for and nothing to release.  The consumer
+// resets cnt to 0 at the start of every iteration.
+struct Resident {
+  uint8_t* base;
+  uint32_t cnt;
+  __device__ __forceinline__ uint32_t wait_full(uint32_t c) const { return smem_u32(base + c * kWgStage); }
+  __device__ __forceinline__ void release(uint32_t) const {}
+};
+
 // Issues one layer, D[64 x N] = A[64 x 16 KS] W^T, chunk by chunk as the weights arrive; each chunk's slot is
 // released as soon as the next chunk's wgmmas are committed and its own have retired.  The last chunk stays in
 // flight: layer_finish waits for it.  mma(acc, kstep, b_desc, scale_d) issues one k-step.

@@ -26,6 +26,15 @@ def mac_per_point(kind, S):
   raise ValueError(kind)
 
 
+def rgbhead_bytes(points, V):
+  """HBM bytes the static blending head (csrc/chains_wg.cu: rgbhead_wg_kernel) moves for `points` points with V
+  source views: per view slot (VP = 8 for V <= 8, else 16) its 256-byte bf16 X row; per view vis2, mask_eff,
+  ray_diff and rgb_in (36 B); per point its 512-byte fp32 GW row and sigma in, and raw (16 B) out.  The
+  weights (54 KB per CTA) are not counted."""
+  VP = 8 if V <= 8 else 16
+  return points * (VP * 256 + V * 36 + 512 + 4 + 16)
+
+
 def flop_per_ray(S_coarse, S_fine, V_dy, V_st):
   """2 * MAC over the coarse pass (S_coarse samples) and, when S_fine > 0, the
   fine pass (S_fine = N_samples + N_importance samples)."""
