@@ -161,13 +161,18 @@ __global__ void aa_w_bwd_kernel(const float* __restrict__ ray_diff, const float*
     const float den = sum + 1e-8f;
     float dot = 0.f;
     for (int v = 0; v < V; ++v) dot += dw[p * V + v] * ((e[v] - emin) * meff[p * V + v] / den);
-    float de_min = 0.f, acc = 0.f;
+    // d|s| = sum_v de_v (g_v - g_min), g_v = de_v/d|s| = e_v (cos_v - 1), the min's share folded in view by view.
+    // Summing de_v g_v and the min's -sum_v de_v g_min separately cancels terms of size |dw| / den, and den = 1e-8
+    // at a point whose valid views are all the argmin (every u = 0, where the exact contribution is 0); an FMA
+    // contraction of that cancellation leaves a product's rounding error 1e8 times amplified.  The argmin's own
+    // term is skipped and the g are rounded products (__fmul_rn: no contraction), so such a point adds exactly 0.
+    const float gmin = __fmul_rn(e[amin], ray_diff[(p * V + amin) * 4 + 3] - 1.f);
+    float acc = 0.f;
     for (int v = 0; v < V; ++v) {
+      if (v == amin) continue;
       const float de = (dw[p * V + v] - dot) / den * meff[p * V + v];
-      de_min -= de;
-      acc += de * e[v] * (ray_diff[(p * V + v) * 4 + 3] - 1.f);
+      acc += de * (__fmul_rn(e[v], ray_diff[(p * V + v) * 4 + 3] - 1.f) - gmin);
     }
-    acc += de_min * e[amin] * (ray_diff[(p * V + amin) * 4 + 3] - 1.f);
     const float sv = *s_param;
     contrib = sv > 0.f ? acc : (sv < 0.f ? -acc : 0.f);  // d|s|/ds, 0 at s = 0 like torch.abs
   }
