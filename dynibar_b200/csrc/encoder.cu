@@ -17,9 +17,13 @@ namespace dyn {
 namespace {
 
 __device__ __forceinline__ int reflect_idx(int i, int n) {
-  // torch 'reflect' padding: -1 -> 1, n -> n - 2 (pads here are < n)
+  // torch 'reflect' padding: -1 -> 1, n -> n - 2 (pads here are < n).  The tile loaders of the forward convolutions
+  // stage the input window of a whole 8 x 16 output tile; on images smaller than a tile (H <= 17 or W <= 33) its rows
+  // and columns past the image reach i >= 2n - 1, which reflects to a negative index.  Those values feed only
+  // outputs that are never stored; the clamp keeps their loads inside the image.
   i = i < 0 ? -i : i;
-  return i >= n ? 2 * n - 2 - i : i;
+  i = i >= n ? 2 * n - 2 - i : i;
+  return min(max(i, 0), n - 1);
 }
 
 // ---------------------------------------------------------------------------
