@@ -833,7 +833,8 @@ int dyn_flow_sceneflow(const float* weights, const float* pts_seq, const float* 
                        int frame_idx, int sf_k, int n_flow, int R, int S, float* flows,
                        float* exp_sf, void* stream) {
   if (R == 0) return DYN_OK;  // empty batch: nothing to do (pointers may be null)
-  DYN_CHECK_ARG(weights && pts_seq && src_cams && uv && flows);
+  // n_flow == 0 (no source views): no flows, and pts_seq / src_cams / flows may be empty
+  DYN_CHECK_ARG(weights && uv && (n_flow == 0 || (pts_seq && src_cams && flows)));
   DYN_CHECK_ARG(n_flow >= 0 && n_flow <= kMaxViews && nb >= 1 && nb <= 8);
   if (R == 0) return DYN_OK;
   cudaStream_t st = (cudaStream_t)stream;
@@ -863,7 +864,11 @@ int dyn_flow_sceneflow(const float* weights, const float* pts_seq, const float* 
 
 int dyn_flow_backward(const float* weights, const float* pts_seq, const float* src_cams, const float* g_flows,
                       int n_flow, int R, int S, float* g_weights, float* g_pts_seq, void* stream) {
-  if (R == 0 || n_flow == 0) return DYN_OK;
+  if (R == 0) return DYN_OK;
+  if (n_flow == 0) {  // no flows: the weights get a zero gradient (g_pts_seq is empty)
+    if (g_weights) DYN_CUDA(cudaMemsetAsync(g_weights, 0, (size_t)R * S * sizeof(float), (cudaStream_t)stream));
+    return DYN_OK;
+  }
   DYN_CHECK_ARG(weights && pts_seq && src_cams && g_flows && (g_weights || g_pts_seq));
   DYN_CHECK_ARG(n_flow >= 1 && n_flow <= kMaxViews && S >= 1 && S <= 256);
   cudaStream_t st = (cudaStream_t)stream;

@@ -278,7 +278,8 @@ int dyn_encoder_backward(const float* params, size_t n_params, const float* imag
 /* ---- a14: flow / expected scene flow, render_ray.py:333-358, :585-595 -----
  * weights [R,S]; pts_seq [V,R,S,3] (first n_flow views used); src_cams
  * [V,34]; uv [R,2]; coeff [R,S,3*nb]; basis [T,nb]; sf_k = 2 (mv) or 1 (mono).
- * flows [n_flow,R,2]; exp_sf [R,3]. */
+ * flows [n_flow,R,2]; exp_sf [R,3].  With n_flow == 0, pts_seq, src_cams and
+ * flows may be NULL. */
 int dyn_flow_sceneflow(const float* weights, const float* pts_seq,
                        const float* src_cams, const float* uv,
                        const float* coeff, const float* basis, int T, int nb,
@@ -349,7 +350,7 @@ int dyn_net_static_backward(dyn_net_t net, const float* rgb_feat, const float* r
  *   (DEVICE; rows = differences of DCT basis rows), coeff [P,3*nb], base [P,3] or NULL, out [n,P,3].  The backward
  *   writes g_coeff [P,3*nb] and / or g_base [P,3] (either may be NULL).
  * dyn_flow_backward: compute_optical_flow (render_ray.py:333-358) -> g_weights [R,S], g_pts_seq [n_flow,R,S,3]
- *   (either may be NULL).  S <= 256. */
+ *   (either may be NULL).  S <= 256.  n_flow == 0 writes a zero g_weights. */
 int dyn_composite_vanilla_backward(const float* raw, const float* z_vals, const float* g_rays,
                                    const float* g_samples, int R, int S, float* g_raw, void* stream);
 int dyn_traj_combine(const float* coeff, const float* D, const float* base, int n, int nb, int P, float* out,
