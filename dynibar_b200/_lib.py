@@ -142,6 +142,12 @@ SIGNATURES = {
     "dyn_encoder_backward": (_i, [_vp, _sz, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp, _i, _vp]),
     "dyn_flow_sceneflow": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i,
                                 _vp, _vp, _vp]),
+    "dyn_splat_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dyn_splat_softmax": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "dyn_forward_splat": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "dyn_sobel_alpha": (_i, [_vp, _i, _i, _i, _f, _vp, _vp]),
+    "dyn_virtual_views_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dyn_virtual_views": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

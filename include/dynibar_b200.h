@@ -568,6 +568,34 @@ int dyn_linear_tc(const float* X, int ldx, const float* W, const float* b, int M
                   int N, int K, int act, float* Y, int ldy, void* packed_ws,
                   size_t packed_ws_bytes, void* stream);
 
+/* ---- virtual source views of a monocular frame (render_source_vv.py; offline data preparation) --------------
+ * Deterministic softmax forward splatting: every source pixel adds value * bilinear weight to the four target pixels
+ * around (x + flow_x, y + flow_y) (NW corner floor(.), a corner outside the image is dropped on its own), and the
+ * output is sum(value e w) / (sum(e w) + 1e-7) with e = exp(metric).  No float atomics: sources are grouped by cell
+ * with a stable sort and summed in a fixed order, so the same inputs give the same bits.  B items, C channels. */
+/* workspace of dyn_splat_softmax / dyn_forward_splat for B items of H x W; 0 for an unsupported shape */
+size_t dyn_splat_workspace_bytes(int B, int H, int W);
+/* splatting_function('softmax', frame, flow, metric) (the external `splatting` extension, render_source_vv.py:58):
+ * frame [B,C,H,W], flow [B,2,H,W], metric [B,1,H,W] -> out [B,C,H,W].  C <= 8. */
+int dyn_splat_softmax(const float* frame, const float* flow, const float* metric, int B, int C, int H, int W,
+                      float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* render_forward_splat (render_source_vv.py:15): imgs [B,H,W,C], depths [B,H,W], cams [B,30] = K_src^-1 | R | t |
+ * K_dst (row-major, fp32).  Each pixel goes to p = K_dst (R (d K_src^-1 [x,y,1]^T) + t), weighted by
+ * exp((imp - min) / (max - min + 1e-6) * 20 - 10), imp = 1 / p_z, min / max per item.
+ * out [B,C+1,H,W] = splatted image channels | splatted 1 / p_z.  C <= 7. */
+int dyn_forward_splat(const float* imgs, const float* depths, const float* cams, int B, int C, int H, int W, float* out,
+                      void* workspace, size_t workspace_bytes, void* stream);
+/* sobel_fg_alpha (render_source_vv.py:118): x [N,H,W] -> alpha [N,H,W] = exp(-beta sqrt(gx^2 + gy^2)), unnormalised
+ * 3x3 Sobel with the border replicated. */
+int dyn_sobel_alpha(const float* x, int N, int H, int W, float beta, float* alpha, void* stream);
+/* One frame's V virtual source views (render_source_vv.py:283-330): img [H,W,3] in [0,1], disp [H,W], cams [V,30]
+ * (as dyn_forward_splat, K_src = K_dst) -> out [V,H,W,3] uint8.  rgba = [img * 255, sobel alpha of (1/disp)/10 with
+ * beta 0.5] is splatted from depth 1/disp; rgb = clip(F_rgb / 255, 0, 1), mask = F_a > 0.5 eroded by the 3x3 cross
+ * (edge replicated), out = uint8(255 rgb mask), truncating. */
+size_t dyn_virtual_views_workspace_bytes(int V, int H, int W);
+int dyn_virtual_views(const float* img, const float* disp, const float* cams, int V, int H, int W, uint8_t* out,
+                      void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
