@@ -52,6 +52,8 @@ int motion_train_backward(const dyn_net* n, const float* xyzt, const float* d_co
                           size_t ws_bytes, float* d_params, float* d_xyzt, int prec, cudaStream_t st);
 
 // training backward of the two aggregation nets (nets_train.cu); the forward is net_*_f32(..., train = true)
+// DYN_OK when the attention backward can run S samples per ray, else DYN_E_INVALID naming its limit
+int check_attention_backward(int S);
 size_t net_train_workspace(int kind, int R, int S, int V);
 size_t net_backward_scratch(int kind, int R, int S, int V);
 int net_dynamic_backward(const dyn_net* n, const float* pts, const float* rgb_feat, const float* ray_dir,

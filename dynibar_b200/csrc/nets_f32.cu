@@ -672,6 +672,7 @@ int net_dynamic_f32(const dyn_net* n, const float* pts, const float* rgb_feat, c
                     size_t ws_bytes, int prec, cudaStream_t st, bool train) {
   const DynamicLayout& L = n->dl;
   RUN(check_attention_samples(S, false));
+  if (train) RUN(check_attention_backward(S));
   const int RC = net_rows_per_chunk(S, V);
   if (train && R_all > RC) return fail(DYN_E_INVALID, "training forward: %d rays exceed one internal chunk (%d)", R_all, RC);
   for (int r0 = 0; r0 < R_all; r0 += RC) {
@@ -727,6 +728,7 @@ int net_static_f32(const dyn_net* n, const float* pts, const float* ref_rays, co
                    int V, float* raw, void* ws, size_t ws_bytes, int prec, cudaStream_t st, bool train) {
   const StaticLayout& L = n->sl;
   RUN(check_attention_samples(S, false));
+  if (train) RUN(check_attention_backward(S));
   const int RC = net_rows_per_chunk(S, V);
   if (train && R_all > RC) return fail(DYN_E_INVALID, "training forward: %d rays exceed one internal chunk (%d)", R_all, RC);
   for (int r0 = 0; r0 < R_all; r0 += RC) {

@@ -279,10 +279,11 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ a
 // QUERY-row mask (rows with <= 1 valid views attend uniformly and pass no gradient to q / k).  One block per
 // (ray, head); phase A: a thread per query row (row statistics, D_i = sum_j p_ij dP_ij, dQ_i); phase B: a thread
 // per key row (dK_j, dV_j).  Q, K, V, dO, dQ, dK, dV are [P,128] rows; the head owns columns 32 h .. 32 h + 31.
-__global__ void attention_bwd_kernel(const float* __restrict__ Q, const float* __restrict__ K,
-                                     const float* __restrict__ Vv, const float* __restrict__ dO,
-                                     const float* __restrict__ nvalid, int S, float* __restrict__ dQ,
-                                     float* __restrict__ dK, float* __restrict__ dV) {
+// Shared memory: (4 S 33 + 4 S) floats.
+__device__ __forceinline__ void attention_bwd_body(const float* __restrict__ Q, const float* __restrict__ K,
+                                                   const float* __restrict__ Vv, const float* __restrict__ dO,
+                                                   const float* __restrict__ nvalid, int S, float* __restrict__ dQ,
+                                                   float* __restrict__ dK, float* __restrict__ dV) {
   extern __shared__ __align__(16) float sm[];
   float* Qs = sm;               // [S][33] (scaled by 1/sqrt(32)); padded rows: conflict-free per-thread rows
   float* Ks = Qs + S * 33;
@@ -379,6 +380,54 @@ __global__ void attention_bwd_kernel(const float* __restrict__ Q, const float* _
       dV[(base + j) * 128 + h * 32 + d] = dv[d];
     }
   }
+}
+
+// Unbounded instance: its register count (about 210) limits a block to 288 threads, so it runs S <= 288.
+__global__ void attention_bwd_kernel(const float* __restrict__ Q, const float* __restrict__ K,
+                                     const float* __restrict__ Vv, const float* __restrict__ dO,
+                                     const float* __restrict__ nvalid, int S, float* __restrict__ dQ,
+                                     float* __restrict__ dK, float* __restrict__ dV) {
+  attention_bwd_body(Q, K, Vv, dO, nvalid, S, dQ, dK, dV);
+}
+
+// The same body bounded to kAttnBwdMaxS threads (at most 168 registers, the rest spills to local memory), for the
+// sample counts above the unbounded instance's block limit.
+constexpr int kAttnBwdMaxS = 384;
+__global__ void __launch_bounds__(kAttnBwdMaxS) attention_bwd_wide_kernel(
+    const float* __restrict__ Q, const float* __restrict__ K, const float* __restrict__ Vv,
+    const float* __restrict__ dO, const float* __restrict__ nvalid, int S, float* __restrict__ dQ,
+    float* __restrict__ dK, float* __restrict__ dV) {
+  attention_bwd_body(Q, K, Vv, dO, nvalid, S, dQ, dK, dV);
+}
+
+static size_t attention_bwd_smem(int S) { return (size_t)(4 * S * 33 + 4 * S) * sizeof(float); }
+
+// Which attention-backward instance runs S samples per ray: the unbounded kernel while S fits its block limit,
+// the bounded one up to kAttnBwdMaxS; limits queried once per process.  *wide = -1: S is not supported (the
+// error is set).
+static int attention_bwd_select(int S, int* wide) {
+  static int max_plain = 0, max_wide = 0, smem_optin = 0;
+  *wide = -1;
+  if (max_plain == 0) {
+    cudaFuncAttributes fa;
+    DYN_CUDA(cudaFuncGetAttributes(&fa, attention_bwd_kernel));
+    const int plain = fa.maxThreadsPerBlock;
+    DYN_CUDA(cudaFuncGetAttributes(&fa, attention_bwd_wide_kernel));
+    const int wide_threads = fa.maxThreadsPerBlock;
+    int dev = 0, optin = 0;
+    DYN_CUDA(cudaGetDevice(&dev));
+    DYN_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    max_wide = wide_threads;
+    smem_optin = optin;
+    max_plain = plain;
+  }
+  const int by_threads = max_wide > max_plain ? max_wide : max_plain;  // a multiple of 32
+  const int by_smem = smem_optin / (int)attention_bwd_smem(1);
+  const int limit = by_threads < by_smem ? by_threads : by_smem;
+  if (S > limit)
+    return fail(DYN_E_INVALID, "training: the attention backward supports S <= %d samples per ray (got %d)", limit, S);
+  *wide = ((S + 31) / 32) * 32 > max_plain ? 1 : 0;
+  return DYN_OK;
 }
 
 // PeriodicEmbed backward for 3 inputs with frequencies 2^k, k < n (layout of pe_kernel): dpe rows have `ld` floats
@@ -632,12 +681,14 @@ int trunk_backward(const dyn_net* n, const Layout& L, const Prod& pr, const Trun
   TR(pr.grad_w(q.pB, 128, 128, P, t.O, 128, 128, dprm + L.fc.w, 128));
   TR(pr.grad_in(q.pB, 128, 128, P, prm + L.fc.w, 128, 128, q.pA, 128));  // q.pA = dO
   {
+    int wide;
+    TR(attention_bwd_select(S, &wide));
     const int threads = ((S + 31) / 32) * 32;
-    const size_t smem = (size_t)(4 * S * 33 + 4 * S) * sizeof(float);
-    if (threads > 1024 || smem > 200 * 1024) return fail(DYN_E_INVALID, "attention backward supports S <= 384 (got %d)", S);
+    const size_t smem = attention_bwd_smem(S);
+    auto kernel = wide ? attention_bwd_wide_kernel : attention_bwd_kernel;
     if (smem > 48 * 1024)
-      DYN_CUDA(cudaFuncSetAttribute(attention_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attention_bwd_kernel<<<R * 4, threads, smem, st>>>(t.Q, t.K, t.V, q.pA, t.nvalid, S, q.pC, q.pD, q.pE);
+      DYN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<R * 4, threads, smem, st>>>(t.Q, t.K, t.V, q.pA, t.nvalid, S, q.pC, q.pD, q.pE);
     DYN_LAUNCH_CHECK();
   }
   // q/k/v projections of G2 (no bias): dG2 = d(resid) + dQ Wq + dK Wk + dV Wv   (accumulated into q.pB)
@@ -704,6 +755,12 @@ int trunk_backward(const dyn_net* n, const Layout& L, const Prod& pr, const Trun
 }
 
 }  // namespace
+
+// The training forward calls this at entry, so that no forward work is done for an S its backward cannot run.
+int check_attention_backward(int S) {
+  int wide;
+  return attention_bwd_select(S, &wide);
+}
 
 size_t net_train_workspace(int kind, int R, int S, int V) {
   Bump b{nullptr, 0};

@@ -15,7 +15,12 @@ mode="kernel" rounds where precision "bf16" rounds, and nowhere else: a product 
 cores multiplies round-to-nearest bf16 copies of both operands (the row-scaled input X rs, the weight, dZ) and
 accumulates exactly; every other product, and all the glue, is exact.  The bias is added after the product.
 
-`plant` names a deliberate wiring error (PLANTS) used to show that the bars of the GPU test would catch it.
+`plant` names a deliberate wiring error (PLANTS, FWD_PLANTS) used to show that the bars of the GPU tests would
+catch it.
+
+The same functions state the inference forward (net_*_f32 with `train = false`): its arithmetic is the training
+forward's, only its buffers differ (X2 and H3 updated in place, the rays split into internal chunks).
+make_forward_case / forward serve that comparison (tests/test_staged_nets_gpu.py).
 """
 
 import math
@@ -235,12 +240,14 @@ def _pool(x, wgt):
   return torch.cat([mean[:, 0], var], -1)
 
 
-def _attention(Q, K, Vv, valid, R, S):
+def _attention(Q, K, Vv, valid, R, S, plant=None):
   """Ray-transformer attention (oracle ray_attention without its projections): query rows with valid == 0
   attend uniformly (mlp_network.py:23-24)."""
   sh = lambda t: t.view(R, S, 4, 32).transpose(1, 2)
   att = (sh(Q) / math.sqrt(32.0)) @ sh(K).transpose(2, 3)
   att = att.masked_fill(valid.view(R, 1, S, 1) == 0, -1e9)
+  if plant == "keys_first256":
+    att[..., 256:] = -math.inf
   return (torch.softmax(att, -1) @ sh(Vv)).transpose(1, 2).reshape(R * S, 128)
 
 
@@ -256,9 +263,11 @@ def _trunk(n, mv, C, feat, w1, mask, P, V, R, S, posenc):
   X2 = X + XV[:, :128]
   H3 = n.lin("vis_fc2.0", [(X2, 1)], "elu", rs=vis1, P=P)
   vis2 = n.lin("vis_fc2.2", [(H3, 1)], "sigmoid", P=P)[:, 0] * m
-  vp = vis2.view(P, V)
+  vp, Xp = vis2.view(P, V), X2.view(P, V, 128)
+  if n.plant == "pool2_first16":
+    vp, Xp = vp[:, :16], Xp[:, :16]
   w2 = vp / (vp.sum(1, keepdim=True) + 1e-8)
-  G = torch.cat([_pool(X2.view(P, V, 128), w2), w2.mean(1, keepdim=True)], -1)  # [P,257]
+  G = torch.cat([_pool(Xp, w2), w2.mean(1, keepdim=True)], -1)  # [P,257]
   GH = n.lin("geometry_fc.0", [(G, 1)], "elu")
   G2 = n.lin("geometry_fc.2", [(GH, 1)], "elu")
   if posenc:
@@ -267,7 +276,7 @@ def _trunk(n, mv, C, feat, w1, mask, P, V, R, S, posenc):
   Q = n.lin("ray_attention.w_qs", [(G2, 1)], "none", acc_in=True)
   K = n.lin("ray_attention.w_ks", [(G2, 1)], "none", acc_in=True)
   Vv = n.lin("ray_attention.w_vs", [(G2, 1)], "none", acc_in=True)
-  Oa = _attention(Q, K, Vv, (nvalid > 1).to(G2.dtype), R, S)
+  Oa = _attention(Q, K, Vv, (nvalid > 1).to(G2.dtype), R, S, n.plant)
   O2 = n.lin("ray_attention.fc", [(Oa, 1)], "none")
   G3 = F.layer_norm(O2 + G2, (128,), n.w["ray_attention.layer_norm.weight"], n.w["ray_attention.layer_norm.bias"],
                     eps=1e-6)
@@ -337,6 +346,9 @@ def net_static(w, pts, ref_rays, src_rays, rgb_feat, ray_diff, mask, anti_alias=
   logit = n.lin("rgb_fc.4", [(ch2, 1)], "none", P=P)[:, 0].view(P, V)
   blend = torch.softmax(logit.masked_fill(mk == 0, -1e9), 1)
   rgb = (blend[..., None] * rf[:, :3].view(P, V, 3)).sum(1)
+  if plant == "blend_first16":
+    b16 = torch.softmax(logit.masked_fill(mk == 0, -1e9)[:, :16], 1)
+    rgb = (b16[..., None] * rf[:, :3].view(P, V, 3)[:, :16]).sum(1)
   sig = sig.masked_fill(nvalid < 1, -1e9)
   return torch.cat([rgb, sig[:, None]], -1).view(R, S, 4)
 
@@ -754,3 +766,106 @@ def ratios(kind, prec, got, ref, V=None):
   """Per tensor: the larger of its relative L2 error and its max-abs ratio, each over its bar."""
   return {k: max(r / bar(kind, prec, k)[0], m / bar(kind, prec, k)[1])
           for k, (r, m) in errors(kind, got, ref, V).items()}
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The inference forward (render_ray.net_dynamic_forward / net_static_forward): tests/test_staged_nets_gpu.py
+# ---------------------------------------------------------------------------------------------------------------
+# Planted errors of the inference forward (tests/test_staged_nets_reference_cpu.py).
+FWD_PLANTS = (
+    "pool2_first16",   # the second pooling (pool2_kernel) over the first 16 views only
+    "keys_first256",   # the attention keys past the first 256 samples of a ray left out of its softmax
+    "rays_chunk0",     # ray_dir / ref_rays of every internal chunk read from chunk 0 (the ray offset r0 dropped)
+    "blend_first16",   # the static blending softmax (st_out_kernel) over the first 16 views only
+)
+
+HOT = 4.0  # weight scale of a "hot" case: pre-activations of several units, ELUs saturate at -1, sigmoids at 0 / 1
+
+
+def make_forward_case(kind, R, S, V, aa=False, mrgb=False, hot=False, s_zero=False, seed=0, device="cpu"):
+  """Seeded module (CPU, fp32) and inputs (fp32, on `device`) of one inference case, built like make_net_case.
+  Points 0, 1 and 2 (flat over R S) see no view, only view 0 (a masked query row of the attention) and every view.
+  mrgb: about 10 % of the source colours are exactly black, which mask_rgb masks out.  hot: every weight matrix
+  but the LayerNorm's scaled by HOT.  s_zero: the anti-aliased pooling's s = 0, so that every view of a point has
+  the same e_v and the pooling weights (e_v - min e) m_v are all 0."""
+  from dynibar_b200 import mlp_network as nets, synthetic
+  torch.manual_seed(seed)
+  args = synthetic.make_args(int(aa), int(mrgb))
+  if kind == "dynamic":
+    mod = nets.DynibarDynamic(args, 32, S, shift=5.0)
+  else:
+    mod = nets.DynibarStatic(args, 32, S)
+  with torch.no_grad():
+    mod.out_geometry_fc[2].bias.fill_(1.0 if kind == "dynamic" else 0.5)
+    if hot:
+      for name, p in mod.named_parameters():
+        if name.endswith(".weight") and "layer_norm" not in name:
+          p.mul_(HOT)
+    if s_zero:
+      mod.s.zero_()
+  g = torch.Generator(device=device).manual_seed(seed + 1)
+  rn = lambda *shape: torch.randn(*shape, generator=g, device=device)
+  ru = lambda *shape: torch.rand(*shape, generator=g, device=device)
+  c = dict(kind=kind, aa=aa, mrgb=mrgb, mod=mod)
+  c["pts"] = rn(R, S, 3) * 2
+  feat = rn(R, S, V, 35)
+  feat[..., :3] = ru(R, S, V, 3)
+  if mrgb:
+    feat[..., :3].masked_fill_(ru(R, S, V, 1) < 0.1, 0.0)
+  mask = (ru(R, S, V, 1) > 0.3).float()
+  mp = mask.view(R * S, V)
+  mp[0] = 0.0
+  mp[1] = 0.0
+  mp[1, 0] = 1.0
+  mp[2] = 1.0
+  c["feat"], c["mask"] = feat, mask
+  c["ray_dir"] = F.normalize(rn(R, 3), dim=-1)
+  c["t"] = float(torch.tensor(0.4, dtype=torch.float32))
+  c["ref_rays"] = rn(R, 6)
+  c["src_rays"] = rn(R, S, V, 6)
+  c["ray_diff"] = torch.cat([F.normalize(rn(R, S, V, 3), dim=-1), ru(R, S, V, 1) * 0.3 + 0.7], -1)
+  return c
+
+
+def forward(c, device, mode, lo=0, hi=None, plant=None, rays_per_chunk=None, dtype=torch.float64):
+  """raw [hi - lo, S, 4] (float64) of rays [lo, hi) of case `c`, evaluated on `device` as one call.  plant
+  "rays_chunk0" reads ray_dir / ref_rays of ray r at r mod rays_per_chunk.  dtype=torch.float32 evaluates the same
+  arithmetic in float32 (see reference)."""
+  hi = c["feat"].shape[0] if hi is None else hi
+  d = lambda x: x[lo:hi].to(device, dtype, copy=True)
+  rays = torch.arange(lo, hi)
+  if plant == "rays_chunk0":
+    rays = rays % rays_per_chunk
+  per_ray = lambda x: x[rays.to(x.device)].to(device, dtype)
+  w = {k: p.detach().to(device, dtype, copy=True) for k, p in c["mod"].named_parameters()}
+  with torch.no_grad():
+    if c["kind"] == "dynamic":
+      return net_dynamic(w, d(c["pts"]), d(c["feat"]), per_ray(c["ray_dir"]), d(c["mask"]), c["t"],
+                         float(c["mod"].shift), mode, plant)
+    return net_static(w, d(c["pts"]), per_ray(c["ref_rays"]), d(c["src_rays"]), d(c["feat"]), d(c["ray_diff"]),
+                      d(c["mask"]), c["aa"], c["mrgb"], mode, plant)
+
+
+# Bars of raw in the inference comparison, per (net, precision): (relative L2 error, max |error| / max |reference|)
+# over the entries that are not the -1e9 sentinel.  The cases with ordinary weights stay within the training
+# comparison's bars of raw (BARS); the hot cases have their own.  How they were set is in
+# tests/test_staged_nets_gpu.py; the comment beside each hot bar records the measured worst and its case.
+FWD_BARS = {
+    ("dynamic", "bf16"): BARS[("dynamic", "bf16")]["out"],
+    ("dynamic", "fp32"): BARS[("dynamic", "fp32")]["out"],
+    ("static", "bf16"): BARS[("static", "bf16")]["out"],
+    ("static", "fp32"): BARS[("static", "fp32")]["out"],
+}
+FWD_HOT_BARS = {
+    ("dynamic", "bf16"): (3e-03, 2e-02),  # 1.47e-03 5.03e-03 s193
+    ("dynamic", "fp32"): (5e-05, 3e-04),  # 2.11e-05 1.46e-04 s193
+    ("static", "bf16"): (2e-01, 6e-01),  # 5.60e-02 2.87e-01 s193
+    ("static", "fp32"): (4e-05, 5e-05),  # 1.51e-05 2.39e-05 v24
+}
+
+
+def fwd_ratio(kind, prec, got, ref, hot=False):
+  """The larger of raw's relative L2 error and max-abs ratio, each over its bar (inf when a sentinel differs)."""
+  rel, mx = errors(kind, {"out": got}, {"out": ref})["out"]
+  b = (FWD_HOT_BARS if hot else FWD_BARS)[(kind, prec)]
+  return max(rel / b[0], mx / b[1]), (rel, mx)
