@@ -21,6 +21,7 @@ if not os.path.exists(LIB_PATH):
 lib = C.CDLL(LIB_PATH)
 
 PREC_FP32, PREC_BF16 = 0, 1
+SCORES_PLAIN, SCORES_EVAL = 0, 1
 NET_DYNAMIC, NET_STATIC, NET_MOTION = 0, 1, 2
 
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
@@ -148,6 +149,8 @@ SIGNATURES = {
     "dyn_sobel_alpha": (_i, [_vp, _i, _i, _i, _f, _vp, _vp]),
     "dyn_virtual_views_workspace_bytes": (_sz, [_i, _i, _i]),
     "dyn_virtual_views": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "dyn_image_scores_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dyn_image_scores": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -596,6 +596,25 @@ size_t dyn_virtual_views_workspace_bytes(int V, int H, int W);
 int dyn_virtual_views(const float* img, const float* disp, const float* cams, int V, int H, int W, uint8_t* out,
                       void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- scores of rendered views (eval_nvidia.py:201-247, :380-457; DESIGN §3.6) ---------------------------------------
+ * pred, gt (and mask) [K,H,W,3] fp32, channels-last, contiguous; H, W >= 7.  SSIM is skimage 0.19.3
+ * structural_similarity(multichannel=True, full=True) on float32: 7x7 uniform window, 'reflect' border, sample
+ * covariance, data_range 2.  For each mask row m: den = sum(w_m) + 1e-8 over all H*W*3 elements,
+ * PSNR = 10 log10(den / sum((pred - gt)^2 w_m)) in fp64 (0 when that sum is 0), SSIM = sum(S w_m) / den.
+ * scores [K,M,2] fp64 = (PSNR, SSIM) per image and row.
+ *   DYN_SCORES_PLAIN  M = 1: the given images, w_0 = mask (1 where mask is NULL).
+ *   DYN_SCORES_EVAL   eval_nvidia.py's scoring of a camera: valid = ((r + g) + b) > 1e-3f on pred (float32), both
+ *                     images multiplied by valid, rows w = valid, mask, 1 - mask (M = 3), or valid alone (M = 1) when
+ *                     mask is NULL.
+ * ssim_map [K,H,W,3] fp32 receives S when not NULL.  Two launches, no float atomics: the same inputs give the same
+ * bits, and an image's scores do not depend on K or the other images. */
+#define DYN_SCORES_PLAIN 0
+#define DYN_SCORES_EVAL 1
+/* workspace of dyn_image_scores for K images of H x W; 0 for an unsupported shape */
+size_t dyn_image_scores_workspace_bytes(int K, int H, int W);
+int dyn_image_scores(const float* pred, const float* gt, const float* mask, int K, int H, int W, int mode,
+                     double* scores, float* ssim_map, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
