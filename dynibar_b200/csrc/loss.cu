@@ -23,6 +23,7 @@ enum Term { T_RGB0 = 0, T_STATIC = 5, T_DISP = 6, T_FLOW = 7, T_CYCLE = 8, T_REG
 constexpr int kAcc = 2 * kTerms;  // numerator 2k, denominator 2k + 1 of term k
 constexpr int kWarps = 8;         // rays per block
 constexpr int kOutComp = 9, kOutScale = 9 + kTerms;  // offsets in `out`, after the nine logged scalars
+constexpr int kMaxDistSamples = 256;  // dist_n limit of the distortion term
 
 struct Dims { int R, S, K, n_sf; };
 
@@ -439,9 +440,11 @@ int check_inputs(const dyn_mono_loss_inputs& in, const dyn_mono_loss_weights& wt
   DYN_CHECK_ARG(!has(T_CYCLE) || (in.traj_ref != nullptr && in.traj_anchor != nullptr &&
                                   in.occ_weights != nullptr && in.K > 0));
   DYN_CHECK_ARG(!(has(T_REG_ABS) || has(T_REG_TIME) || has(T_REG_SPACE)) || (in.sf_seq != nullptr && in.n_sf >= 2));
-  DYN_CHECK_ARG(!has(T_DIST) || (in.dist_w != nullptr && in.dist_n > 0 && in.dist_n <= 256 &&
-                                 in.dist_ld >= in.dist_n &&
+  DYN_CHECK_ARG(!has(T_DIST) || (in.dist_w != nullptr && in.dist_n > 0 && in.dist_ld >= in.dist_n &&
                                  (in.s_vals != nullptr || (in.dist_m != nullptr && in.dist_interval != nullptr))));
+  if (has(T_DIST) && in.dist_n > kMaxDistSamples)
+    return fail(DYN_E_INVALID, "dyn_mono_loss: the distortion term supports at most %d samples per ray, got %d",
+                kMaxDistSamples, in.dist_n);
   return DYN_OK;
 }
 

@@ -105,15 +105,16 @@ def ulp32(x):
   return torch.where(x == 0, torch.full_like(x, 2.0 ** -149), torch.ldexp(torch.ones_like(x), (e - 24).clamp(min=-149)))
 
 
-def bar(name, ref, mag, sens, ulps=None):
-  atol, u = TOL[name]
+def bar(name, ref, mag, sens, ulps=None, tol=TOL):
+  """atol + ulps (ulp(ref) + 2^-24 mag) + sens, with (atol, ulps) = tol[name]."""
+  atol, u = tol[name]
   u = u if ulps is None else ulps
   return atol + u * (ulp32(ref) + EPS * mag) + sens
 
 
-def excess(name, got, ref, mag, sens):
-  """(err - atol - sens) / (ulp + 2^-24 mag): the measured quantity behind TOL[name]'s ulps."""
-  atol, _ = TOL[name]
+def excess(name, got, ref, mag, sens, tol=TOL):
+  """(err - atol - sens) / (ulp + 2^-24 mag): the measured quantity behind tol[name]'s ulps."""
+  atol, _ = tol[name]
   return ((d64(got) - ref).abs() - atol - sens) / (ulp32(ref) + EPS * mag)
 
 
