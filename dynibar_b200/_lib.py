@@ -79,10 +79,12 @@ SIGNATURES = {
                                 _vp, _vp, _vp, _vp, _vp]),
     "dyn_project_gather_mc": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
                                    _vp, _vp, _vp, _vp, _vp]),
+    "dyn_project_gather_tbl": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp] + [_i] * 8 + [_vp] * 5),
     "dyn_compute_projections": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "dyn_compute_angle": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     "dyn_plucker_ref": (_i, [_vp, _vp, _i, _vp, _vp]),
     "dyn_plucker_src": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "dyn_plucker_src_tbl": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "dyn_net_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "dyn_net_dynamic": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp, _vp, _sz, _i, _vp]),
     "dyn_net_static": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, _i, _vp]),
@@ -95,6 +97,9 @@ SIGNATURES = {
                                      _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "dyn_net_dynamic_fused": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _i,
                                    _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "dyn_net_static_fused_tbl": (_i, [_vp] * 5 + [_i, _vp, _vp, _i] + [_vp] * 3 + [_i] * 8 + [_vp] * 3 + [_sz, _vp]),
+    "dyn_net_dynamic_fused_tbl": (_i, [_vp] * 5 + [_i, _vp, _vp, _i] + [_vp] * 3 + [_f] + [_i] * 8 + [_vp] * 3
+                                  + [_sz, _vp]),
     "dyn_composite": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "dyn_composite_vanilla": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "dyn_resample": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
@@ -211,6 +216,12 @@ class Args(object):
     c = t.detach().to(torch.float32).contiguous()
     if c.is_cuda:
       c = c.cpu()
+    self.keep.append(c)
+    return c.data_ptr()
+
+  def host_i32(self, t):
+    """Small int32 tables (view tables): a HOST pointer, like `host`."""
+    c = t.detach().to(device="cpu", dtype=torch.int32).contiguous()
     self.keep.append(c)
     return c.data_ptr()
 

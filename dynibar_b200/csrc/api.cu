@@ -4,6 +4,7 @@
 
 #include <vector>
 
+#include "geometry.cuh"
 #include "linear_tc.cuh"
 #include "nets.cuh"
 #include "nets_fused.cuh"
@@ -264,7 +265,22 @@ int dyn_net_static_fused_mc(dyn_net_t net, const float* pts, const float* ray_o,
   DYN_CHECK_ARG(src_cams && feat_cl && raw && mask_out && workspace && C == kC);
   DYN_CHECK_ARG(R >= 0 && S >= 1 && V >= 1 && V <= 16);
   if (R == 0) return DYN_OK;
-  return net_static_fused(net, pts, ray_o, ray_d, query_cams, K, K > 1 ? query_idx : nullptr, src_rgbs, src_cams,
+  return net_static_fused(net, pts, ray_o, ray_d, query_cams, K, K > 1 ? query_idx : nullptr, nullptr, V, src_rgbs,
+                          src_cams, feat_cl, R, S, V, H, W, h, w, raw, mask_out, workspace, workspace_bytes,
+                          (cudaStream_t)stream);
+}
+
+int dyn_net_static_fused_tbl(dyn_net_t net, const float* pts, const float* ray_o, const float* ray_d,
+                             const float* query_cams, int K, const int* camera_index, const int* view_tbl, int pool,
+                             const float* src_rgbs, const float* src_cams, const void* feat_cl, int R, int S, int V,
+                             int H, int W, int C, int h, int w, float* raw, float* mask_out, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+  const int rc = check_tbl_args(K, camera_index, view_tbl, pool, V, 16);
+  if (rc) return rc;
+  if (R == 0) return DYN_OK;
+  DYN_CHECK_ARG(net && net->kind == DYN_NET_STATIC && pts && ray_o && ray_d && query_cams && src_rgbs);
+  DYN_CHECK_ARG(src_cams && feat_cl && raw && mask_out && workspace && C == kC && R >= 0 && S >= 1);
+  return net_static_fused(net, pts, ray_o, ray_d, query_cams, K, camera_index, view_tbl, pool, src_rgbs, src_cams,
                           feat_cl, R, S, V, H, W, h, w, raw, mask_out, workspace, workspace_bytes,
                           (cudaStream_t)stream);
 }
@@ -279,8 +295,24 @@ int dyn_net_dynamic_fused(dyn_net_t net, const float* pts, const float* pts_seq,
   DYN_CHECK_ARG(src_rgbs && src_cams && feat_cl && raw && mask_out && workspace && C == kC);
   DYN_CHECK_ARG(R >= 0 && S >= 1 && V >= 1 && V <= 16);
   if (R == 0) return DYN_OK;
-  return net_dynamic_fused(net, pts, pts_seq, ray_dir, query_cam, src_rgbs, src_cams, feat_cl, time, R, S,
-                           V, H, W, h, w, raw, mask_out, workspace, workspace_bytes, (cudaStream_t)stream);
+  return net_dynamic_fused(net, pts, pts_seq, ray_dir, query_cam, 1, nullptr, nullptr, V, src_rgbs, src_cams, feat_cl,
+                           time, R, S, V, H, W, h, w, raw, mask_out, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
+}
+
+int dyn_net_dynamic_fused_tbl(dyn_net_t net, const float* pts, const float* pts_seq, const float* ray_dir,
+                              const float* query_cam, int K, const int* camera_index, const int* view_tbl, int pool,
+                              const float* src_rgbs, const float* src_cams, const void* feat_cl, float time, int R,
+                              int S, int V, int H, int W, int C, int h, int w, float* raw, float* mask_out,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+  const int rc = check_tbl_args(K, camera_index, view_tbl, pool, V, 16);
+  if (rc) return rc;
+  if (R == 0) return DYN_OK;
+  DYN_CHECK_ARG(net && net->kind == DYN_NET_DYNAMIC && pts && pts_seq && ray_dir && query_cam);
+  DYN_CHECK_ARG(src_rgbs && src_cams && feat_cl && raw && mask_out && workspace && C == kC && R >= 0 && S >= 1);
+  return net_dynamic_fused(net, pts, pts_seq, ray_dir, query_cam, K, camera_index, view_tbl, pool, src_rgbs,
+                           src_cams, feat_cl, time, R, S, V, H, W, h, w, raw, mask_out, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
 }
 
 int dyn_debug_point_chain(dyn_net_t net, const float* G, const float* nvalid, const float* pts,

@@ -202,11 +202,14 @@ __global__ void rgb_to_rgba_kernel(const float* __restrict__ in, float4* __restr
 // with coalesced 16-byte stores.
 // Bilinear, zero padding, align_corners=True, coordinates normalised by the
 // SOURCE IMAGE size for both maps (projection.py:22-30, :143-158).
-// tgt_idx [R] (multi-camera launches, else null): ray r's target camera centre is cams.tgts[tgt_idx[r]].
+// tgt_idx [R] (multi-camera launches, else null): ray r's target camera is k = tgt_idx[r]; its centre is
+// cams.tgts[k], and its view slot v reads pool entry tbl.v[k][v] (camera, image and feature map).  Everything
+// indexed by slot (xyz, the outputs) stays as it is.
 __global__ void __launch_bounds__(256)
 project_gather_kernel(const float* __restrict__ xyz_st, const float* __restrict__ xyz,
                       const float* __restrict__ rgbs, const float* __restrict__ feat_cl,
-                      const __grid_constant__ ViewCams cams, const int* __restrict__ tgt_idx, int S, int V,
+                      const __grid_constant__ ViewCams cams, const __grid_constant__ ViewTable tbl,
+                      const int* __restrict__ tgt_idx, int S, int V,
                       long long N /* R*S */, int H, int W, int h, int w, float* __restrict__ rgb_feat,
                       float* __restrict__ ray_diff, float* __restrict__ mask) {
   // A block owns 256 consecutive (point, view) pairs.  Phase 1: every thread projects ONE pair (all lanes
@@ -225,8 +228,11 @@ project_gather_kernel(const float* __restrict__ xyz_st, const float* __restrict_
     const int t0 = (int)(pair0 - q0 * V) + (int)threadIdx.x;
     float gx = 0.f, gy = 0.f;
     const int v = t0 % V;
+    int vc = v;  // pool entry of slot v
     if (gid < total) {
       const long long pt = q0 + t0 / V;
+      const int k = tgt_idx != nullptr ? tgt_idx[pt / S] : 0;
+      vc = tbl.v[k][v];
       const float sx = xyz_st[pt * 3], sy = xyz_st[pt * 3 + 1], sz = xyz_st[pt * 3 + 2];
       float x = sx, y = sy, z = sz;
       if (xyz != nullptr) {
@@ -235,23 +241,23 @@ project_gather_kernel(const float* __restrict__ xyz_st, const float* __restrict_
       }
       float u, vv;
       bool front;
-      project_point(cams.P[v], x, y, z, u, vv, front);
+      project_point(cams.P[vc], x, y, z, u, vv, front);
       gx = 2.f * u / (cams.w_img - 1.f) - 1.f;
       gy = 2.f * vv / (cams.h_img - 1.f) - 1.f;
       const bool inb = (u <= cams.w_img - 1.f) && (u >= 0.f) && (vv <= cams.h_img - 1.f) && (vv >= 0.f);
       mask[gid] = (inb && front) ? 1.f : 0.f;
       // compute_angle, projection.py:61-101
-      const float* tgt = tgt_idx != nullptr ? cams.tgts[tgt_idx[pt / S]] : cams.tgt;
+      const float* tgt = tgt_idx != nullptr ? cams.tgts[k] : cams.tgt;
       float a0 = tgt[0] - sx, a1 = tgt[1] - sy, a2 = tgt[2] - sz;
       normalize3(a0, a1, a2);
-      float b0 = cams.center[v][0] - x, b1 = cams.center[v][1] - y, b2 = cams.center[v][2] - z;
+      float b0 = cams.center[vc][0] - x, b1 = cams.center[vc][1] - y, b2 = cams.center[vc][2] - z;
       normalize3(b0, b1, b2);
       float d0 = a0 - b0, d1 = a1 - b1, d2 = a2 - b2;
       const float dot = a0 * b0 + a1 * b1 + a2 * b2;
       normalize3(d0, d1, d2);
       reinterpret_cast<float4*>(ray_diff)[gid] = make_float4(d0, d1, d2, dot);
     }
-    s_gx[threadIdx.x] = gx; s_gy[threadIdx.x] = gy; s_v[threadIdx.x] = v;
+    s_gx[threadIdx.x] = gx; s_gy[threadIdx.x] = gy; s_v[threadIdx.x] = vc;
   }
   __syncthreads();
   const int lp = threadIdx.x >> 3;  // pair inside the round
@@ -355,13 +361,15 @@ __global__ void plucker_ref_kernel(const float* __restrict__ ray_o, const float*
   o[5] = ox * dy - oy * dx;
 }
 
+// tgt_idx / tbl: as in project_gather_kernel (slot v of ray r's camera k reads pool entry tbl.v[k][v])
 __global__ void plucker_src_kernel(const float* __restrict__ pts,
-                                   const __grid_constant__ ViewCams cams, int V, long long N,
+                                   const __grid_constant__ ViewCams cams, const __grid_constant__ ViewTable tbl,
+                                   const int* __restrict__ tgt_idx, int S, int V, long long N,
                                    float* __restrict__ out) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * V) return;
   long long pt = idx / V;
-  int v = (int)(idx % V);
+  const int v = tbl.v[tgt_idx != nullptr ? tgt_idx[pt / S] : 0][(int)(idx % V)];
   float ox = cams.center[v][0], oy = cams.center[v][1], oz = cams.center[v][2];
   float dx = pts[pt * 3] - ox, dy = pts[pt * 3 + 1] - oy, dz = pts[pt * 3 + 2] - oz;
   normalize3(dx, dy, dz);
@@ -575,6 +583,25 @@ int build_view_cams(const float* src_cams, int V, const float* query_cam, cudaSt
   return DYN_OK;
 }
 
+int build_view_table(const int* tbl, int K, int V, int pool, cudaStream_t st, ViewTable* out) {
+  DYN_CHECK_ARG(K >= 1 && K <= kMaxTargets && V >= 1 && V <= kMaxViews && pool >= 1 && pool <= kMaxViews);
+  for (int k = 0; k < kMaxTargets; ++k)
+    for (int s = 0; s < kMaxViews; ++s) out->v[k][s] = (uint8_t)s;
+  if (tbl == nullptr) return DYN_OK;
+  static thread_local int host[kMaxTargets * kMaxViews];
+  static_assert(sizeof(int) == sizeof(float), "fetch_small copies 4-byte words");
+  int rc = fetch_small(reinterpret_cast<const float*>(tbl), (size_t)K * V, reinterpret_cast<float*>(host), st);
+  if (rc) return rc;
+  for (int k = 0; k < K; ++k)
+    for (int s = 0; s < V; ++s) {
+      const int e = host[k * V + s];
+      if (e < 0 || e >= pool)
+        return fail(DYN_E_INVALID, "view table: camera %d slot %d names pool entry %d, the pool has %d", k, s, e, pool);
+      out->v[k][s] = (uint8_t)e;
+    }
+  return DYN_OK;
+}
+
 int launch_to_channels_last(const float* featmaps, float* out, int V, int C, int hw, cudaStream_t st) {
   dim3 tb(32, 8), tg(cdiv(hw, 32), cdiv(C, 32), V);
   to_channels_last_kernel<<<tg, tb, 0, st>>>(featmaps, out, C, hw);
@@ -613,6 +640,55 @@ int build_flow_cams(const float* src_cams, int V, cudaStream_t st, FlowCams* fc)
       fc->tw[v][i] = (float)w2c[i * 4 + 3];
     }
   }
+  return DYN_OK;
+}
+
+int check_tbl_args(int K, const int* camera_index, const int* view_tbl, int pool, int V, int max_slots) {
+  if (K < 1 || K > kMaxTargets) return fail(DYN_E_INVALID, "target camera count K = %d outside 1..%d", K, kMaxTargets);
+  if (K > 1 && camera_index == nullptr) return fail(DYN_E_INVALID, "K = %d target cameras need a per-ray camera index", K);
+  if (view_tbl == nullptr) return fail(DYN_E_INVALID, "pooled launch without a view table [K, V]");
+  if (pool < 1 || pool > kMaxViews) return fail(DYN_E_INVALID, "view pool of %d entries outside 1..%d", pool, kMaxViews);
+  if (V < 1 || V > max_slots) return fail(DYN_E_INVALID, "%d view slots per camera outside 1..%d", V, max_slots);
+  return DYN_OK;
+}
+
+int project_gather_tbl(const float* xyz_st, const float* xyz, const float* query_cams, int K, const int* camera_index,
+                       const int* view_tbl, int pool, const float* src_rgbs, const float* src_cams,
+                       const float* featmaps, int V, int R, int S, int H, int W, int C, int h, int w,
+                       float* feat_cl_ws, float* rgb_feat, float* ray_diff, float* mask, cudaStream_t st) {
+  DYN_CHECK_ARG(xyz_st && query_cams && src_rgbs && src_cams && featmaps && feat_cl_ws);
+  DYN_CHECK_ARG(rgb_feat && ray_diff && mask);
+  DYN_CHECK_ARG(C == kC && H > 1 && W > 1 && h > 1 && w > 1 && S >= 1);
+  ViewCams vc;
+  int rc = build_view_cams(src_cams, pool, query_cams, st, &vc, K);
+  if (rc) return rc;
+  static thread_local ViewTable tbl;
+  rc = build_view_table(view_tbl, K, V, pool, st, &tbl);
+  if (rc) return rc;
+  // the whole pool goes channels-last (an entry no camera uses included: the kernel never reads it)
+  dim3 tb(32, 8), tg(cdiv(h * w, 32), cdiv(C, 32), pool);
+  to_channels_last_kernel<<<tg, tb, 0, st>>>(featmaps, feat_cl_ws, C, h * w);
+  DYN_LAUNCH_CHECK();
+  long long N = (long long)R * S;
+  ProfScope prof(PROF_GATHER, st);
+  project_gather_kernel<<<cdiv(N * V, 256), 256, 0, st>>>(xyz_st, xyz, src_rgbs, feat_cl_ws, vc, tbl, camera_index, S,
+                                                            V, N, H, W, h, w, rgb_feat, ray_diff, mask);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+int plucker_src_tbl(const float* pts, const float* src_cams, int pool, int K, const int* camera_index,
+                    const int* view_tbl, int V, int R, int S, float* out, cudaStream_t st) {
+  DYN_CHECK_ARG(pts && src_cams && out && R >= 0 && S >= 1);
+  ViewCams vc;
+  int rc = build_view_cams(src_cams, pool, nullptr, st, &vc);
+  if (rc) return rc;
+  static thread_local ViewTable tbl;
+  rc = build_view_table(view_tbl, K, V, pool, st, &tbl);
+  if (rc) return rc;
+  long long N = (long long)R * S;
+  plucker_src_kernel<<<cdiv(N * V, 256), 256, 0, st>>>(pts, vc, tbl, camera_index, S, V, N, out);
+  DYN_LAUNCH_CHECK();
   return DYN_OK;
 }
 
@@ -736,24 +812,23 @@ int dyn_project_gather_mc(const float* xyz_st, const float* xyz, const float* qu
   if (K < 1 || K > kMaxTargets) return fail(DYN_E_INVALID, "target camera count K = %d outside 1..%d", K, kMaxTargets);
   if (K > 1 && query_idx == nullptr) return fail(DYN_E_INVALID, "K = %d target cameras need a per-ray camera index", K);
   if (R == 0) return DYN_OK;  // empty batch: nothing to do (pointers may be null)
-  DYN_CHECK_ARG(xyz_st && query_cams && src_rgbs && src_cams && featmaps && feat_cl_ws);
-  DYN_CHECK_ARG(rgb_feat && ray_diff && mask);
-  DYN_CHECK_ARG(C == kC && V >= 1 && V <= kMaxViews && H > 1 && W > 1 && h > 1 && w > 1 && (K == 1 || S >= 1));
-  if (R == 0) return DYN_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  ViewCams vc;
-  int rc = build_view_cams(src_cams, V, query_cams, st, &vc, K);
+  DYN_CHECK_ARG(V >= 1 && V <= kMaxViews);
+  // every camera's slots are the shared views themselves: the identity table over a pool of V views
+  return project_gather_tbl(xyz_st, xyz, query_cams, K, K > 1 ? query_idx : nullptr, nullptr, V, src_rgbs, src_cams,
+                            featmaps, V, R, S, H, W, C, h, w, feat_cl_ws, rgb_feat, ray_diff, mask,
+                            (cudaStream_t)stream);
+}
+
+int dyn_project_gather_tbl(const float* xyz_st, const float* xyz, const float* query_cams, int K,
+                           const int* camera_index, const int* view_tbl, int pool, const float* src_rgbs,
+                           const float* src_cams, const float* featmaps, int V, int R, int S, int H, int W, int C,
+                           int h, int w, float* feat_cl_ws, float* rgb_feat, float* ray_diff, float* mask,
+                           void* stream) {
+  const int rc = check_tbl_args(K, camera_index, view_tbl, pool, V, kMaxViews);
   if (rc) return rc;
-  dim3 tb(32, 8), tg(cdiv(h * w, 32), cdiv(C, 32), V);
-  to_channels_last_kernel<<<tg, tb, 0, st>>>(featmaps, feat_cl_ws, C, h * w);
-  DYN_LAUNCH_CHECK();
-  long long N = (long long)R * S;
-  ProfScope prof(PROF_GATHER, st);
-  project_gather_kernel<<<cdiv(N * V, 256), 256, 0, st>>>(xyz_st, xyz, src_rgbs, feat_cl_ws, vc,
-                                                            K > 1 ? query_idx : nullptr, S, V, N, H, W, h,
-                                                            w, rgb_feat, ray_diff, mask);
-  DYN_LAUNCH_CHECK();
-  return DYN_OK;
+  if (R == 0) return DYN_OK;
+  return project_gather_tbl(xyz_st, xyz, query_cams, K, camera_index, view_tbl, pool, src_rgbs, src_cams, featmaps,
+                            V, R, S, H, W, C, h, w, feat_cl_ws, rgb_feat, ray_diff, mask, (cudaStream_t)stream);
 }
 
 int dyn_compute_projections(const float* xyz, const float* src_cams, int V, int N, float* pix,
@@ -816,16 +891,16 @@ int dyn_plucker_ref(const float* ray_o, const float* ray_d, int R, float* out6, 
 int dyn_plucker_src(const float* pts, const float* src_cams, int V, int R, int S, float* out,
                     void* stream) {
   if (R == 0) return DYN_OK;  // empty batch: nothing to do (pointers may be null)
-  DYN_CHECK_ARG(pts && src_cams && out && R >= 0);
-  if (R == 0) return DYN_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  ViewCams vc;
-  int rc = build_view_cams(src_cams, V, nullptr, st, &vc);
+  DYN_CHECK_ARG(V >= 1 && V <= kMaxViews);
+  return plucker_src_tbl(pts, src_cams, V, 1, nullptr, nullptr, V, R, S, out, (cudaStream_t)stream);
+}
+
+int dyn_plucker_src_tbl(const float* pts, const float* src_cams, int pool, int K, const int* camera_index,
+                        const int* view_tbl, int V, int R, int S, float* out, void* stream) {
+  const int rc = check_tbl_args(K, camera_index, view_tbl, pool, V, kMaxViews);
   if (rc) return rc;
-  long long N = (long long)R * S;
-  plucker_src_kernel<<<cdiv(N * V, 256), 256, 0, st>>>(pts, vc, V, N, out);
-  DYN_LAUNCH_CHECK();
-  return DYN_OK;
+  if (R == 0) return DYN_OK;
+  return plucker_src_tbl(pts, src_cams, pool, K, camera_index, view_tbl, V, R, S, out, (cudaStream_t)stream);
 }
 
 int dyn_flow_sceneflow(const float* weights, const float* pts_seq, const float* src_cams,

@@ -16,6 +16,19 @@ struct ViewCams {
   float tgts[kMaxTargets][3];  // multi-camera launches: centre of target camera k (tgts[0] == tgt)
 };
 
+// Per-camera view slots of a multi-camera launch over a pool of source views: slot v of target camera k reads
+// pool entry v[k][v] (its projection, centre, image and feature map).  Launches without a table use the
+// identity, v[k][s] = s.
+struct ViewTable {
+  uint8_t v[kMaxTargets][kMaxViews];
+};
+
+// tbl: [K, V] int32 (host or device pointer) or null for the identity; every entry must lie in [0, pool)
+int build_view_table(const int* tbl, int K, int V, int pool, cudaStream_t st, ViewTable* out);
+// argument checks of the pooled (tabled) entry points, made before any CUDA call: K target cameras, the camera
+// index when K > 1, the table, a pool of 1..kMaxViews entries, 1..max_slots slots per camera
+int check_tbl_args(int K, const int* camera_index, const int* view_tbl, int pool, int V, int max_slots);
+
 __device__ __forceinline__ void project_point(const float* P, float x, float y, float z, float& u,
                                               float& v, bool& front) {
   float px = P[0] * x + P[1] * y + P[2] * z + P[3];

@@ -22,15 +22,20 @@ int motion_f32(const dyn_net* n, const float* x, int ldx, bool time_is_column, f
                float* coeff, void* ws, size_t ws_bytes, int prec, cudaStream_t st);
 // fused DYN_PREC_BF16 path (per-view stage = nets_fused.cu)
 size_t net_fused_workspace(int kind, int R, int S, int V);
-// query_cams [K,34]; query_idx [R] (device) = target camera of each ray, null for one camera
+// query_cams [K,34]; query_idx [R] (device) = target camera of each ray, null for one camera; the source views
+// are a pool of `pool` entries and view_tbl [K,V] (host or device) maps each camera's slots into it, null = the
+// identity over shared views (pool == V)
 int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, const float* ray_d,
-                     const float* query_cams, int K, const int* query_idx, const float* src_rgbs,
-                     const float* src_cams, const void* feat_cl, int R, int S, int V, int H, int W, int h,
-                     int w, float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st);
+                     const float* query_cams, int K, const int* query_idx, const int* view_tbl, int pool,
+                     const float* src_rgbs, const float* src_cams, const void* feat_cl, int R, int S, int V,
+                     int H, int W, int h, int w, float* raw, float* mask_out, void* ws, size_t ws_bytes,
+                     cudaStream_t st);
+// query_cam: one camera [34] (the dynamic net's outputs do not read it); cam_idx / view_tbl as above
 int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, const float* ray_dir,
-                      const float* query_cam, const float* src_rgbs, const float* src_cams,
-                      const void* feat_cl, float time, int R, int S, int V, int H, int W, int h, int w,
-                      float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st);
+                      const float* query_cam, int K, const int* cam_idx, const int* view_tbl, int pool,
+                      const float* src_rgbs, const float* src_cams, const void* feat_cl, float time, int R,
+                      int S, int V, int H, int W, int h, int w, float* raw, float* mask_out, void* ws,
+                      size_t ws_bytes, cudaStream_t st);
 int debug_point_chain(const dyn_net* n, const float* G, const float* nvalid, const float* pts,
                       const float* ray_dir, int R, int S, float* g2, float* Q, float* K, float* V,
                       float* O, float* out_a, float* out_b, float* posenc_ws, cudaStream_t st);

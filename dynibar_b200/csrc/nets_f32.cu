@@ -1116,11 +1116,17 @@ static int capture_view_outputs(const ViewFusedArgs& va, long long p0, long long
   return DYN_OK;
 }
 
+// pool: the source views src_rgbs / src_cams / feat_cl hold; view_tbl [n_query, V] (null: slot v is view v)
 static int fill_view_args(ViewFusedArgs* a, const float* query_cam, const float* src_rgbs,
                           const float* src_cams, const void* feat_cl, int V, int S, int H, int W,
-                          int h, int w, cudaStream_t st, int n_query = 1) {
+                          int h, int w, cudaStream_t st, int n_query, const int* view_tbl, int pool) {
   memset(a, 0, sizeof(*a));
-  RUN(build_view_cams(src_cams, V, query_cam, st, &a->cams, n_query));
+  RUN(build_view_cams(src_cams, pool, query_cam, st, &a->cams, n_query));
+  static thread_local ViewTable tbl;
+  RUN(build_view_table(view_tbl, n_query, V, pool, st, &tbl));
+  for (int k = 0; k < kMaxTargets; ++k)
+    for (int v = 0; v < 16; ++v) a->tbl[k][v] = tbl.v[k][v];
+  a->pooled = view_tbl != nullptr;
   a->h_img = a->cams.h_img; a->w_img = a->cams.w_img;
   a->rgba = src_rgbs; a->feat_bf = reinterpret_cast<const uint16_t*>(feat_cl);
   a->H = H; a->W = W; a->h = h; a->w = w; a->V = V; a->S = S;
@@ -1128,14 +1134,15 @@ static int fill_view_args(ViewFusedArgs* a, const float* query_cam, const float*
 }
 
 int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, const float* ray_d,
-                     const float* query_cams, int K, const int* query_idx, const float* src_rgbs,
-                     const float* src_cams, const void* feat_cl, int R_all, int S, int V, int H, int W, int h,
-                     int w, float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+                     const float* query_cams, int K, const int* query_idx, const int* view_tbl, int pool,
+                     const float* src_rgbs, const float* src_cams, const void* feat_cl, int R_all, int S, int V,
+                     int H, int W, int h, int w, float* raw, float* mask_out, void* ws, size_t ws_bytes,
+                     cudaStream_t st) {
   const StaticLayout& L = n->sl;
   const int prec = DYN_PREC_BF16;
   RUN(check_attention_samples(S, true));
   ViewFusedArgs va{};
-  RUN(fill_view_args(&va, query_cams, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st, K));
+  RUN(fill_view_args(&va, query_cams, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st, K, view_tbl, pool));
   const int RC = net_rows_per_chunk(S, V);
   for (int r0 = 0; r0 < R_all; r0 += RC) {
     const int R = (R_all - r0) < RC ? (R_all - r0) : RC;
@@ -1174,14 +1181,23 @@ int net_static_fused(const dyn_net* n, const float* pts, const float* ray_o, con
 }
 
 int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, const float* ray_dir,
-                      const float* query_cam, const float* src_rgbs, const float* src_cams,
-                      const void* feat_cl, float time, int R_all, int S, int V, int H, int W, int h,
-                      int w, float* raw, float* mask_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+                      const float* query_cam, int K, const int* cam_idx, const int* view_tbl, int pool,
+                      const float* src_rgbs, const float* src_cams, const void* feat_cl, float time, int R_all,
+                      int S, int V, int H, int W, int h, int w, float* raw, float* mask_out, void* ws,
+                      size_t ws_bytes, cudaStream_t st) {
   const DynamicLayout& L = n->dl;
   const int prec = DYN_PREC_BF16;
   RUN(check_attention_samples(S, true));
   ViewFusedArgs va{};
-  RUN(fill_view_args(&va, query_cam, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st));
+  // the dynamic net's outputs do not read the target camera: one camera row, K only sizes the table
+  RUN(fill_view_args(&va, query_cam, src_rgbs, src_cams, feat_cl, V, S, H, W, h, w, st, 1, nullptr, pool));
+  if (view_tbl != nullptr) {
+    static thread_local ViewTable tbl;
+    RUN(build_view_table(view_tbl, K, V, pool, st, &tbl));
+    for (int k = 0; k < kMaxTargets; ++k)
+      for (int v = 0; v < 16; ++v) va.tbl[k][v] = tbl.v[k][v];
+    va.pooled = 1;
+  }
   const long long P_all = (long long)R_all * S;
   const int RC = net_rows_per_chunk(S, V);
   for (int r0 = 0; r0 < R_all; r0 += RC) {
@@ -1194,6 +1210,7 @@ int net_dynamic_fused(const dyn_net* n, const float* pts, const float* pts_seq, 
     dyn_time_feat_kernel<<<1, 256, 0, st>>>(n->params, L, time, d.small, 0);
     DYN_LAUNCH_CHECK();
     va.pts = pts + p0 * 3; va.pts_seq = pts_seq + p0 * 3; va.seq_stride = P_all; va.P = P;
+    va.tgt_idx = cam_idx != nullptr ? cam_idx + r0 : nullptr;
     va.ref_feat = nullptr; va.dfeat = d.small;
     va.G = d.G; va.nvalid = d.t.nvalid; va.mask_proj = mask_out + p0 * V; va.mask_eff = nullptr;
     va.X = nullptr; va.vis2 = nullptr; va.ray_diff = nullptr; va.rgb_in = nullptr;

@@ -39,7 +39,7 @@ int launch_view_fused(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st
   }
   switch (g_view_kernel < 0 ? kDefaultViewKernel : g_view_kernel) {
     case 0:
-      if (a.tgt_idx != nullptr)
+      if (a.tgt_idx != nullptr || a.pooled)
         return fail(DYN_E_INVALID, "the twin-warp per-view kernel (view_twin.cu) has no multi-camera form: "
                                    "select the warpgroup kernel (dyn_debug_set_view_kernel(-1))");
       return launch_view_twin(n, a, V, st);

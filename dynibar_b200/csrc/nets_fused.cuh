@@ -49,7 +49,11 @@ struct ViewFusedArgs {
   float* ray_diff;   // static [P*V,4]
   float* rgb_in;     // static [P*V,3] gathered source colours
   long long* dbg;    // optional: clock64() phase timestamps of block 0 (profiling builds/tests only)
-  const int* tgt_idx;  // static, multi-camera launches: [R] target camera of each ray (cams.tgts), else null
+  const int* tgt_idx;  // multi-camera launches: [R] target camera of each ray (cams.tgts, tbl), else null
+  // multi-camera launches (tgt_idx set, or pooled): slot v of camera k reads pool entry tbl[k][v] of cams, rgba and
+  // feat_bf; the identity for a launch over shared views
+  int pooled;          // a pooled launch: the table applies even with one camera and no tgt_idx
+  uint8_t tbl[kMaxTargets][16];
 };
 
 // ---- MotionMLP (motion_wg.cu) ----

@@ -33,11 +33,13 @@ namespace {
 // 64 rows
 constexpr int kPeBytes = 14 * 1024, kPoolBytes = 30 * 1024, kWgATile = kPeBytes + kPoolBytes;
 // constants (floats): biases in true units; W6V = row 128 of vis_fc.2 (visibility logit), W8 = vis_fc2.2;
-// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; W1 / MK = per-row pooling weight and mask of each consumer;
-// TGT = the target camera centres of a multi-camera launch (3 floats each)
+// MISC = b(vis_fc.2)[128], b(vis_fc2.2), |s|; CAMS = projection and centre of each pool entry (16 floats each);
+// W1 / MK = per-row pooling weight and mask of each consumer; TGT = the target camera centres of a multi-camera
+// launch (3 floats each); TBL = its view table, bytes [kMaxTargets][16] (slot -> pool entry)
 constexpr int C_B1 = 0, C_B2 = 256, C_B3 = 304, C_B4 = 560, C_B5 = 688, C_B6 = 816, C_W6V = 944, C_B7 = 1072,
-              C_W8 = 1200, C_MISC = 1328, C_DFEAT = 1332, C_CAMS = 1372, C_W1 = 1628, C_MK = 1756, C_TGT = 1884;
-constexpr int kWgConst = C_TGT + 3 * kMaxTargets;
+              C_W8 = 1200, C_MISC = 1328, C_DFEAT = 1332, C_CAMS = 1372, C_W1 = C_CAMS + 16 * kMaxViews,
+              C_MK = C_W1 + 128, C_TGT = C_MK + 128, C_TBL = C_TGT + 3 * kMaxTargets;
+constexpr int kWgConst = C_TBL + kMaxTargets * 16 / 4;
 // mbarriers: the weight ring's full / empty pairs, then per consumer its operand tiles' full and empty
 constexpr int kViewBars = 2 * kWgRing + 4;
 constexpr int kWgSmem = kWgRing * kWgStage + 2 * kWgATile + kWgConst * 4 + 4 /* align */ + kViewBars * 8;
@@ -134,7 +136,9 @@ __device__ __forceinline__ void store2_64(uint8_t* tile, int r, int col, float x
 // The front end of the 64 rows from row0 on, row layout (t = thread of the front-end warpgroup: twin tw = t / 64 of
 // row t % 64): projection, masks, gather, first pooling into columns 0..119 of pool_tile, [static] positional
 // encodings into pe_tile; each row's pooling weight and mask into s_w1 / s_mk; the per-(point, view) outputs.
-// MC (static, multi-camera launch): the target camera centre of the row's ray is cst[C_TGT + 3 a.tgt_idx[ray]].
+// MC (multi-camera launch): the row's ray belongs to camera k = a.tgt_idx[ray] (0 without an index), whose slot v
+// reads pool entry tbl[k][v] (projection, centre, feature map, image); [static] its target camera centre is
+// cst[C_TGT + 3 k].  Everything indexed by slot (masks, pooling, per-(point, view) outputs) stays as it is.
 template <int VP, bool ST, bool MC>
 __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* cst, int t, long long row0,
                                           uint8_t* pe_tile, uint8_t* pool_tile, float* s_w1, float* s_mk) {
@@ -156,7 +160,8 @@ __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* c
     q3[0] = qq[0]; q3[1] = qq[1]; q3[2] = qq[2];
   }
 
-  const int vc = valid ? v : 0;
+  const int k = (MC && pt_ok && a.tgt_idx != nullptr) ? a.tgt_idx[(int)pl / a.S] : 0;
+  const int vc = valid ? (MC ? reinterpret_cast<const uint8_t*>(cst + C_TBL)[16 * k + v] : v) : 0;
   const float* cam = cst + C_CAMS + 16 * vc;
   float pu, pv;
   bool front;
@@ -238,7 +243,7 @@ __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* c
   float rd[4];
   {
     const float* tgt = a.cams.tgt;
-    if (MC) tgt = cst + C_TGT + 3 * (pt_ok ? a.tgt_idx[(int)pl / a.S] : 0);
+    if (MC && ST) tgt = cst + C_TGT + 3 * k;
     float a0 = tgt[0] - p3[0], a1 = tgt[1] - p3[1], a2 = tgt[2] - p3[2];
     normalize3(a0, a1, a2);
     float b0 = cam[12] - q3[0], b1 = cam[13] - q3[1], b2 = cam[14] - q3[2];
@@ -340,7 +345,6 @@ __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* c
 
 template <int VP, bool ST, bool MC>
 __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_constant__ ViewFusedArgs a) {
-  static_assert(ST || !MC, "multi-camera launches are static-net only");
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem;
   uint8_t* atiles = smem + kWgRing * kWgStage;
@@ -366,9 +370,11 @@ __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_c
   }
   {
     const float* prm = a.params;
-    for (int i = tid; i < 256; i += blockDim.x) {
+    for (int i = tid; i < 16 * kMaxViews; i += blockDim.x) {
       const int vv = i >> 4, j = i & 15;
       cst[C_CAMS + i] = j < 12 ? a.cams.P[vv][j] : (j < 15 ? a.cams.center[vv][j - 12] : 0.f);
+    }
+    for (int i = tid; i < 256; i += blockDim.x) {
       cst[C_B1 + i] = ST ? prm[a.o_b1 + i] : 0.f;
       cst[C_B3 + i] = prm[a.o_b3 + i];
     }
@@ -387,7 +393,9 @@ __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_c
       cst[C_MISC + 1] = prm[a.o_b8];
       cst[C_MISC + 2] = (ST && a.o_s >= 0) ? fabsf(prm[a.o_s]) : 0.f;
     }
-    if (MC && tid < 3 * kMaxTargets) cst[C_TGT + tid] = a.cams.tgts[tid / 3][tid % 3];
+    if (MC && ST && tid < 3 * kMaxTargets) cst[C_TGT + tid] = a.cams.tgts[tid / 3][tid % 3];
+    if (MC && tid < kMaxTargets * 4)
+      reinterpret_cast<uint32_t*>(cst + C_TBL)[tid] = reinterpret_cast<const uint32_t*>(&a.tbl[0][0])[tid];
   }
   __syncthreads();
 
@@ -756,12 +764,11 @@ int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
 #define PREP_WG(VPV, STV, MCV) \
     DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV, MCV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem))
     PREP_WG(8, true, false); PREP_WG(16, true, false); PREP_WG(8, false, false); PREP_WG(16, false, false);
-    PREP_WG(8, true, true); PREP_WG(16, true, true);
+    PREP_WG(8, true, true); PREP_WG(16, true, true); PREP_WG(8, false, true); PREP_WG(16, false, true);
 #undef PREP_WG
   }
   const bool st_net = n->kind == DYN_NET_STATIC;
-  const bool mc = a.tgt_idx != nullptr;
-  if (mc && !st_net) return fail(DYN_E_INVALID, "multi-camera per-view launches are for the static net only");
+  const bool mc = a.tgt_idx != nullptr || a.pooled;
   const int VP = V <= 8 ? 8 : 16;
   const long long n_iter = (a.P * VP + 127) / 128;
   const int grid = (int)(n_iter < sms ? n_iter : sms);
@@ -773,6 +780,9 @@ int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
   } else if (st_net) {
     if (VP == 8) view_wg_kernel<8, true, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
     else view_wg_kernel<16, true, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+  } else if (mc) {
+    if (VP == 8) view_wg_kernel<8, false, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    else view_wg_kernel<16, false, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
   } else {
     if (VP == 8) view_wg_kernel<8, false, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
     else view_wg_kernel<16, false, false><<<grid, kViewThreads, kWgSmem, st>>>(a);

@@ -69,15 +69,19 @@ class Projector(object):
     return project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmaps)
 
 
-def project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmaps, camera_index=None):
+def project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmaps, camera_index=None,
+                   view_tbl=None):
   """`xyz` may be None: every view then uses xyz_st (static branch).  With `camera_index` ([R] int32 on the
   device) query_camera is [K,34] and ray r's view-direction term (ray_diff) uses camera camera_index[r]; the
-  kernel trusts the values to lie in [0, K)."""
+  kernel trusts the values to lie in [0, K).  With `view_tbl` ([K,V] int32, host) train_imgs / train_cameras /
+  featmaps hold a pool of source views and slot v of ray r reads pool entry view_tbl[camera_index[r], v]; the
+  outputs have V slots."""
   R, S = xyz_st.shape[:2]
-  V = train_cameras.shape[1]
+  pool = train_cameras.shape[1]
+  V = pool if view_tbl is None else view_tbl.shape[1]
   _, _, H, W, _ = train_imgs.shape
   Vf, Cc, h, w = featmaps.shape
-  assert Vf == V and (xyz is None or xyz.shape[0] == V)
+  assert Vf == pool and (xyz is None or xyz.shape[0] == V)
   dev = dev_of(xyz_st)
   rgb_feat = torch.empty(R, S, V, 3 + Cc, device=dev)
   ray_diff = torch.empty(R, S, V, 4, device=dev)
@@ -86,7 +90,14 @@ def project_gather(xyz_st, xyz, query_camera, train_imgs, train_cameras, featmap
   ws = _lib.workspace.get(fm.numel() * 4, dev, slot=1)
   A = Args()
   with torch.cuda.device(dev):
-    if camera_index is None:
+    if view_tbl is not None:
+      K = query_camera.shape[0]
+      assert view_tbl.shape[0] == K, "one table row per target camera"
+      check(lib.dyn_project_gather_tbl(
+          A(xyz_st), A(xyz), A.host(query_camera), K, A(camera_index, torch.int32) if camera_index is not None
+          else None, A.host_i32(view_tbl), pool, A(train_imgs), A.host(train_cameras), ptr(fm), V, R, S, H, W,
+          Cc, h, w, ws.data_ptr(), ptr(rgb_feat), ptr(ray_diff), ptr(mask), stream()))
+    elif camera_index is None:
       check(lib.dyn_project_gather(
           A(xyz_st), A(xyz),
           A.host(query_camera), A(train_imgs), A.host(train_cameras), ptr(fm),

@@ -253,14 +253,20 @@ def compute_ref_plucker_coordinate(ray_o, ray_d):
   return out
 
 
-def compute_src_plucker_coordinate(pts, src_cameras):
-  """pts [R,S,3], src_cameras [1,V,34] -> [R,S,V,6] (render_ray.py:380-396)."""
+def compute_src_plucker_coordinate(pts, src_cameras, camera_index=None, view_tbl=None):
+  """pts [R,S,3], src_cameras [1,V,34] -> [R,S,V,6] (render_ray.py:380-396).  With `view_tbl` ([K,V] int32, host)
+  src_cameras is a pool [1,P,34] and slot v of ray r is pool entry view_tbl[camera_index[r], v]."""
   R, S = pts.shape[:2]
-  V = src_cameras.shape[1]
+  V = src_cameras.shape[1] if view_tbl is None else view_tbl.shape[1]
   out = torch.empty(R, S, V, 6, device=dev_of(pts))
   A = Args()
   with torch.cuda.device(pts.device):
-    check(lib.dyn_plucker_src(A(pts), A.host(src_cameras), V, R, S, ptr(out), stream()))
+    if view_tbl is None:
+      check(lib.dyn_plucker_src(A(pts), A.host(src_cameras), V, R, S, ptr(out), stream()))
+    else:
+      check(lib.dyn_plucker_src_tbl(A(pts), A.host(src_cameras), src_cameras.shape[1], view_tbl.shape[0],
+                                    A(camera_index, torch.int32) if camera_index is not None else None,
+                                    A.host_i32(view_tbl), V, R, S, ptr(out), stream()))
   return out
 
 
@@ -368,15 +374,17 @@ def source_rgba(src_rgbs):
   return _frame_cache.get("rgba", src_rgbs, _pack_rgba)
 
 
-def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, feat_cl, camera_index=None):
+def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, feat_cl, camera_index=None,
+                     view_tbl=None):
   """Projector.compute_with_motions + DynibarStatic.forward fused
   (projection.py:103-176 + mlp_network.py:423-527) -> raw [R,S,4], mask [R,S,V,1].
   With `camera_index` ([R] int32, device) query_cam is [K,34] and ray r is seen from camera camera_index[r]
-  (values trusted to lie in [0, K))."""
+  (values trusted to lie in [0, K)).  With `view_tbl` ([K,V] int32, host) the source views are a pool and slot v
+  of ray r reads pool entry view_tbl[camera_index[r], v]."""
   dev = dev_of(pts)
   net = _weights.packed_of(module, dev)
   R, S = pts.shape[:2]
-  V = src_cams.shape[1]
+  V = src_cams.shape[1] if view_tbl is None else view_tbl.shape[1]
   _, _, H, W, _ = src_rgbs.shape
   _, h, w, Cc = feat_cl.shape
   raw = torch.empty(R, S, 4, device=dev)
@@ -385,7 +393,14 @@ def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, f
   ws = _lib.workspace.get(nbytes, dev)
   A = Args()
   with torch.cuda.device(dev):
-    if camera_index is None:
+    if view_tbl is not None:
+      check(lib.dyn_net_static_fused_tbl(net.handle, A(pts), A(ray_o), A(ray_d), A.host(query_cam),
+                                         query_cam.shape[0], A(camera_index, torch.int32)
+                                         if camera_index is not None else None, A.host_i32(view_tbl),
+                                         src_cams.shape[1], ptr(source_rgba(src_rgbs)), A.host(src_cams),
+                                         ptr(feat_cl, torch.bfloat16), R, S, V, H, W, Cc, h, w, ptr(raw),
+                                         ptr(mask), ws.data_ptr(), nbytes, stream()))
+    elif camera_index is None:
       check(lib.dyn_net_static_fused(net.handle, A(pts), A(ray_o), A(ray_d), A.host(query_cam),
                                      ptr(source_rgba(src_rgbs)), A.host(src_cams),
                                      ptr(feat_cl, torch.bfloat16), R, S, V, H, W, Cc, h, w, ptr(raw),
@@ -400,13 +415,15 @@ def net_static_fused(module, pts, ray_o, ray_d, query_cam, src_rgbs, src_cams, f
   return raw, mask
 
 
-def net_dynamic_fused(module, pts, pts_seq, ray_dir, query_cam, src_rgbs, src_cams, feat_cl, time):
+def net_dynamic_fused(module, pts, pts_seq, ray_dir, query_cam, src_rgbs, src_cams, feat_cl, time,
+                      camera_index=None, view_tbl=None):
   """Projector.compute_with_motions + DynibarDynamic.forward fused
-  (projection.py:103-176 + mlp_network.py:236-316) -> raw [R,S,4], mask [R,S,V,1]."""
+  (projection.py:103-176 + mlp_network.py:236-316) -> raw [R,S,4], mask [R,S,V,1].  `camera_index` /
+  `view_tbl` as for net_static_fused (query_cam stays one camera: the dynamic net's outputs do not read it)."""
   dev = dev_of(pts)
   net = _weights.packed_of(module, dev)
   R, S = pts.shape[:2]
-  V = src_cams.shape[1]
+  V = src_cams.shape[1] if view_tbl is None else view_tbl.shape[1]
   _, _, H, W, _ = src_rgbs.shape
   _, h, w, Cc = feat_cl.shape
   raw = torch.empty(R, S, 4, device=dev)
@@ -415,10 +432,18 @@ def net_dynamic_fused(module, pts, pts_seq, ray_dir, query_cam, src_rgbs, src_ca
   ws = _lib.workspace.get(nbytes, dev)
   A = Args()
   with torch.cuda.device(dev):
-    check(lib.dyn_net_dynamic_fused(net.handle, A(pts), A(pts_seq), A(ray_dir), A.host(query_cam),
-                                    ptr(source_rgba(src_rgbs)), A.host(src_cams),
-                                    ptr(feat_cl, torch.bfloat16), float(time), R, S, V, H, W,
-                                    Cc, h, w, ptr(raw), ptr(mask), ws.data_ptr(), nbytes, stream()))
+    if view_tbl is not None:
+      check(lib.dyn_net_dynamic_fused_tbl(net.handle, A(pts), A(pts_seq), A(ray_dir), A.host(query_cam),
+                                          view_tbl.shape[0], A(camera_index, torch.int32)
+                                          if camera_index is not None else None, A.host_i32(view_tbl),
+                                          src_cams.shape[1], ptr(source_rgba(src_rgbs)), A.host(src_cams),
+                                          ptr(feat_cl, torch.bfloat16), float(time), R, S, V, H, W, Cc, h, w,
+                                          ptr(raw), ptr(mask), ws.data_ptr(), nbytes, stream()))
+    else:
+      check(lib.dyn_net_dynamic_fused(net.handle, A(pts), A(pts_seq), A(ray_dir), A.host(query_cam),
+                                      ptr(source_rgba(src_rgbs)), A.host(src_cams),
+                                      ptr(feat_cl, torch.bfloat16), float(time), R, S, V, H, W,
+                                      Cc, h, w, ptr(raw), ptr(mask), ws.data_ptr(), nbytes, stream()))
   return raw, mask
 
 
@@ -538,8 +563,14 @@ def camera_count(ray_batch):
   return K
 
 
+def is_pooled(ray_batch):
+  """True for a pooled multi-camera batch (sample_ray.stack_pooled_ray_batches): per-camera view tables
+  `src_views` / `static_src_views` over pools of source views."""
+  return ray_batch.get("src_views") is not None and ray_batch.get("static_src_views") is not None
+
+
 def _refuse_multi_camera(ray_batch, what):
-  if camera_count(ray_batch) > 1:
+  if camera_count(ray_batch) > 1 or is_pooled(ray_batch):
     raise NotImplementedError(
         "%s renders one target camera per time step; multi-camera ray batches (batched target cameras) are "
         "for render_rays_mv / render_image.render_multi_image_nvi" % what)
@@ -569,29 +600,36 @@ def _render_pass(ray_batch, feat_dy, feat_st, pts, z, s, t, frame_idx, offsets, 
   # multi-camera batch: only the static branch's ray_diff reads the target camera (the dynamic net discards
   # ray_diff, mlp_network.py:236-316), so the dynamic calls keep one camera
   cam_idx = ray_batch.get("camera_index")
-  cam_dy = cam if cam_idx is None else cam[0:1]
+  # pooled batch (sample_ray.stack_pooled_ray_batches): the source views are pools and each camera's view slots
+  # map into them through the [K, V] tables (both branches: every camera keeps its K rows); the per-slot results
+  # are those of the camera's own views
+  tbl_dy, tbl_st = ray_batch.get("src_views"), ray_batch.get("static_src_views")
+  cam_dy = cam if cam_idx is None or tbl_dy is not None else cam[0:1]
+  v_dy = ray_batch["src_cameras"].shape[1] if tbl_dy is None else tbl_dy.shape[1]
+  v_st = ray_batch["static_src_cameras"].shape[1] if tbl_st is None else tbl_st.shape[1]
+  ci_dy = None if tbl_dy is None else cam_idx
   ref_plucker = compute_ref_plucker_coordinate(ray_o, ray_d)  # [d_hat, o x d_hat]
   ray_dir = ref_plucker[:, :3]  # == F.normalize(ray_d) (render_ray.py:455)
   coeff = motion_coefficients(motion, pts, t)
   seq = displaced_points(pts, coeff, basis, frame_idx, offsets, num_vv)
-  fused = (_prec() == _lib.PREC_BF16 and USE_FUSED and ray_batch["src_cameras"].shape[1] <= 16
-           and ray_batch["static_src_cameras"].shape[1] <= 16)
+  fused = _prec() == _lib.PREC_BF16 and USE_FUSED and v_dy <= 16 and v_st <= 16
   if fused:
     # gather + per-view MLP chain + pooling in one tensor-core kernel per branch: the
     # [R,S,V,35] gather output and the per-view activations never reach HBM
     raw_dy, m_dy = net_dynamic_fused(net_dy, pts, seq, ray_dir, cam_dy, ray_batch["src_rgbs"],
-                                     ray_batch["src_cameras"], featmaps_channels_last(feat_dy), t)
+                                     ray_batch["src_cameras"], featmaps_channels_last(feat_dy), t, ci_dy, tbl_dy)
     raw_st, m_st = net_static_fused(net_st, pts, ray_o, ray_d, cam, ray_batch["static_src_rgbs"],
                                     ray_batch["static_src_cameras"],
-                                    featmaps_channels_last(feat_st), cam_idx)
+                                    featmaps_channels_last(feat_st), cam_idx, tbl_st)
   else:
     f_dy, _, m_dy = project_gather(pts, seq, cam_dy, ray_batch["src_rgbs"], ray_batch["src_cameras"],
-                                   feat_dy)
+                                   feat_dy, ci_dy, tbl_dy)
     f_st, rd_st, m_st = project_gather(pts, None, cam, ray_batch["static_src_rgbs"],
-                                       ray_batch["static_src_cameras"], feat_st, cam_idx)
+                                       ray_batch["static_src_cameras"], feat_st, cam_idx, tbl_st)
     raw_dy = net_dynamic_forward(net_dy, pts, f_dy, ray_dir, m_dy, t)
     raw_st = net_static_forward(net_st, pts, ref_plucker,
-                                compute_src_plucker_coordinate(pts, ray_batch["static_src_cameras"]),
+                                compute_src_plucker_coordinate(pts, ray_batch["static_src_cameras"],
+                                                               cam_idx, tbl_st),
                                 f_st, rd_st, m_st)
   V_dy, V_st = m_dy.shape[2], m_st.shape[2]
   # a sample counts when MORE THAN ONE view sees it (render_ray.py:524-529)
@@ -666,8 +704,13 @@ def render_rays_mono(frame_idx, time_embedding, time_offset, ray_batch, model, f
   """Coarse-only rendering for monocular video (render_ray.py:870-1277), including the
   cross-time branch (:1099-1270) when is_train=True.  With gradients enabled and parameters / feature
   maps that require grad the differentiable fp32 training path runs (`_render_mono_train`); otherwise
-  the forward-only kernels (fused tensor-core path in bf16 mode) under no_grad."""
-  _refuse_multi_camera(ray_batch, "render_rays_mono (and its training path)")
+  the forward-only kernels (fused tensor-core path in bf16 mode) under no_grad.
+  `ray_batch` may be a pooled multi-camera batch (sample_ray.stack_pooled_ray_batches) when is_train=False and no
+  gradient is wanted: the rays of K target cameras of one time step, each camera with its own source views from
+  shared pools.  Its table and camera_index values are not checked here (render_image.render_multi_image_mono
+  checks them once per call)."""
+  if not (is_pooled(ray_batch) and not is_train and not _wants_grad(model, featmaps)):
+    _refuse_multi_camera(ray_batch, "render_rays_mono (and its training path)")
   if _wants_grad(model, featmaps):
     with precision_scope(precision):
       return _render_mono_train_chunked(frame_idx, time_embedding, time_offset, ray_batch, model, featmaps,

@@ -202,3 +202,103 @@ def stack_ray_batches(batches):
   out["camera_index"] = torch.repeat_interleave(torch.arange(K, dtype=torch.int32),
                                                 torch.tensor(counts)).to(dev)
   return out, counts, hw.pop()
+
+
+MAX_POOL = 32  # source views of one pool (csrc/common.cuh: kMaxViews)
+
+
+def _is_virtual(ident):
+  return isinstance(ident, tuple) and len(ident) > 0 and ident[0] == "vv"
+
+
+def _pool_views(batches, ids, rgb_key, cam_key):
+  """Union of the batches' source views by identity -> (rgbs [1,P,H,W,3], cameras [1,P,34], table int32 [K,V]).
+  Entries keep the order in which they are first met (batch 0's slots first)."""
+  index, rgbs, cams, rows = {}, [], [], []
+  for k, (b, idk) in enumerate(zip(batches, ids)):
+    r, c = b[rgb_key], b[cam_key]
+    if len(idk) != c.shape[1] or r.shape[1] != c.shape[1]:
+      raise ValueError("stack_pooled_ray_batches: batch %d has %d '%s' views and %d identities"
+                       % (k, c.shape[1], cam_key, len(idk)))
+    row = []
+    for v, ident in enumerate(idk):
+      i = index.get(ident)
+      if i is None:
+        i = index[ident] = len(cams)
+        rgbs.append(r[0, v])
+        cams.append(c[0, v])
+      elif not (_same(rgbs[i], r[0, v]) and _same(cams[i], c[0, v])):
+        raise ValueError("stack_pooled_ray_batches: batch %d's '%s' view %r differs from the view of that identity in "
+                         "an earlier batch (equal identities must be equal views)" % (k, cam_key, ident))
+      row.append(i)
+    rows.append(row)
+  if len(cams) > MAX_POOL:
+    raise ValueError("stack_pooled_ray_batches: the '%s' pool holds %d views, at most %d" % (cam_key, len(cams), MAX_POOL))
+  if len({len(r) for r in rows}) != 1:
+    raise ValueError("stack_pooled_ray_batches: the batches have different numbers of '%s' slots" % cam_key)
+  return torch.stack(rgbs)[None], torch.stack(cams)[None], torch.tensor(rows, dtype=torch.int32), list(index)
+
+
+def stack_pooled_ray_batches(batches, dy_ids, st_ids):
+  """K `get_all()` batches of target cameras of ONE time step of a monocular video, each with its own source views
+  (render_monocular_bt.py: a bullet-time sweep) -> (pooled batch, per-camera ray counts, (H, W) of the targets).
+
+  dy_ids[k] / st_ids[k] name the source view of every slot of batch k's src_* / static_src_* views (frame ids for
+  frames, ("vv", j) for the frame's virtual view j, any hashable).  Views are pooled by identity: equal identities
+  must carry equal views.  The pooled batch is a multi-camera batch (stack_ray_batches: camera [K,34],
+  camera_index int32 [R], the rays concatenated) whose src_rgbs / src_cameras [1,Pd,...] and static_src_rgbs /
+  static_src_cameras [1,Ps,...] hold the pools, and src_views int32 [K,V_dy] / static_src_views int32 [K,V_st]
+  (host) name the pool entry of each camera's slots; src_view_ids / static_src_view_ids list the pools' identities
+  in pool order (to encode or mask the pools' images).  The temporal views (every leading identity that is not a
+  virtual view) must be the same slots in every batch; they come first in the dynamic pool, so the flows, which
+  read the first slots, see them.  ValueError for more than 16 batches, a pool of more than 32 views, temporal slots
+  that differ, or per-frame tensors (depth range) that differ.
+  render_image.render_multi_image_mono renders it; feature maps are the pools' (one encoder run per pool)."""
+  K = len(batches)
+  if not 1 <= K <= 16:
+    raise ValueError("stack_pooled_ray_batches: %d batches, 1..16 target cameras per batch" % K)
+  if len(dy_ids) != K or len(st_ids) != K:
+    raise ValueError("stack_pooled_ray_batches: %d batches, %d / %d identity lists" % (K, len(dy_ids), len(st_ids)))
+  dy_ids = [list(x) for x in dy_ids]
+  st_ids = [list(x) for x in st_ids]
+  first = batches[0]
+  for i, b in enumerate(batches[1:], 1):
+    if not _same(first.get("depth_range"), b.get("depth_range")):
+      raise ValueError("stack_pooled_ray_batches: batch %d does not share 'depth_range' with batch 0 (the target "
+                       "cameras of one time step share the frame's depth range)" % i)
+  temporal = []
+  for ids in dy_ids:
+    n = 0
+    while n < len(ids) and not _is_virtual(ids[n]):
+      n += 1
+    if any(not _is_virtual(x) for x in ids[n:]):
+      raise ValueError("stack_pooled_ray_batches: temporal views must lead the dynamic slots, got %r" % (ids,))
+    temporal.append(ids[:n])
+  if any(t != temporal[0] for t in temporal):
+    raise ValueError("stack_pooled_ray_batches: the temporal slots differ between cameras (%r vs %r); every camera "
+                     "of one time step uses the same temporal views" % (temporal[0], next(t for t in temporal
+                                                                                       if t != temporal[0])))
+  if len(temporal[0]) < min(6, len(dy_ids[0])):
+    raise ValueError("stack_pooled_ray_batches: %d temporal slots; the flows read the first %d dynamic slots"
+                     % (len(temporal[0]), min(6, len(dy_ids[0]))))
+  cams = [b["camera"] for b in batches]
+  if any(c.dim() != 2 or c.shape[0] != 1 for c in cams):
+    raise ValueError("stack_pooled_ray_batches: every batch has one target camera [1,34]")
+  hw = {(int(c[0, 0]), int(c[0, 1])) for c in cams}
+  if len(hw) != 1:
+    raise ValueError("stack_pooled_ray_batches: the target cameras have different image sizes %s" % sorted(hw))
+  src_rgbs, src_cams, src_views, dy_pool = _pool_views(batches, dy_ids, "src_rgbs", "src_cameras")
+  st_rgbs, st_cams, st_views, st_pool = _pool_views(batches, st_ids, "static_src_rgbs", "static_src_cameras")
+  out = {k: v for k, v in first.items() if not k.startswith("anchor_src_") and k != "static_src_masks"}
+  for k in _CAMERA_KEYS + _RAY_KEYS:
+    if k in first:
+      out[k] = _stack(batches, k, 0)
+  for k in ("flows", "masks"):  # [n_views, R, c]
+    if k in first:
+      out[k] = _stack(batches, k, 1)
+  out.update(src_rgbs=src_rgbs, src_cameras=src_cams, static_src_rgbs=st_rgbs, static_src_cameras=st_cams,
+             src_views=src_views, static_src_views=st_views, src_view_ids=dy_pool, static_src_view_ids=st_pool)
+  counts = [b["ray_o"].shape[0] for b in batches]
+  out["camera_index"] = torch.repeat_interleave(torch.arange(K, dtype=torch.int32),
+                                                torch.tensor(counts)).to(first["ray_o"].device)
+  return out, counts, hw.pop()

@@ -160,6 +160,20 @@ int dyn_project_gather_mc(const float* xyz_st, const float* xyz,
                           int W, int C, int h, int w, float* feat_cl_ws,
                           float* rgb_feat, float* ray_diff, float* mask,
                           void* stream);
+/* Pooled multi-camera form: every target camera has its own view slots, drawn from one shared pool of source
+ * views.  src_rgbs [pool,H,W,3], src_cams [pool,34] and featmaps [pool,C,h,w] hold the pool (1 <= pool <= 32);
+ * view_tbl [K,V] int32 (host or device) names the pool entry of slot v of camera k, camera_index [R] (device,
+ * int32; NULL allowed when K = 1) the camera of each ray.  Slot v of ray r projects onto, and gathers from, pool
+ * entry view_tbl[camera_index[r], v]; xyz [V,R,S,3] and the outputs stay indexed by slot.  With
+ * view_tbl[k] = 0..V-1 for every k the call is dyn_project_gather_mc.  K, camera_index, view_tbl, pool and
+ * 1 <= V <= 32 are checked before any CUDA call; the table's values (in [0, pool)) are checked before any launch.
+ * The kernel trusts camera_index to lie in [0, K). */
+int dyn_project_gather_tbl(const float* xyz_st, const float* xyz,
+                           const float* query_cams, int K, const int* camera_index,
+                           const int* view_tbl, int pool, const float* src_rgbs,
+                           const float* src_cams, const float* featmaps, int V, int R,
+                           int S, int H, int W, int C, int h, int w, float* feat_cl_ws,
+                           float* rgb_feat, float* ray_diff, float* mask, void* stream);
 /* compute_projections only (projection.py:32-59): pix [V,N,2], front [V,N] u8 */
 int dyn_compute_projections(const float* xyz, const float* src_cams, int V,
                             int N, float* pix, uint8_t* front, void* stream);
@@ -176,6 +190,11 @@ int dyn_plucker_ref(const float* ray_o, const float* ray_d, int R, float* out6,
                     void* stream);
 int dyn_plucker_src(const float* pts, const float* src_cams, int V, int R,
                     int S, float* out /* [R,S,V,6] */, void* stream);
+/* Pooled form (see dyn_project_gather_tbl): src_cams [pool,34]; slot v of ray r is the centre of pool entry
+ * view_tbl[camera_index[r], v].  Same checks as dyn_project_gather_tbl. */
+int dyn_plucker_src_tbl(const float* pts, const float* src_cams, int pool, int K,
+                        const int* camera_index, const int* view_tbl, int V, int R,
+                        int S, float* out /* [R,S,V,6] */, void* stream);
 
 /* ---- a8-a11: the two aggregation networks ---------------------------------
  * DynibarDynamic.forward mlp_network.py:236-316 -> raw [R,S,4].
@@ -235,6 +254,27 @@ int dyn_net_dynamic_fused(dyn_net_t net, const float* pts, const float* pts_seq,
                           int H, int W, int C, int h, int w, float* raw,
                           float* mask_out, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* Pooled multi-camera forms of the two fused calls (see dyn_project_gather_tbl): src_rgba [pool,H,W,4],
+ * src_cams [pool,34] and feat_cl [pool,h,w,C] hold the pool (pool <= 32), view_tbl [K,V] int32 and
+ * camera_index [R] map each ray's slots into it, V <= 16.  Every output, per (point, slot) included, equals the
+ * single-camera call on that camera's own views, pool[view_tbl[k]], bit for bit.  The dynamic net reads the
+ * table only (its target camera does not enter its outputs): query_cam is one camera [34].  Checks as for
+ * dyn_project_gather_tbl; warpgroup per-view kernel only (DYN_E_INVALID with the twin-warp kernel selected). */
+int dyn_net_static_fused_tbl(dyn_net_t net, const float* pts, const float* ray_o,
+                             const float* ray_d, const float* query_cams, int K,
+                             const int* camera_index, const int* view_tbl, int pool,
+                             const float* src_rgba, const float* src_cams,
+                             const void* feat_cl, int R, int S, int V, int H, int W,
+                             int C, int h, int w, float* raw, float* mask_out,
+                             void* workspace, size_t workspace_bytes, void* stream);
+int dyn_net_dynamic_fused_tbl(dyn_net_t net, const float* pts, const float* pts_seq,
+                              const float* ray_dir, const float* query_cam, int K,
+                              const int* camera_index, const int* view_tbl, int pool,
+                              const float* src_rgba, const float* src_cams,
+                              const void* feat_cl, float time, int R, int S, int V,
+                              int H, int W, int C, int h, int w, float* raw,
+                              float* mask_out, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 /* ---- a12: raw2outputs / raw2outputs_vanilla, render_ray.py:134-330 --------
  * raw_* [R,S,4]; z_vals [R,S]; mask_* [R,S,V*] as produced by
