@@ -53,6 +53,12 @@ class MonoLossGrads(C.Structure):
                                   "sf_seq")])
 
 
+# ---- a device-resident monocular scene (include/dynibar_b200.h: dyn_scene_t) -------------------------------------
+class Scene(C.Structure):
+  _fields_ = ([(k, _vp) for k in ("frames", "vviews", "srcmask", "motion", "stat", "disp", "flows", "flow_masks")] +
+              [(k, _i) for k in ("N", "H", "W", "mc", "flow_base", "NF")])
+
+
 # name -> (restype, argtypes); mirrors include/dynibar_b200.h one to one
 SIGNATURES = {
     "dyn_version": (_i, []),
@@ -156,6 +162,10 @@ SIGNATURES = {
     "dyn_virtual_views": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "dyn_image_scores_workspace_bytes": (_sz, [_i, _i, _i]),
     "dyn_image_scores": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "dyn_scene_masks_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dyn_scene_masks": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dyn_scene_views": (_i, [C.POINTER(Scene), _vp, _i, _vp, _i, _vp, _i, _vp, _i] + [_vp] * 7),
+    "dyn_scene_rays": (_i, [C.POINTER(Scene), _vp, _vp, _vp, _i] + [_vp] * 9 + [_vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

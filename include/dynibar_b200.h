@@ -655,6 +655,48 @@ size_t dyn_image_scores_workspace_bytes(int K, int H, int W);
 int dyn_image_scores(const float* pred, const float* gt, const float* mask, int K, int H, int W, int mode,
                      double* scores, float* ssim_map, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- a monocular training scene resident on the device (DESIGN §3.7; csrc/scene.cu) --------------------------------
+ * MonocularDataset.__getitem__ (ibrnet/data_loaders/monocular.py:146-426) and RaySamplerSingleImage.random_sample
+ * (ibrnet/sample_ray.py:262-331) on a scene uploaded once.  Float values are the reference's float32 expressions,
+ * rounded as numpy rounds them: u8 / 255.0f, 1 - x, the masked view's product.  No float atomics, no host
+ * synchronisation: the same inputs give the same bits. */
+typedef struct {
+  const uint8_t* frames;     /* [N,H,W,3] images_WxH */
+  const uint8_t* vviews;     /* [N,8,H,W,3] source_virtual_views_WxH */
+  const uint8_t* srcmask;    /* [N,H,W,mc] nearest-resized dynamic masks, raw values (load_src_view's mask) */
+  const uint8_t* motion;     /* [N,H,W] {0,1} */
+  const uint8_t* stat;       /* [N,H,W] {0,1} */
+  const float* disp;         /* [N,H,W] disparity / float32(scale) */
+  const float* flows;        /* [NF,6,H,W,2]: frame flow_base + i, offsets 1, 2, 3, -1, -2, -3 */
+  const uint8_t* flow_masks; /* [NF,6,H,W] {0,1} */
+  int N, H, W, mc, flow_base, NF;
+} dyn_scene_t;
+/* workspace of dyn_scene_masks: the eroded masks at eh x ew */
+size_t dyn_scene_masks_workspace_bytes(int N, int eh, int ew);
+/* Masks of N frames (monocular.py:131-142, :164-204): dyn [N,mh,mw,mc] uint8 (mc 1 or 3; channel 0 is the motion
+ * mask's), st [N,sh,sw] uint8.  cv2 INTER_NEAREST resizes (src index min(floor(x (1 / (dst / src))), src - 1) in
+ * double).  motion [N,H,W] = nearest (H, W) of the erosion by disk(radius) (scipy grey_erosion, mode 'reflect') of
+ * (1 - dyn / 255 > 1e-3) at its nearest (eh, ew) (eh = 288, ew = round(288 W / H)); stat [N,H,W] = 1 - st / 255 >
+ * 1e-3 at its nearest (H, W); srcmask [N,H,W,mc] = dyn at its nearest (H, W).  radius <= 16.  Two launches. */
+int dyn_scene_masks(const uint8_t* dyn, int mh, int mw, int mc, const uint8_t* st, int sh, int sw, int N, int H, int W,
+                    int eh, int ew, int radius, uint8_t* motion, uint8_t* stat, uint8_t* srcmask, void* workspace,
+                    size_t workspace_bytes, void* stream);
+/* One step's source-view stacks and target frame, one launch.  table (device, 16-byte aligned) int32 [(V + 1) * 4]:
+ * rows 0..V-1 = (frame, virtual view 0..7 or -1 for the frame itself, masked, stack << 8 | slot) with stack 0 src,
+ * 1 anchor, 2 static; row V = (target frame, -, -, -).  A masked view is multiplied by its frame's srcmask / 255
+ * (a 1-channel mask broadcasts over the 3 channels).  Stacks [n_*,H,W,3] fp32; rgb [H,W,3], disp / motion_mask /
+ * static_mask [H,W], flows [6,H,W,2], masks [6,H,W] fp32 of the target frame. */
+int dyn_scene_views(const dyn_scene_t* scene, const int* table, int V, float* src_rgbs, int n_src,
+                    float* anchor_src_rgbs, int n_anchor, float* static_src_rgbs, int n_static, float* rgb, float* disp,
+                    float* motion_mask, float* static_mask, float* flows, float* masks, void* stream);
+/* R rays of the target frame *target (device int), one thread per ray: pixel sel[i] (device int32 [R]; NULL: pixel i,
+ * R = H W).  cam (device) fp32 [12] = M (3x3 row-major) | t with M = R_c2w K^-1 formed on the host in float32:
+ * ray_d = (M0 u + M1 v) + M2 per row, ray_o = t, uv_grid = (u, v).  With rgb != NULL also rgb [R,3], disp /
+ * motion_mask / static_mask [R], flows [6,R,2], masks [6,R,1] at the selected pixels. */
+int dyn_scene_rays(const dyn_scene_t* scene, const float* cam, const int* target, const int* sel, int R, float* ray_o,
+                   float* ray_d, float* uv_grid, float* rgb, float* disp, float* motion_mask, float* static_mask,
+                   float* flows, float* masks, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
