@@ -53,7 +53,9 @@ constexpr int kViewConsumerRegs = 208, kViewFrontRegs = 72, kViewProducerRegs = 
 // Phase profile of block 0 (dyn_debug_set_view_timestamps).  Thread 0 of each warpgroup charges the cycles since
 // its previous mark to one phase, less the weight-ring waits in between, which go to PH_WEIGHTS; the counters sit in
 // shared memory while the kernel runs and are copied to dbg[32 wg + phase] at its end.  tools/view_phases.py reads
-// them; the indices are its table.
+// them; the indices are its table.  In the static net only the PROF instantiations, launched while the hook is
+// set, carry the marks and the ring's wait timers (78 clock reads and their predicated bookkeeping, issued every
+// iteration; 7 % of the kernel's instructions).  The dynamic net keeps them: without them ptxas spills 2 KB.
 enum Phase {
   PH_FRONT, PH_BAR, PH_WEIGHTS, PH_F1, PH_F1_EPI, PH_F2, PH_F2_EPI, PH_F3, PH_F3_EPI, PH_F4, PH_F4_EPI, PH_F5,
   PH_F5_EPI, PH_F6, PH_F6_EPI, PH_F7, PH_F7_EPI, PH_POOL2, PH_HANDOFF,
@@ -61,10 +63,13 @@ enum Phase {
 };
 constexpr int kPhaseSlots = 32;
 __shared__ long long s_phase[3][kPhaseSlots];  // consumers 0, 1, front end
+template <bool PROF>
 struct PhaseClock {
   const ViewFusedArgs& a;  // profiling when a.dbg is set: thread 0 of each warpgroup of block 0
   int wg;
-  __device__ __forceinline__ bool on() const { return a.dbg != nullptr && blockIdx.x == 0 && (threadIdx.x & 127) == 0; }
+  __device__ __forceinline__ bool on() const {
+    return PROF && a.dbg != nullptr && blockIdx.x == 0 && (threadIdx.x & 127) == 0;
+  }
   __device__ __forceinline__ long long* c() const { return s_phase[wg]; }
   __device__ __forceinline__ void start() {
     if (!on()) return;
@@ -343,7 +348,7 @@ __device__ __forceinline__ void front_end(const ViewFusedArgs& a, const float* c
   }
 }
 
-template <int VP, bool ST, bool MC>
+template <int VP, bool ST, bool MC, bool PROF>
 __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_constant__ ViewFusedArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem;
@@ -409,7 +414,7 @@ __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_c
   }
   if (wg == 2) {
     setmaxnreg_dec<kViewFrontRegs>();
-    PhaseClock pc{a, 2};
+    PhaseClock<PROF || !ST> pc{a, 2};
     pc.start();
     uint32_t k = 0;  // iterations handed over to each consumer so far
     for (int it = blockIdx.x; it < n_iter; it += gridDim.x, ++k) {
@@ -438,7 +443,7 @@ __global__ void __launch_bounds__(kViewThreads, 1) view_wg_kernel(const __grid_c
   // fragment layout: rows fr[h] of the half-tile
   const int fr[2] = {16 * ww + (lane >> 2), 16 * ww + (lane >> 2) + 8};
 
-  PhaseClock pc{a, wg};
+  PhaseClock<PROF || !ST> pc{a, wg};
   Ring rg{ring, bar0, 0u, pc.on(), 0};
   pc.start();
 #define TS(ph) pc.mark(ph, rg.wait_cycles)
@@ -751,6 +756,12 @@ int view_wg_build(dyn_net* n, const float* P, void* dst_dev, size_t dst_bytes, c
   return upload_wg_image(img, tab, dst_dev, dst_bytes, "per-view", &n->wg, st);
 }
 
+template <int VP, bool ST, bool MC>
+void launch_view_wg_inst(const ViewFusedArgs& a, int grid, cudaStream_t st) {
+  if (a.dbg != nullptr) view_wg_kernel<VP, ST, MC, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+  else view_wg_kernel<VP, ST, MC, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+}
+
 int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
   if (n->wg.img == nullptr) return fail(DYN_E_INVALID, "net has no per-view weight images");
   a.wimg = n->wg.img;
@@ -761,8 +772,10 @@ int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
     int dev = 0;
     DYN_CUDA(cudaGetDevice(&dev));
     DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-#define PREP_WG(VPV, STV, MCV) \
-    DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV, MCV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem))
+#define PREP_WG(VPV, STV, MCV)                                                                                    \
+    DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV, MCV, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                  kWgSmem));                                                                      \
+    DYN_CUDA(cudaFuncSetAttribute(view_wg_kernel<VPV, STV, MCV, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem))
     PREP_WG(8, true, false); PREP_WG(16, true, false); PREP_WG(8, false, false); PREP_WG(16, false, false);
     PREP_WG(8, true, true); PREP_WG(16, true, true); PREP_WG(8, false, true); PREP_WG(16, false, true);
 #undef PREP_WG
@@ -775,17 +788,17 @@ int launch_view_wg(const dyn_net* n, ViewFusedArgs& a, int V, cudaStream_t st) {
   if (grid == 0) return DYN_OK;
   ProfScope prof(st_net ? PROF_VIEW_ST : PROF_VIEW_DY, st);
   if (st_net && mc) {
-    if (VP == 8) view_wg_kernel<8, true, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, true, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    if (VP == 8) launch_view_wg_inst<8, true, true>(a, grid, st);
+    else launch_view_wg_inst<16, true, true>(a, grid, st);
   } else if (st_net) {
-    if (VP == 8) view_wg_kernel<8, true, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, true, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    if (VP == 8) launch_view_wg_inst<8, true, false>(a, grid, st);
+    else launch_view_wg_inst<16, true, false>(a, grid, st);
   } else if (mc) {
-    if (VP == 8) view_wg_kernel<8, false, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, false, true><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    if (VP == 8) launch_view_wg_inst<8, false, true>(a, grid, st);
+    else launch_view_wg_inst<16, false, true>(a, grid, st);
   } else {
-    if (VP == 8) view_wg_kernel<8, false, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
-    else view_wg_kernel<16, false, false><<<grid, kViewThreads, kWgSmem, st>>>(a);
+    if (VP == 8) launch_view_wg_inst<8, false, false>(a, grid, st);
+    else launch_view_wg_inst<16, false, false>(a, grid, st);
   }
   DYN_LAUNCH_CHECK();
   return DYN_OK;
