@@ -90,49 +90,98 @@ def static_bootstrap_loss(ret, ray_batch):
   return rgb_loss(pred, ray_batch, mask)
 
 
-def mono_step_loss(ret, ray_batch, args, epoch):
-  """train.py:300-456 -> (loss, dict of the scalars :458-464 logs plus cycle_loss and reg_loss)."""
+def step_denominators(ret, ray_batch, args, epoch):
+  """The quantities through which mono_step_loss couples rays: the normalisers of its terms and the counts of its
+  means.  Each is built from supervision, from masks or from forward values the loss detaches (occ_weight_map,
+  occ_weights, `ratio` in the static mask), so a ray-chunked evaluation computes them once over all rays and holds
+  them fixed (tests/train_step_ref.py).  The rgb and disparity normalisers are left live: with the reference's
+  detaches they carry no gradient, and a caller that removes one sees its effect."""
   ref, ref_dy = ret["outputs_coarse_ref"], ret["outputs_coarse_ref_dy"]
   anc, anc_dy = ret["outputs_coarse_anchor"], ret["outputs_coarse_anchor_dy"]
   dt = ref["rgb"].dtype
   sw = step_weights(args, epoch)
   motion = ray_batch["motion_mask"].to(dt)
   pred_mask = ref["mask"].to(dt)
-  # rgb, :304-328
-  rgb = criterion_rgb(ref, ray_batch) + temporal_rgb(anc, ray_batch)
+  R = pred_mask.shape[0]
+  sum_dy, sum_st = ref["weights_dy"].sum(-1), ref["weights_st"].sum(-1)
+  ratio = (sum_dy / torch.clamp(sum_dy + sum_st, min=1e-9)).detach()
+  smask = (1.0 - ray_batch["static_mask"].to(dt)) * pred_mask * (1.0 - ratio)
+  sf = anc["sf_seq"]
+  n, _, S, c = sf.shape
+  flow_m = (pred_mask[None, :, None] * ray_batch["masks"].to(dt)).expand(-1, -1, 2)
+  t_anc = anc["pts_traj_anchor"]
+  d = dict(
+      rgb_ref=pred_mask.sum() * 3 + 1e-6,  # charbonnier: mask.sum() * channels + 1e-6
+      rgb_anchor=(anc["mask"].to(dt) * anc["occ_weight_map"].to(dt)).sum() * 3 + 1e-8,
+      rgb_ref_dy=(ref_dy["mask"].to(dt) * motion).sum() * 3 + 1e-6,
+      rgb_anchor_dy=(anc_dy["mask"].to(dt) * motion * anc_dy["occ_weight_map"].to(dt)).sum() * 3 + 1e-8,
+      disp=pred_mask.sum() + 1e-8,
+      flow=flow_m.sum() + 1e-8,
+      cycle=anc["occ_weights"].to(dt).sum() * t_anc.shape[0] * t_anc.shape[-1] + 1e-8,
+      n_rays=float(R), n_sf=float(n * R * S * c), n_sf_time=float((n - 1) * R * S * c),
+      n_sf_space=float(n * R * (S - 1) * c),
+      static=smask.sum() * 3 + 1e-6)
   if sw["dynamic_rgb"]:
-    rgb = rgb + rgb_loss(ref["rgb_dy"], ray_batch, pred_mask * motion)
-  rgb = rgb + criterion_rgb(ref_dy, ray_batch, motion_mask=motion) * sw["dy_rgb"]
-  rgb = rgb + temporal_rgb(anc_dy, ray_batch, motion_mask=motion) * sw["dy_rgb"]
+    d["rgb_dynamic"] = (pred_mask * motion).sum() * 3 + 1e-6
+  if sw["static_dy"]:
+    d["static_dy"] = (smask * (ratio < 0.1).to(dt) + 1e-8).sum()
+  return d
+
+
+def mono_step_loss(ret, ray_batch, args, epoch, den=None):
+  """train.py:300-456 -> (loss, dict of the scalars :458-464 logs plus cycle_loss and reg_loss).
+
+  den: None, or step_denominators() of the whole batch when `ret` / `ray_batch` hold a chunk of its rays; the
+  chunks' losses then sum to the batch's loss and their gradients to its gradient."""
+  ref, ref_dy = ret["outputs_coarse_ref"], ret["outputs_coarse_ref_dy"]
+  anc, anc_dy = ret["outputs_coarse_anchor"], ret["outputs_coarse_anchor_dy"]
+  dt = ref["rgb"].dtype
+  sw = step_weights(args, epoch)
+  if den is None:
+    den = step_denominators(ret, ray_batch, args, epoch)
+  motion = ray_batch["motion_mask"].to(dt)
+  pred_mask = ref["mask"].to(dt)
+  gt = ray_batch["rgb"].to(dt)
+  charb = lambda x: torch.sqrt((x - gt) ** 2 + 0.001 ** 2)
+  # rgb, :304-328 (criterion_rgb, temporal_rgb, rgb_loss with the normalisers of `den`)
+  rgb = (charb(ref["rgb"]) * pred_mask[:, None]).sum() / den["rgb_ref"]
+  w_anc = anc["mask"].to(dt) * anc["occ_weight_map"].to(dt)
+  rgb = rgb + (charb(anc["rgb"]) * w_anc[:, None]).sum() / den["rgb_anchor"]
+  if sw["dynamic_rgb"]:
+    rgb = rgb + (charb(ref["rgb_dy"]) * (pred_mask * motion)[:, None]).sum() / den["rgb_dynamic"]
+  rgb = rgb + (charb(ref_dy["rgb"]) * (ref_dy["mask"].to(dt) * motion)[:, None]).sum() / den["rgb_ref_dy"] * sw["dy_rgb"]
+  w_anc_dy = anc_dy["mask"].to(dt) * motion * anc_dy["occ_weight_map"].to(dt)
+  rgb = rgb + (charb(anc_dy["rgb"]) * w_anc_dy[:, None]).sum() / den["rgb_anchor_dy"] * sw["dy_rgb"]
   # disparity, :331-342
   pred_disp = 1.0 / torch.clamp(ref["depth"], min=1e-2)
-  disp = sw["w_disp"] * ((pred_disp - ray_batch["disp"].to(dt)).abs() * pred_mask).sum() / (pred_mask.sum() + 1e-8)
+  disp = sw["w_disp"] * ((pred_disp - ray_batch["disp"].to(dt)).abs() * pred_mask).sum() / den["disp"]
   # flow, :345-351
-  flow = sw["w_flow"] * flow_l1(ref["render_flows"], ray_batch["flows"],
-                                pred_mask[None, :, None] * ray_batch["masks"].to(dt))
+  m = (pred_mask[None, :, None] * ray_batch["masks"].to(dt)).expand(-1, -1, 2)
+  flow = sw["w_flow"] * ((ref["render_flows"] - ray_batch["flows"].to(dt)).abs() * m).sum() / den["flow"]
   # trajectory cycle, :359-371
   t_ref, t_anc = anc["pts_traj_ref"], anc["pts_traj_anchor"]
   occ = anc["occ_weights"].to(dt)[None, ..., None].expand(t_anc.shape[0], -1, -1, t_anc.shape[-1])
-  cycle = sw["w_cycle"] * ((t_ref - t_anc).abs() * occ).sum() / (occ.sum() + 1e-8)
+  cycle = sw["w_cycle"] * ((t_ref - t_anc).abs() * occ).sum() / den["cycle"]
   # scene-flow regularisers, :374-397
   sf = anc["sf_seq"]
-  reg = args.w_reg * sf.abs().mean()
-  reg = reg + args.w_reg * 0.5 * ((sf[:-1] - sf[1:]) ** 2).mean()
-  reg = reg + args.w_reg * (sf[:, :, 1:] - sf[:, :, :-1]).abs().mean()
+  reg = args.w_reg * sf.abs().sum() / den["n_sf"]
+  reg = reg + args.w_reg * 0.5 * ((sf[:-1] - sf[1:]) ** 2).sum() / den["n_sf_time"]
+  reg = reg + args.w_reg * (sf[:, :, 1:] - sf[:, :, :-1]).abs().sum() / den["n_sf_space"]
   # weight entropy, :400-413
   sum_dy, sum_st = ref["weights_dy"].sum(-1), ref["weights_st"].sum(-1)
   ratio = sum_dy / torch.clamp(sum_dy + sum_st, min=1e-9)
   ent = -(ratio * torch.log(ratio + 1e-9) + (1.0 - ratio) * torch.log(1.0 - ratio + 1e-9))
-  ent = args.w_skew_entropy * ent.mean()
+  ent = args.w_skew_entropy * ent.sum() / den["n_rays"]
   # distortion, :416-423
   s = ref["s_vals"].to(dt)
-  dist = args.w_distortion * distortion(ref["weights"][:, :-1], (s[:, 1:] + s[:, :-1]) * 0.5, s[:, 1:] - s[:, :-1])
+  dist = args.w_distortion * distortion(ref["weights"][:, :-1], (s[:, 1:] + s[:, :-1]) * 0.5,
+                                        s[:, 1:] - s[:, :-1]) * (s.shape[0] / den["n_rays"])
   # adaptive static loss, :426-445
   smask = (1.0 - ray_batch["static_mask"].to(dt)) * pred_mask * (1.0 - ratio).detach()
-  static = rgb_loss(ref["rgb_static"], ray_batch, smask)
+  static = (charb(ref["rgb_static"]) * smask[:, None]).sum() / den["static"]
   if sw["static_dy"]:
     m2 = (smask * (ratio < 0.1).to(dt)).detach()
-    static = static + 0.1 * (sum_dy * m2).abs().sum() / (m2 + 1e-8).sum()
+    static = static + 0.1 * (sum_dy * m2).abs().sum() / den["static_dy"]
   loss = rgb + cycle + flow + disp + reg + ent + dist + static  # :447-456
   vals = (loss, flow, disp, rgb, dist, ent, static, cycle, reg)
   return loss, {k: v.detach() for k, v in zip(TERM_NAMES, vals)}

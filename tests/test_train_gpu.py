@@ -6,7 +6,10 @@ differentiable pieces (compute_traj_pts) and the whole
 Bar, precision "fp32": forward values rtol 2e-4; gradients 1e-3 relative in the L2 norm per tensor (fp32 kernels
 with a different summation order than ATen; ELU is C1, so there are no kink flips except the MotionMLP's ReLUs, see
 test_backward_gpu.py).  Precision "bf16" (tensor-core products with bf16 operands, everything else fp32): forward
-2e-2, gradients 5e-2 (matrices) / 1e-1 (vectors) against the same fp32 oracle."""
+2e-2, gradients 5e-2 (matrices) / 1e-1 (vectors) against the same fp32 oracle.
+
+The composed step at the shipped config's shape, with the real criterion instead of a random linear functional, every
+gradient against a float64 reference at per-tensor bars and planted glue errors, is tests/test_train_step_gpu.py."""
 
 import pytest
 import torch
