@@ -824,11 +824,14 @@ def _cat_slices(parts):
 
 
 def _keep_mask(S, dev):
-  """[1,S,1]: 0 on the last round(0.1 S) samples, whose motion coefficients the reference zeroes (:471-472)."""
+  """[1,S,1]: 0 on the last round(0.1 S) samples, whose motion coefficients the reference zeroes (:471-472).  When
+  that count is 0 the reference's slice `[:, -0:]` is the whole axis, so every sample is zeroed (as the forward kernel,
+  csrc/nets_f32.cu, does)."""
   keep = torch.ones(1, S, 1, device=dev)
   n_last = int(round(S * 0.1))
-  if n_last > 0:
-    keep[:, S - n_last:] = 0.0
+  if n_last <= 0:
+    n_last = S
+  keep[:, S - n_last:] = 0.0
   return keep
 
 

@@ -894,6 +894,37 @@ def resample(case, plant=None):
   return dict(fine=ref, lo=lo, hi=hi, sens=sens, kink=kink, merged=merged, above=above0)
 
 
+def resample_check(case, ref, out):
+  """The kernel's merged depths `out` [R, S + Ni] against `resample(case)`: -> (rows whose coarse depths are not all
+  present bit for bit or whose fine samples leave the [lo - bar, hi + bar] intervals, the worst excess over the rays'
+  kink-free samples)."""
+  b_lo = bar("resample", ref["lo"], ref["lo"].abs(), ref["sens"])
+  b_hi = bar("resample", ref["hi"], ref["hi"].abs(), ref["sens"])
+  bad, worst = [], -1e30
+  for r in range(case["R"]):
+    row = out[r].tolist()
+    try:
+      for v in case["z"][r].tolist():  # every coarse depth appears bit for bit
+        row.remove(v)
+    except ValueError:
+      bad.append(r)
+      continue
+    fine = d64(torch.tensor(row, dtype=torch.float32))
+    if not (torch.isfinite(fine).all() and torch.isfinite(ref["lo"][r]).all() and torch.isfinite(ref["hi"][r]).all()):
+      bad.append(r)
+      continue
+    lo = torch.sort(ref["lo"][r] - b_lo[r]).values
+    hi = torch.sort(ref["hi"][r] + b_hi[r]).values
+    if not ((fine >= lo) & (fine <= hi)).all():
+      bad.append(r)
+    clean = ~ref["kink"][r]
+    if clean.any():
+      srt, m = torch.sort(ref["fine"][r])
+      ex = excess("resample", fine, srt, srt.abs(), ref["sens"][r][m])
+      worst = max(worst, torch.nan_to_num(ex[clean[m]], nan=float("inf")).max().item())
+  return bad, worst
+
+
 def resample_oracle(case):
   with float64():
     return O.resample_depths(d64(case["z"]), d64(case["weights"]), case["Ni"], case["inv_uniform"],

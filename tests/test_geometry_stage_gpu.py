@@ -310,8 +310,6 @@ def test_resample(S, Ni, inv_uniform, det):
   out = rr.resample_depths(case["z"].to(DEV), case["weights"].to(DEV), Ni, inv_uniform, det, u).cpu()
   tag = "S%d_Ni%d_inv%d_%s" % (S, Ni, inv_uniform, "det" if det else "u")
   assert (out[:, 1:] >= out[:, :-1]).all(), tag
-  b_lo = G.bar("resample", ref["lo"], ref["lo"].abs(), ref["sens"])
-  b_hi = G.bar("resample", ref["hi"], ref["hi"].abs(), ref["sens"])
   n_kink = int(ref["kink"].sum())
   M = S - 2
   if det:
@@ -326,22 +324,6 @@ def test_resample(S, Ni, inv_uniform, det):
   # within rounding of one with probability ~ 1e-3 at M = 126 (about one expected over 3 rays x 384 u)
   allowed += 3
   assert n_kink <= allowed, (tag, n_kink, allowed)
-  worst = -1e30
-  for r in range(R):
-    row = out[r].tolist()
-    for v in case["z"][r].tolist():  # every coarse depth appears bit for bit
-      row.remove(v)
-    fine = G.d64(torch.tensor(row, dtype=torch.float32))
-    assert torch.isfinite(fine).all() and torch.isfinite(ref["lo"][r]).all() and torch.isfinite(ref["hi"][r]).all(), (
-        tag, r)
-    lo = torch.sort(ref["lo"][r] - b_lo[r]).values
-    hi = torch.sort(ref["hi"][r] + b_hi[r]).values
-    bad = ~((fine >= lo) & (fine <= hi))
-    assert not bad.any(), (tag, r, bad.nonzero().flatten().tolist()[:5], fine[bad][:3], lo[bad][:3], hi[bad][:3])
-    clean = ~ref["kink"][r]
-    if clean.any():
-      srt = torch.sort(ref["fine"][r]).values
-      m = torch.sort(ref["fine"][r]).indices
-      ex = G.excess("resample", fine, srt, srt.abs(), ref["sens"][r][m])
-      worst = max(worst, torch.nan_to_num(ex[clean[m]], nan=float("inf")).max().item())
+  bad, worst = G.resample_check(case, ref, out)
+  assert not bad, (tag, bad)
   _WORST["resample"] = max(_WORST.get("resample", -1e30), worst)

@@ -173,14 +173,22 @@ _TRAIN_KEYS = {
 }
 
 
-@pytest.mark.parametrize("name,prec", [("mono_train", "fp32"), ("mono_train_near", "fp32"), ("mono_train", "bf16")])
+_STEP_CONFIGS = dict(
+    scenes.GOLDEN_CONFIGS,
+    # 5 samples: int(round(0.5)) = 0, and the reference's `[:, -0:]` zeroes the motion coefficients of every sample
+    mono_train_short=dict(scenes.GOLDEN_CONFIGS["mono_train"], N_samples=5),
+)
+
+
+@pytest.mark.parametrize("name,prec", [("mono_train", "fp32"), ("mono_train_near", "fp32"), ("mono_train", "bf16"),
+                                       ("mono_train_short", "fp32")])
 def test_render_rays_mono_training_step_matches_oracle_autograd(name, prec):
   """The whole differentiable path: loss = sum of randomly weighted differentiable outputs of
   render_rays_mono(is_train=True); d loss / d (every parameter of motion_mlp, net_coarse_dy, net_coarse_st and the
   three feature maps) against torch autograd through the oracle."""
   from dynibar_b200 import render_ray as rr
   from dynibar_b200.projection import Projector
-  cfg = dict(scenes.GOLDEN_CONFIGS[name])
+  cfg = dict(_STEP_CONFIGS[name])
   if prec == "bf16":
     cfg["rays"] = 96  # >= 2048 (point, view) rows per product: the tensor-core kernels take over
   batch, feat_c, _, frame, t, offs, model, args = scenes.build(cfg)
@@ -234,7 +242,10 @@ def test_render_rays_mono_training_step_matches_oracle_autograd(name, prec):
       # to ~1e-3 of their magnitude (e.g. the blending head: sum_v d logit_v = 0 per point), so the summation order
       # shows; a wrong or missing term is an O(1) error
       if prec == "fp32":
-        _close("%s.%s" % (mname, k), p.grad, w[k].grad, 5e-3 if p.dim() > 1 else 2e-2)
+        # 5 samples: sums that cancel (vis_fc2.2's bias) over 100 points are ~3e-5, so fp32 rounding of either side
+        # reaches the 1e-6 floor; what this case is for is the zeroed motion (every coefficient 0 on both sides)
+        _close("%s.%s" % (mname, k), p.grad, w[k].grad, 5e-3 if p.dim() > 1 else 2e-2,
+               floor=1e-5 if name == "mono_train_short" else 1e-6)
       elif mname == "motion_mlp" and k.startswith("pts_linears"):
         # ReLU network with bf16 products: pre-activations within bf16 rounding of 0 (~0.3 % of the units per layer)
         # take the other side of the kink, each flip is an O(1) change of that unit's gradient -> sqrt(0.003) ~ 5 %

@@ -2,7 +2,10 @@
 oracle: the fine pass of render_rays_mv (fine_render_rays, render_ray.py:407-597) with its coarse pass under no_grad
 (:672), trajectory_basis / trajectory_basis_fine as trainable tensors (ibrnet/model.py:94-118, :331-351), and the two
 kernels that make them differentiable: the basis-row gradient of traj_combine and the expected scene flow
-(:585-595).  Bars: those of test_train_gpu.py."""
+(:585-595).  Bars: those of test_train_gpu.py.
+
+The fine-stage step at the Nvidia benchmark shape, with a stand-in loss, every gradient against a float64 reference at
+per-tensor bars and planted glue errors, is tests/test_train_mv_step_gpu.py."""
 
 import pytest
 import torch

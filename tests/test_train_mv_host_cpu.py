@@ -32,6 +32,21 @@ def test_basis_rows_match_the_reference_rows_and_carry_the_gradient():
     rr._basis_rows(live, [(24, 0)], "cpu")
 
 
+@pytest.mark.parametrize("S", [1, 2, 3, 4, 5, 6, 15, 25, 35, 45])
+def test_keep_mask_zeroes_the_reference_tail(S):
+  """The training paths' zeroed tail is the reference's `[:, -n:]` with n = int(round(0.1 S)): all S samples when n is
+  0 (S <= 5, `-0:` is the whole axis), and Python's round-half-even at S = 25 (2) and 35 (4)."""
+  import motion_stage_ref
+  keep = rr._keep_mask(S, "cpu")
+  n = motion_stage_ref.n_last(S)
+  want = torch.ones(1, S, 1)
+  want[:, S - n:] = 0.0
+  assert torch.equal(keep, want), (S, keep.flatten().tolist())
+  ref = torch.ones(1, S, 1)
+  ref[:, -int(round(S * 0.1)):] *= 0.0  # the reference's own slice, ibrnet/render_ray.py:459, :472
+  assert torch.equal(keep, ref)
+
+
 def _mv_model():
   model, args = synthetic.make_model(8, 8, num_frames=24)
   return model, args

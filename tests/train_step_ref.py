@@ -94,13 +94,7 @@ def make_case(name):
       H=c["H"], W=c["W"], V_dy=c["V_dy"], V_st=c["V_st"], num_vv=c["num_vv"], seed=c["seed"], rays=c["rays"],
       frame_idx=c["frame_idx"], anchor_offset=c["anchor_offset"])
   if c["edge_rays"]:
-    batch["static_src_cameras"][0, :, 18 + 3] *= 6.0  # baseline 0.48: pooling weights e_v - min e well above 0
-    K = batch["camera"][0, 2:18].reshape(4, 4)[:3, :3]
-    uv = torch.tensor([[u, 0.25 * c["H"] + 3.0 * i] for i, u in enumerate(_EDGE_U)])
-    d = torch.cat([uv, torch.ones(len(_EDGE_U), 1)], 1) @ torch.inverse(K).t()
-    batch["ray_o"] = torch.cat([batch["ray_o"], torch.zeros(len(_EDGE_U), 3)])
-    batch["ray_d"] = torch.cat([batch["ray_d"], d])
-    batch["uv_grid"] = torch.cat([batch["uv_grid"], uv])
+    add_edge_rays(batch, c["H"])
   args = synthetic.make_args(c["aa"], c["mrgb"], c["occ"])
   model, args = synthetic.make_model(c["S"], 0, args=args, seed=c["seed"], mono=True)
   args = SimpleNamespace(**dict(vars(args), **LOSS_ARGS))
@@ -116,6 +110,17 @@ def make_case(name):
   c.update(batch=batch, featmaps=feat, frame=frame, t=t, offs=offs, model=model, args=args, sup=sup,
            jitter=torch.rand(R, c["S"], generator=g))
   return c
+
+
+def add_edge_rays(batch, H):
+  """Widens the static rig and appends the rays of _EDGE_U to `batch`, in place."""
+  batch["static_src_cameras"][0, :, 18 + 3] *= 6.0  # baseline 0.48: pooling weights e_v - min e well above 0
+  K = batch["camera"][0, 2:18].reshape(4, 4)[:3, :3]
+  uv = torch.tensor([[u, 0.25 * H + 3.0 * i] for i, u in enumerate(_EDGE_U)])
+  d = torch.cat([uv, torch.ones(len(_EDGE_U), 1)], 1) @ torch.inverse(K).t()
+  batch["ray_o"] = torch.cat([batch["ray_o"], torch.zeros(len(_EDGE_U), 3)])
+  batch["ray_d"] = torch.cat([batch["ray_d"], d])
+  batch["uv_grid"] = torch.cat([batch["uv_grid"], uv])
 
 
 def view_counts(c):
@@ -326,7 +331,8 @@ def _companion(name, V_st):
   """Gradients whose terms cancel are measured against the weight gradient of the same layer
   (train_stage_ref.companion)."""
   net, _, k = name.partition(".")
-  kind = {"net_coarse_dy": "dynamic", "net_coarse_st": "static"}.get(net)
+  kind = {"net_coarse_dy": "dynamic", "net_coarse_st": "static", "net_fine_dy": "dynamic",
+          "net_fine_st": "static"}.get(net)
   cn = tsr.companion(kind, k, V_st) if kind else None
   return "%s.%s" % (net, cn) if cn else None
 
