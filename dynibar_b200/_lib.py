@@ -59,6 +59,11 @@ class Scene(C.Structure):
               [(k, _i) for k in ("N", "H", "W", "mc", "flow_base", "NF")])
 
 
+# ---- a device-resident Nvidia scene (include/dynibar_b200.h: dyn_nvi_scene_t) ------------------------------------
+class NviScene(C.Structure):
+  _fields_ = [(k, _vp) for k in ("frames", "smask", "gt", "dmask")] + [(k, _i) for k in ("N", "H", "W", "T", "S")]
+
+
 # name -> (restype, argtypes); mirrors include/dynibar_b200.h one to one
 SIGNATURES = {
     "dyn_version": (_i, []),
@@ -166,6 +171,10 @@ SIGNATURES = {
     "dyn_scene_masks": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dyn_scene_views": (_i, [C.POINTER(Scene), _vp, _i, _vp, _i, _vp, _i, _vp, _i] + [_vp] * 7),
     "dyn_scene_rays": (_i, [C.POINTER(Scene), _vp, _vp, _vp, _i] + [_vp] * 9 + [_vp]),
+    "dyn_area_resize": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "dyn_nearest_resize": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "dyn_nvi_time_step": (_i, [C.POINTER(NviScene), _vp, _i, _i, _i] + [_vp] * 6 + [_vp]),
+    "dyn_nvi_rays": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -12,6 +12,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "scene_common.cuh"
 
 namespace dyn {
 namespace {
@@ -21,12 +22,6 @@ constexpr int kTileW = 32, kTileH = 16;  // erosion output tile
 constexpr int kThreads = 256;
 constexpr int kStacks = 3;
 constexpr int kMaxTableViews = 3 * kMaxViews;
-
-// cv2 resizeNN (INTER_NEAREST): src index of dst index x = min(floor(x * (1 / (dst / src))), src - 1), in double
-__device__ __forceinline__ int nn_index(int x, int dst, int src) {
-  const double ifx = 1.0 / ((double)dst / (double)src);
-  return min((int)floor((double)x * ifx), src - 1);
-}
 
 // scipy.ndimage mode 'reflect' (d c b a | a b c d), periodic with period 2n for offsets beyond the image
 __device__ __forceinline__ int reflect(int i, int n) {
@@ -89,8 +84,6 @@ __global__ void __launch_bounds__(kThreads) frame_masks_kernel(const uint8_t* __
   for (int c = 0; c < mc; ++c) srcmask[o * mc + c] = m[c];
 }
 
-__device__ __forceinline__ float u8f(uint8_t v) { return __fdiv_rn((float)v, 255.0f); }
-
 struct Stacks {
   float* out[kStacks];
   int views[kStacks];
@@ -150,8 +143,8 @@ __global__ void __launch_bounds__(kThreads) views_kernel(dyn_scene_t s, const in
   }
 }
 
-// One thread per ray.  cam (device) = M [3x3 row-major] | t [3] with M = R_c2w K^-1 formed on the host in float32
-// (sample_ray.py:154-158); ray_d = M [u, v, 1]^T summed left to right, ray_o = t.  sel == NULL: ray i is pixel i.
+// One thread per ray (pixel_ray: cam = M | t, M = R_c2w K^-1 formed on the host in float32).  sel == NULL: ray i is
+// pixel i.
 // Supervision pointers may be NULL (get_all: rays only).
 __global__ void __launch_bounds__(kThreads) rays_kernel(dyn_scene_t s, const float* __restrict__ cam,
                                                         const int* __restrict__ target, const int* __restrict__ sel,
@@ -163,11 +156,7 @@ __global__ void __launch_bounds__(kThreads) rays_kernel(dyn_scene_t s, const flo
   const int p = sel ? sel[i] : i;
   if (p < 0 || p >= HW) return;
   const float u = (float)(p % s.W), v = (float)(p / s.W);
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    ray_d[3 * i + a] = __fadd_rn(__fadd_rn(__fmul_rn(cam[3 * a], u), __fmul_rn(cam[3 * a + 1], v)), cam[3 * a + 2]);
-    ray_o[3 * i + a] = cam[9 + a];
-  }
+  pixel_ray(cam, u, v, ray_o + 3 * i, ray_d + 3 * i);
   uv[2 * i] = u;
   uv[2 * i + 1] = v;
   if (tg.rgb == nullptr) return;

@@ -697,6 +697,39 @@ int dyn_scene_rays(const dyn_scene_t* scene, const float* cam, const int* target
                    float* ray_d, float* uv_grid, float* rgb, float* disp, float* motion_mask, float* static_mask,
                    float* flows, float* masks, void* stream);
 
+/* ---- an Nvidia-benchmark scene resident on the device (DESIGN §3.8; csrc/nvi_scene.cu) -----------------------------
+ * eval_nvidia.py's DynamicVideoDataset.__getitem__ (:71-198) and its ground-truth / mask reads (:383-428) on a scene
+ * uploaded once.  No float atomics, no host synchronisation: the same inputs give the same bits. */
+/* cv2.resize(INTER_AREA) of N uint8 images src [N,sh,sw,C] -> dst [N,dh,dw,C], C 1..4, downscaling only (sh >= dh,
+ * sw >= dw).  Integer factors in both axes: the integer box sum s of a = fy fx pixels, (s + 2) >> 2 at 2 x 2, else
+ * s * (1.f / a) in float32 rounded to nearest even.  Any other factor: OpenCV's area tables in double (alpha as
+ * float32, slivers <= 1e-3 dropped), horizontal then vertical weights in table order, float32 products and sums
+ * without contraction, rounded to nearest even.  One launch, one 32 x 8 output tile per CTA. */
+int dyn_area_resize(const uint8_t* src, int N, int sh, int sw, int C, int dh, int dw, uint8_t* dst, void* stream);
+/* cv2.resize(INTER_NEAREST) of N uint8 images [N,sh,sw,C] -> [N,dh,dw,C] (resizeNN's index rule, dyn_scene_masks);
+ * threshold != 0 writes (value > 0) as 0 / 1, which equals thresholding at > 1e-3 before the resize. */
+int dyn_nearest_resize(const uint8_t* src, int N, int sh, int sw, int C, int dh, int dw, int threshold, uint8_t* dst,
+                       void* stream);
+typedef struct {
+  const uint8_t* frames; /* [N,H,W,3] images_WxH */
+  const uint8_t* smask;  /* [N,H,W] coarse static masks at frame size, raw values (255 where none applies) */
+  const uint8_t* gt;     /* [T*S,H,W,3] ground truth resized to the render size */
+  const uint8_t* dmask;  /* [T*S,H,W,3] dynamic masks at the render size, 0 / 1, BGR channel order */
+  int N, H, W, T, S;
+} dyn_nvi_scene_t;
+/* One time step, one launch.  table (device) int32 [nd + ns + K]: nd dynamic source frames, ns static source frames,
+ * K ground-truth rows (t * S + s).  Writes src_rgbs [nd,H,W,3], static_src_rgbs [ns,H,W,3] as u8 / 255.0f,
+ * static_src_masks [ns,H,W] = smask / 255.0f, static_masked [ns,H,W,3] = static_src_rgbs * mask (__fmul_rn),
+ * gt [K,H,W,3] = u8 / 255.0f and dynamic_mask [K,H,W,3] (0 / 1), all fp32. */
+int dyn_nvi_time_step(const dyn_nvi_scene_t* scene, const int* table, int nd, int ns, int K, float* src_rgbs,
+                      float* static_src_rgbs, float* static_src_masks, float* static_masked, float* gt,
+                      float* dynamic_mask, void* stream);
+/* Every pixel's ray of K <= 16 target cameras of H x W, one launch: cams (device) fp32 [K,12] = M | t per camera
+ * (dyn_scene_rays); ray k H W + p is camera k's pixel p: ray_o, ray_d [K H W,3], uv_grid [K H W,2],
+ * camera_index int32 [K H W] = k. */
+int dyn_nvi_rays(const float* cams, int K, int H, int W, float* ray_o, float* ray_d, float* uv_grid, int* camera_index,
+                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif
