@@ -479,7 +479,10 @@ __device__ __forceinline__ void attend(const uint32_t (&qf)[8][4], uint32_t (&of
                                        const float* sc, const int* lo, int S) {
   constexpr int NL = KEYS / 2, KG = KEYS * 16;
   const int q = threadIdx.x & 3;
-  const bool part = S < KEYS;
+  // rows attend to part of the key tile only at KEYS = 64 (S < 64); KEYS = 128 runs S = 128 alone.  Known at compile
+  // time, the masks and their key indices cost no registers in the 128-key instantiations, which keeps ptxas from
+  // spilling and serializing their wgmmas (C7511).
+  const bool part = KEYS == 64 && S < KEYS;
 #pragma unroll
   for (int hd = 0; hd < 4; ++hd) {
     float lg[NL];
