@@ -147,6 +147,8 @@ SIGNATURES = {
     "dyn_mono_loss": (_i, [C.POINTER(MonoLossInputs), C.POINTER(MonoLossWeights), _vp, _vp, _sz, _vp]),
     "dyn_mono_loss_backward": (_i, [C.POINTER(MonoLossInputs), C.POINTER(MonoLossWeights), _vp, _vp,
                                     C.POINTER(MonoLossGrads), _vp]),
+    "dyn_mono_loss_rows": (_i, [C.POINTER(MonoLossInputs), C.POINTER(MonoLossWeights), _vp, _i, _vp]),
+    "dyn_mono_loss_finish": (_i, [_vp, _i, C.POINTER(MonoLossWeights), _i, _i, _i, _i, _vp, _vp]),
     "dyn_debug_tc_grad_w": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "dyn_debug_tc_grad_in": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _i, _vp, _sz, _vp]),
     "dyn_debug_tc_grad_in_scratch_bytes": (_sz, []),

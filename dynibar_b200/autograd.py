@@ -21,6 +21,8 @@ of the path, so that `render_ray.render_rays_mono(..., is_train=True)` is differ
   * `expected_scene_flow`  exp_sf of the mv fine pass (render_ray.py:585-595).
   * `mono_loss`         the criterion of a DynibarMono step (train.py:187-196, :300-456): every loss term in one
                         forward and one backward call (csrc/loss.cu); dynibar_b200/criterion.py is its interface.
+                        `mono_loss_rows` / `mono_loss_finish` are its two forward passes as separate calls, for a
+                        batch evaluated in ray slices (dynibar_b200/train_step.py).
 
 tests/test_backward_gpu.py and tests/test_train_gpu.py check them -- and the whole training forward/backward --
 against torch autograd through the oracle's restatement of the same functions.
@@ -456,50 +458,65 @@ def _rows(A, t, width):
   return c.data_ptr(), c.stride(0)
 
 
+def _loss_inputs(weights, fixed, x):
+  """(Args keeping the tensors alive, dyn_mono_loss_inputs) of one criterion call; x: {name of _LOSS_INPUTS: tensor}.
+  Tensors sliced along a ray axis other than the first ([n, R, ...] inputs of a ray slice) are copied contiguous, so
+  that in.R is the stride of every [n, R, ...] input."""
+  from dynibar_b200 import _lib
+  A, inp = Args(), _lib.MonoLossInputs()
+  inp.R, inp.S = int(fixed["R"]), int(fixed["S"])
+  on = lambda k: (weights.terms >> k) & 1
+  for k in range(_lib.LOSS_RGB_SLOTS):
+    slot = fixed.get("slot%d" % k)
+    if slot is None:
+      continue
+    sl = inp.rgb[k]
+    if x["rgb%d" % k] is not None:
+      sl.pred, sl.ld = _rows(A, x["rgb%d" % k], 3)
+    sl.mask, sl.w0, sl.w1, sl.flags = A(slot.get("mask"), torch.bool), A(slot.get("w0")), A(slot.get("w1")), \
+        int(slot.get("flags", 0))
+  inp.gt_rgb = A(fixed.get("gt_rgb"))
+  if on(6):
+    inp.depth, inp.depth_ld = _rows(A, x["depth"], 1)
+    inp.gt_disp = A(fixed["gt_disp"])
+  inp.ray_mask = A(fixed.get("ray_mask"), torch.bool)
+  if on(7):
+    inp.flows, inp.gt_flows, inp.flow_masks = A(x["flows"]), A(fixed["gt_flows"]), A(fixed["flow_masks"])
+    inp.n_flow = int(x["flows"].shape[0])
+  if on(8):
+    inp.traj_ref, inp.traj_anchor, inp.occ_weights = A(x["traj_ref"]), A(x["traj_anchor"]), A(fixed["occ_weights"])
+    inp.K = int(x["traj_ref"].shape[0])
+  if on(9) or on(10) or on(11):
+    inp.sf_seq, inp.n_sf = A(x["sf_seq"]), int(x["sf_seq"].shape[0])
+  inp.weights_dy, inp.weights_st = A(x["weights_dy"]), A(x["weights_st"])
+  if on(13):
+    inp.dist_w, inp.dist_ld, inp.dist_n = A(x["weights"]), int(x["weights"].shape[1]), int(fixed["dist_n"])
+    inp.s_vals, inp.dist_m, inp.dist_interval = A(fixed.get("s_vals")), A(fixed.get("dist_m")), \
+        A(fixed.get("dist_interval"))
+  if not A.keep:
+    raise ValueError("dynibar_b200: the criterion was given no tensor")
+  return A, inp
+
+
 class _MonoLoss(torch.autograd.Function):
   @staticmethod
   def forward(ctx, weights, fixed, *diff):
     from dynibar_b200 import _lib
-    x = dict(zip(_LOSS_INPUTS, diff))
-    R, S = int(fixed["R"]), int(fixed["S"])
-    A, inp = Args(), _lib.MonoLossInputs()
-    inp.R, inp.S = R, S
-    on = lambda k: (weights.terms >> k) & 1
-    for k in range(_lib.LOSS_RGB_SLOTS):
-      slot = fixed.get("slot%d" % k)
-      if slot is None:
-        continue
-      sl = inp.rgb[k]
-      if x["rgb%d" % k] is not None:
-        sl.pred, sl.ld = _rows(A, x["rgb%d" % k], 3)
-      sl.mask, sl.w0, sl.w1, sl.flags = A(slot.get("mask"), torch.bool), A(slot.get("w0")), A(slot.get("w1")), \
-          int(slot.get("flags", 0))
-    inp.gt_rgb = A(fixed.get("gt_rgb"))
-    if on(6):
-      inp.depth, inp.depth_ld = _rows(A, x["depth"], 1)
-      inp.gt_disp = A(fixed["gt_disp"])
-    inp.ray_mask = A(fixed.get("ray_mask"), torch.bool)
-    if on(7):
-      inp.flows, inp.gt_flows, inp.flow_masks = A(x["flows"]), A(fixed["gt_flows"]), A(fixed["flow_masks"])
-      inp.n_flow = int(x["flows"].shape[0])
-    if on(8):
-      inp.traj_ref, inp.traj_anchor, inp.occ_weights = A(x["traj_ref"]), A(x["traj_anchor"]), A(fixed["occ_weights"])
-      inp.K = int(x["traj_ref"].shape[0])
-    if on(9) or on(10) or on(11):
-      inp.sf_seq, inp.n_sf = A(x["sf_seq"]), int(x["sf_seq"].shape[0])
-    inp.weights_dy, inp.weights_st = A(x["weights_dy"]), A(x["weights_st"])
-    if on(13):
-      inp.dist_w, inp.dist_ld, inp.dist_n = A(x["weights"]), int(x["weights"].shape[1]), int(fixed["dist_n"])
-      inp.s_vals, inp.dist_m, inp.dist_interval = A(fixed.get("s_vals")), A(fixed.get("dist_m")), \
-          A(fixed.get("dist_interval"))
-    if not A.keep:
-      raise ValueError("dynibar_b200: the criterion was given no tensor")
+    A, inp = _loss_inputs(weights, fixed, dict(zip(_LOSS_INPUTS, diff)))
     dev = dev_of(A.keep[0])
-    out = torch.empty(_lib.LOSS_OUT_FLOATS, device=dev)
-    nbytes = int(lib.dyn_mono_loss_workspace_bytes(R))
-    ws = _lib.workspace.get(nbytes, dev, slot=5)
-    with torch.cuda.device(dev):
-      check(lib.dyn_mono_loss(ctypes.byref(inp), ctypes.byref(weights), ptr(out), ws.data_ptr(), nbytes, stream()))
+    table = fixed.get("table")
+    if table is None:
+      out = torch.empty(_lib.LOSS_OUT_FLOATS, device=dev)
+      nbytes = int(lib.dyn_mono_loss_workspace_bytes(inp.R))
+      ws = _lib.workspace.get(nbytes, dev, slot=5)
+      with torch.cuda.device(dev):
+        check(lib.dyn_mono_loss(ctypes.byref(inp), ctypes.byref(weights), ptr(out), ws.data_ptr(), nbytes, stream()))
+    else:  # a ray slice of a batch: the batch's table, written by mono_loss_finish
+      if table.shape != (_lib.LOSS_OUT_FLOATS,):
+        raise ValueError("mono_loss: the batch table has shape %s, [%d] expected" % (tuple(table.shape),
+                                                                                      _lib.LOSS_OUT_FLOATS))
+      out = table.detach().clone()
+      ptr(out)
     ctx.inp, ctx.weights, ctx.keep, ctx.out = inp, weights, A, out
     ctx.shapes = [(None if t is None else (t.shape, t.dtype)) for t in diff]
     return out
@@ -527,13 +544,54 @@ class _MonoLoss(torch.autograd.Function):
     return (None, None) + tuple(grads)
 
 
+def _check_names(inputs):
+  unknown = set(inputs) - set(_LOSS_INPUTS)
+  if unknown:
+    raise TypeError("mono_loss: unknown inputs %s" % sorted(unknown))
+
+
 def mono_loss(term_weights, fixed, **inputs):
   """The criterion kernels (csrc/loss.cu) as one differentiable call -> out [40] (include/dynibar_b200.h,
   dyn_mono_loss): out[0] is the loss and the only differentiable element; out[1:9] are the logged scalars, out[9:24]
   the unweighted components.  `term_weights`: a `_lib.MonoLossWeights`; `fixed`: R, S and the tensors that carry no
   gradient (supervision, masks, occ_weights, s_vals; "slot<k>" = dict(mask, w0, w1, flags) of rgb slot k); `inputs`:
-  the differentiable tensors by the names of `_LOSS_INPUTS` (absent = None)."""
-  unknown = set(inputs) - set(_LOSS_INPUTS)
-  if unknown:
-    raise TypeError("mono_loss: unknown inputs %s" % sorted(unknown))
+  the differentiable tensors by the names of `_LOSS_INPUTS` (absent = None).
+
+  With fixed["table"] (the [40] output of mono_loss_finish for a whole batch) the inputs are one ray slice of that
+  batch: nothing is computed forward, the call returns a copy of the table, and its backward is the slice's share of
+  d(batch loss) / d(inputs) -- dyn_mono_loss_backward on the slice against the batch's denominators."""
+  _check_names(inputs)
   return _MonoLoss.apply(term_weights, fixed, *[inputs.get(k) for k in _LOSS_INPUTS])
+
+
+def mono_loss_rows(term_weights, fixed, partial, first_ray, **inputs):
+  """Pass 1 of the criterion over one ray slice (dyn_mono_loss_rows): the slice starting at ray `first_ray` of its
+  batch (a multiple of 8) writes its rows into `partial`, a uint8 device buffer of
+  dyn_mono_loss_workspace_bytes(R_batch) bytes.  Same arguments as `mono_loss`, no gradient.  -> (S, K, n_sf), the
+  dimensions mono_loss_finish takes with the batch's R."""
+  _check_names(inputs)
+  if first_ray % 8:
+    raise ValueError("mono_loss_rows: a slice starts on a multiple of 8 rays, got %d" % first_ray)
+  A, inp = _loss_inputs(term_weights, fixed, {k: inputs.get(k) for k in _LOSS_INPUTS})
+  need = int(lib.dyn_mono_loss_workspace_bytes(first_ray + inp.R))
+  if partial.dtype != torch.uint8 or partial.numel() < need:
+    raise ValueError("mono_loss_rows: rows up to ray %d need a uint8 buffer of %d bytes" % (first_ray + inp.R, need))
+  with torch.cuda.device(dev_of(partial)):
+    check(lib.dyn_mono_loss_rows(ctypes.byref(inp), ctypes.byref(term_weights), ptr(partial, torch.uint8),
+                                 first_ray // 8, stream()))
+  return inp.S, inp.K, inp.n_sf
+
+
+def mono_loss_finish(partial, term_weights, R, S, K, n_sf):
+  """Pass 2 of the criterion for a batch of R rays whose rows mono_loss_rows wrote into `partial` -> out [40], the
+  same floats `mono_loss` returns for the whole batch (not differentiable)."""
+  from dynibar_b200 import _lib
+  nblocks = (int(R) + 7) // 8
+  if partial.dtype != torch.uint8 or partial.numel() < int(lib.dyn_mono_loss_workspace_bytes(int(R))):
+    raise ValueError("mono_loss_finish: the rows of %d rays need %d bytes" %
+                     (R, int(lib.dyn_mono_loss_workspace_bytes(int(R)))))
+  out = torch.empty(_lib.LOSS_OUT_FLOATS, device=dev_of(partial))
+  with torch.cuda.device(out.device):
+    check(lib.dyn_mono_loss_finish(ptr(partial, torch.uint8), nblocks, ctypes.byref(term_weights), int(R), int(S),
+                                   int(K), int(n_sf), ptr(out), stream()))
+  return out

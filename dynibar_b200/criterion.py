@@ -85,6 +85,12 @@ def mono_step_loss(ret, ray_batch, args, epoch):
 def mono_step_table(ret, ray_batch, args, epoch):
   """Everything the forward kernels write for a step, one [40] device tensor: [0:9] the scalars of TERM_NAMES (element 0,
   the loss, is the differentiable one), [COMPONENTS + k] term k before its weight (k: the indices above)."""
+  wt, fixed, inputs = _step_call(ret, ray_batch, args, epoch)
+  return ag.mono_loss(wt, fixed, **inputs)
+
+
+def _step_call(ret, ray_batch, args, epoch):
+  """(weights, fixed, differentiable inputs) of the criterion call of a step (train.py:300-456)."""
   ref, ref_dy = ret["outputs_coarse_ref"], ret["outputs_coarse_ref_dy"]
   anc, anc_dy = ret["outputs_coarse_anchor"], ret["outputs_coarse_anchor_dy"]
   wt = step_weights(args, epoch)
@@ -106,8 +112,8 @@ def mono_step_table(ret, ray_batch, args, epoch):
       "gt_flows": ray_batch["flows"], "flow_masks": ray_batch["masks"],
       "occ_weights": anc["occ_weights"], "s_vals": ref["s_vals"], "dist_n": S - 1,
   }
-  return ag.mono_loss(
-      wt, fixed, rgb0=ref["rgb"], rgb1=anc["rgb"], rgb2=ref["rgb_dy"] if (wt.terms >> RGB_DYNAMIC) & 1 else None,
+  return wt, fixed, dict(
+      rgb0=ref["rgb"], rgb1=anc["rgb"], rgb2=ref["rgb_dy"] if (wt.terms >> RGB_DYNAMIC) & 1 else None,
       rgb3=ref_dy["rgb"], rgb4=anc_dy["rgb"], rgb5=ref["rgb_static"], depth=ref["depth"], flows=ref["render_flows"],
       weights=ref["weights"], weights_dy=ref["weights_dy"], weights_st=ref["weights_st"],
       traj_ref=anc["pts_traj_ref"], traj_anchor=anc["pts_traj_anchor"], sf_seq=anc["sf_seq"])
@@ -116,15 +122,53 @@ def mono_step_table(ret, ray_batch, args, epoch):
 def static_bootstrap_loss(ret, ray_batch):
   """The loss of the static warm-up (train.py:187-196): Charbonnier of outputs_coarse_st['rgb'] under
   (1 - static_mask) * outputs_coarse_ref['mask']."""
+  wt, fixed, inputs = _bootstrap_call(ret, ray_batch)
+  return ag.mono_loss(wt, fixed, **inputs)[0]
+
+
+def _bootstrap_call(ret, ray_batch):
   pred = ret["outputs_coarse_st"]["rgb"]
   slot = _slot(ret["outputs_coarse_ref"]["mask"], ray_batch["static_mask"].float(),
                flags=_lib.LOSS_SLOT_COMPLEMENT_W0)
-  return _rgb_term(STATIC, pred, ray_batch["rgb"], slot)
+  return _rgb_call(STATIC, pred, ray_batch["rgb"], slot)
+
+
+# ---- the criterion of a batch evaluated in ray slices (dynibar_b200/train_step.py) ----------------------------------
+# The terms couple rays only through denominators built from supervision, masks and detached forward values, so a
+# batch's loss and gradient come from: rows of every slice (pass 1, no gradient) -> one finish with the batch's
+# dimensions -> each slice's backward against that table.  `bootstrap` selects static_bootstrap_loss's single term
+# instead of mono_step_loss's.
+def _call(ret, ray_batch, args, epoch, bootstrap):
+  return _bootstrap_call(ret, ray_batch) if bootstrap else _step_call(ret, ray_batch, args, epoch)
+
+
+def slice_rows(ret, ray_batch, args, epoch, partial, first_ray, bootstrap=False):
+  """Writes the criterion rows of one ray slice (`ret` its render output, `ray_batch` its rays and supervision) that
+  starts at ray `first_ray` of the batch into `partial` (uint8, dyn_mono_loss_workspace_bytes(R_batch) bytes).
+  -> (weights, (S, K, n_sf)) for batch_table."""
+  wt, fixed, inputs = _call(ret, ray_batch, args, epoch, bootstrap)
+  return wt, ag.mono_loss_rows(wt, fixed, partial, first_ray, **inputs)
+
+
+def batch_table(partial, weights, R, dims):
+  """The [40] table of mono_step_table (or the bootstrap's) for the R-ray batch whose rows `partial` holds."""
+  return ag.mono_loss_finish(partial, weights, R, *dims)
+
+
+def slice_loss(ret, ray_batch, args, epoch, table, bootstrap=False):
+  """0-d tensor whose backward adds one ray slice's share of d(batch loss) / d(render outputs); its value is the
+  batch's loss.  `table`: batch_table of the batch."""
+  wt, fixed, inputs = _call(ret, ray_batch, args, epoch, bootstrap)
+  return ag.mono_loss(wt, dict(fixed, table=table), **inputs)[0]
+
+
+def _rgb_call(k, pred, gt, slot):
+  return _weights({k: 1.0}), {"R": pred.shape[0], "S": 2, "gt_rgb": gt, "slot%d" % k: slot}, {"rgb%d" % k: pred}
 
 
 def _rgb_term(k, pred, gt, slot):
-  fixed = {"R": pred.shape[0], "S": 2, "gt_rgb": gt, "slot%d" % k: slot}
-  return ag.mono_loss(_weights({k: 1.0}), fixed, **{"rgb%d" % k: pred})[0]
+  wt, fixed, inputs = _rgb_call(k, pred, gt, slot)
+  return ag.mono_loss(wt, fixed, **inputs)[0]
 
 
 class Criterion(torch.nn.Module):

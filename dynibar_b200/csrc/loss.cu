@@ -5,6 +5,9 @@
 //                           of 8 rays writes one row of partial sums.  pass 2: one block adds the rows in block order,
 //                           forms component = numerator / denominator, applies the weights and writes the nine logged
 //                           scalars, the components and the table weight / denominator for the backward.
+//   dyn_mono_loss_rows / dyn_mono_loss_finish  the two passes as separate calls, so that a batch can be evaluated in
+//                           ray slices: each slice writes its rows into one batch-wide buffer, finish runs once with
+//                           the batch's dimensions (the same bits as dyn_mono_loss when slices start on a block).
 //   dyn_mono_loss_backward  one warp per ray writes every requested gradient element exactly once; the upstream
 //                           gradient is read from device memory.
 //
@@ -458,6 +461,35 @@ extern "C" size_t dyn_mono_loss_workspace_bytes(int R) {
   return R > 0 ? (size_t)cdiv(R, kWarps) * kAcc * sizeof(float) : 0;
 }
 
+extern "C" int dyn_mono_loss_rows(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host,
+                                  float* partial, int first_block, void* stream) {
+  DYN_CHECK_ARG(in_host != nullptr && weights_host != nullptr && partial != nullptr && first_block >= 0);
+  const int rc = check_inputs(*in_host, *weights_host);
+  if (rc != DYN_OK) return rc;
+  // in.R is the slice's ray count and the stride of its [n, R, ...] inputs; the block rows land at first_block
+  mono_loss_kernel<<<cdiv(in_host->R, kWarps), kWarps * 32, 0, (cudaStream_t)stream>>>(
+      *in_host, weights_host->terms, partial + (long long)first_block * kAcc);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+extern "C" int dyn_mono_loss_finish(const float* partial, int nblocks, const dyn_mono_loss_weights* weights_host,
+                                    int R, int S, int K, int n_sf, float* out, void* stream) {
+  DYN_CHECK_ARG(partial != nullptr && weights_host != nullptr && out != nullptr);
+  const unsigned t = weights_host->terms;
+  auto has = [t](int k) { return ((t >> k) & 1u) != 0; };
+  DYN_CHECK_ARG(R > 0 && S >= 2 && K >= 0 && n_sf >= 0 && (t >> kTerms) == 0);
+  DYN_CHECK_ARG(!has(T_CYCLE) || K > 0);
+  DYN_CHECK_ARG(!(has(T_REG_ABS) || has(T_REG_TIME) || has(T_REG_SPACE)) || n_sf >= 2);
+  if (nblocks != cdiv(R, kWarps))
+    return fail(DYN_E_INVALID, "dyn_mono_loss_finish: %d rows given for %d rays, %d expected", nblocks, R,
+                cdiv(R, kWarps));
+  const Dims d{R, S, K, n_sf};
+  mono_loss_finish_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(partial, nblocks, *weights_host, d, out);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
 extern "C" int dyn_mono_loss(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host,
                              float* out, void* workspace, size_t workspace_bytes, void* stream) {
   DYN_CHECK_ARG(in_host != nullptr && weights_host != nullptr && out != nullptr && workspace != nullptr);
@@ -466,14 +498,10 @@ extern "C" int dyn_mono_loss(const dyn_mono_loss_inputs* in_host, const dyn_mono
   if (workspace_bytes < dyn_mono_loss_workspace_bytes(in_host->R))
     return fail(DYN_E_WORKSPACE, "dyn_mono_loss: workspace of %zu bytes, %zu needed", workspace_bytes,
                 dyn_mono_loss_workspace_bytes(in_host->R));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nblocks = cdiv(in_host->R, kWarps);
-  mono_loss_kernel<<<nblocks, kWarps * 32, 0, st>>>(*in_host, weights_host->terms, (float*)workspace);
-  DYN_LAUNCH_CHECK();
-  const Dims d{in_host->R, in_host->S, in_host->K, in_host->n_sf};
-  mono_loss_finish_kernel<<<1, 32, 0, st>>>((const float*)workspace, nblocks, *weights_host, d, out);
-  DYN_LAUNCH_CHECK();
-  return DYN_OK;
+  const int rc_rows = dyn_mono_loss_rows(in_host, weights_host, (float*)workspace, 0, stream);
+  if (rc_rows != DYN_OK) return rc_rows;
+  return dyn_mono_loss_finish((const float*)workspace, cdiv(in_host->R, kWarps), weights_host, in_host->R, in_host->S,
+                              in_host->K, in_host->n_sf, out, stream);
 }
 
 extern "C" int dyn_mono_loss_backward(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host,

@@ -441,6 +441,14 @@ int dyn_expected_scene_flow_backward(const float* weights, const float* sf, cons
  * Two launches: one warp per ray writes a block's partial sums into `workspace`
  * (dyn_mono_loss_workspace_bytes(R) bytes), one block then adds them in block order.  No float atomics: the same
  * inputs give the same bits.  S >= 2; with term 9-11 n_sf >= 2; with term 13 dist_n <= 256.
+ * The two passes as separate calls, for a batch evaluated in ray slices: dyn_mono_loss_rows runs pass 1 over one
+ * slice (`in` holds the slice: in.R is its ray count and the stride of its [n, R, ...] inputs, which are contiguous
+ * slices) and writes its cdiv(in.R, 8) rows of 2 * DYN_LOSS_TERMS floats at row `first_block` of `partial`, a
+ * batch-wide buffer of dyn_mono_loss_workspace_bytes(R_batch) bytes; a slice starts on a multiple of 8 rays
+ * (first_block = first ray / 8) and only the batch's last slice may hold a count that is not a multiple of 8.
+ * dyn_mono_loss_finish runs pass 2 once with the batch's R, S, K, n_sf (nblocks = cdiv(R, 8)); the REG, entropy and
+ * distortion denominators use that R.  Rows plus finish give the bits dyn_mono_loss gives on the whole batch.  The
+ * backward of a slice is dyn_mono_loss_backward on the slice's inputs with the batch's `out`.
  * dyn_mono_loss_backward: `g_loss` is the DEVICE address of d/d loss, `out` the forward's output.  Every non-NULL
  * pointer of `grads` is written exactly once per element in one launch (no zero-fill needed): rgb[k] [R,3],
  * depth [R], flows [n_flow,R,2], weights [R,dist_ld] (columns >= dist_n get 0), weights_dy / weights_st [R,S],
@@ -502,6 +510,10 @@ int dyn_mono_loss(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weigh
 int dyn_mono_loss_backward(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host,
                            const float* out, const float* g_loss, const dyn_mono_loss_grads* grads_host,
                            void* stream);
+int dyn_mono_loss_rows(const dyn_mono_loss_inputs* in_host, const dyn_mono_loss_weights* weights_host, float* partial,
+                       int first_block, void* stream);
+int dyn_mono_loss_finish(const float* partial, int nblocks, const dyn_mono_loss_weights* weights_host, int R, int S,
+                         int K, int n_sf, float* out, void* stream);
 
 /* Unit-test hooks of the tensor-core training products (csrc/train_tc.cu; bf16 operands, fp32 accumulation):
  * dyn_debug_tc_grad_w: dW[out,width] += dz[rows,out]^T (x[rows,width] * kscale[rows] or 1); out, width <= 256.
