@@ -177,6 +177,8 @@ SIGNATURES = {
     "dyn_nearest_resize": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "dyn_nvi_time_step": (_i, [C.POINTER(NviScene), _vp, _i, _i, _i] + [_vp] * 6 + [_vp]),
     "dyn_nvi_rays": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dyn_scene_pools": (_i, [C.POINTER(Scene), _vp, _i, _vp, _i, _vp, _i, _vp]),
+    "dyn_bt_frames": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -3,6 +3,7 @@
 //
 //   dyn_scene_masks      once per scene: motion, static and source masks of all frames (two launches)
 //   dyn_scene_views      per step: the three float source-view stacks and the target's full-frame supervision
+//   dyn_scene_pools      per bullet-time group: the same view rows into two stacks (the pools), no target frame
 //   dyn_scene_rays       per step: the selected pixels' rays and supervision (or every pixel's rays)
 //
 // Per step everything the kernels need to know (view table, target frame, camera matrix) sits in device memory the
@@ -225,6 +226,22 @@ int dyn_scene_views(const dyn_scene_t* scene, const int* table, int V, float* sr
   Stacks stk{{src_rgbs, anchor_src_rgbs, static_src_rgbs}, {n_src, n_anchor, n_static}};
   Target tg{rgb, disp, motion_mask, static_mask, flows, masks};
   views_kernel<<<dim3(cdiv((long long)scene->H * scene->W, kThreads), V + 1), kThreads, 0, (cudaStream_t)stream>>>(
+      *scene, table, V, stk, tg);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
+
+int dyn_scene_pools(const dyn_scene_t* scene, const int* table, int V, float* src_rgbs, int n_src,
+                    float* static_src_rgbs, int n_static, void* stream) {
+  DYN_CHECK_ARG(scene && scene->frames && scene->vviews && scene->N >= 1 && scene->H >= 1 && scene->W >= 1);
+  DYN_CHECK_ARG((long long)scene->H * scene->W < (1ll << 31) / 8);
+  DYN_CHECK_ARG(scene->srcmask == nullptr || scene->mc == 1 || scene->mc == 3);
+  DYN_CHECK_ARG(table && V >= 1 && V <= kMaxTableViews && n_src >= 0 && n_static >= 0 && n_src + n_static == V);
+  DYN_CHECK_ARG((n_src == 0 || src_rgbs) && (n_static == 0 || static_src_rgbs));
+  Stacks stk{{src_rgbs, nullptr, static_src_rgbs}, {n_src, 0, n_static}};
+  Target tg{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  // V rows only: the target row (blockIdx.y == V) is never launched, so the target fields are not read
+  views_kernel<<<dim3(cdiv((long long)scene->H * scene->W, kThreads), V), kThreads, 0, (cudaStream_t)stream>>>(
       *scene, table, V, stk, tg);
   DYN_LAUNCH_CHECK();
   return DYN_OK;

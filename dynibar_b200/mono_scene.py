@@ -112,7 +112,8 @@ def load_cameras(scene_path, height, bd_factor=0.75):
   """The scene's cameras as MonocularDataset.__init__ builds them (load_mono_data with load_imgs=False).
 
   Returns a dict: rgb_files, hw (of the training images), K [N,4,4], c2w [N,4,4], vv_c2w [N,8,4,4] (float64),
-  scale (float64), depth_range float32 [2] (near * 0.9, far * 1.5).  `scale` is computed in float64 and applied as
+  scale (float64), depth_range float32 [2] (near * 0.9, far * 1.5), poses float32 [N,3,5] (the recentred llff
+  poses) and bounds (min, max of the scaled bounds as Python floats).  `scale` is computed in float64 and applied as
   float32(scale) in float32, as numpy 1.x (the reference's environment) evaluates the float32 array operations with
   a float64 scalar; the near / far arithmetic is float64, rounded to float32 at the end, as numpy 1.x does."""
   arr = _npload(os.path.join(scene_path, "poses_bounds_cvd.npy"))
@@ -152,7 +153,8 @@ def load_cameras(scene_path, height, bd_factor=0.75):
   cams = [_opencv_camera(p) for p in poses]
   vv_c2w = np.stack([np.stack([_opencv_camera(p)[1] for p in frame]) for frame in vv])
   return dict(rgb_files=files, hw=tuple(hw), K=np.stack([c[0] for c in cams]), c2w=np.stack([c[1] for c in cams]),
-              vv_c2w=vv_c2w, scale=scale, depth_range=np.array([near * 0.9, far * 1.5]).astype(np.float32))
+              vv_c2w=vv_c2w, scale=scale, depth_range=np.array([near * 0.9, far * 1.5]).astype(np.float32),
+              poses=poses, bounds=(near, top))
 
 
 # ---- the draws (monocular.py:148, :215-298, :313-315, :375-377) --------------------------------------------------

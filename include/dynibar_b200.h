@@ -708,6 +708,13 @@ int dyn_scene_views(const dyn_scene_t* scene, const int* table, int V, float* sr
 int dyn_scene_rays(const dyn_scene_t* scene, const float* cam, const int* target, const int* sel, int R, float* ray_o,
                    float* ray_d, float* uv_grid, float* rgb, float* disp, float* motion_mask, float* static_mask,
                    float* flows, float* masks, void* stream);
+/* The source-view pools of a bullet-time group (DESIGN §3.9), one launch: dyn_scene_views's view rows without its
+ * target row.  table (device, 16-byte aligned) int32 [V * 4], rows (frame, virtual view 0..7 or -1, masked,
+ * stack << 8 | slot) with stack 0 -> src_rgbs [n_src,H,W,3] and stack 2 -> static_src_rgbs [n_static,H,W,3] fp32.
+ * Only frames and vviews are read (srcmask for masked rows); a virtual-view row's frame names one [8,H,W,3] set of
+ * vviews, which may hold fewer sets than there are frames (the caller's table stays in range). */
+int dyn_scene_pools(const dyn_scene_t* scene, const int* table, int V, float* src_rgbs, int n_src,
+                    float* static_src_rgbs, int n_static, void* stream);
 
 /* ---- an Nvidia-benchmark scene resident on the device (DESIGN §3.8; csrc/nvi_scene.cu) -----------------------------
  * eval_nvidia.py's DynamicVideoDataset.__getitem__ (:71-198) and its ground-truth / mask reads (:383-428) on a scene
@@ -741,6 +748,13 @@ int dyn_nvi_time_step(const dyn_nvi_scene_t* scene, const int* table, int nd, in
  * camera_index int32 [K H W] = k. */
 int dyn_nvi_rays(const float* cams, int K, int H, int W, float* ray_o, float* ray_d, float* uv_grid, int* camera_index,
                  void* stream);
+
+/* ---- a monocular bullet-time sweep from a device-resident scene (DESIGN §3.9; csrc/bt_scene.cu) -------------------
+ * render_monocular_bt.py's loader on a scene uploaded once: dyn_nearest_resize (masks), dyn_scene_pools (pools),
+ * dyn_nvi_rays (rays), and the output frames below. */
+/* rgb [K,H,W,3] fp32 -> out [K,H-2 crop_h,W-2 crop_w,3] uint8 = (255 * clip(x, 0, 1)).astype(np.uint8) of the
+ * cropped window (:346-354): a float32 product without contraction, truncated toward zero.  One launch. */
+int dyn_bt_frames(const float* rgb, int K, int H, int W, int crop_h, int crop_w, uint8_t* out, void* stream);
 
 #ifdef __cplusplus
 }
