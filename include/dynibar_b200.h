@@ -19,6 +19,18 @@
  *     fused kernels (2 x SMs x 256 KB, kept for the life of the process; a
  *     CTA holds one slot of it while it runs, so streams can share it).  The
  *     first fused launches on a device must not be inside a stream capture.
+ *   - workspaces and scratch buffers (`workspace`, `scratch`, `feat_cl_ws`,
+ *     `posenc_ws`, ...): the base must be 256-byte aligned, because the
+ *     library carves them into sub-buffers that assume it.  An entry point
+ *     neither depends on what a workspace held before the call (every byte
+ *     it reads it wrote first in the same call) nor writes past the size its
+ *     `*_workspace_bytes` / `*_scratch_bytes` function declares, whatever
+ *     the buffer's real size.  Outputs likewise: an entry point writes only
+ *     inside their stated extents and reads none of their prior contents
+ *     unless it says it accumulates into them (the `d_params` of the
+ *     training backwards).
+ *   - `saved` buffers (the train forwards) are not scratch: they carry state
+ *     from a train forward to its backward and must be passed unchanged.
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it,
  *     nothing synchronises.
  *   - return 0 on success, a negative DYN_E_* otherwise; `dyn_last_error()`
