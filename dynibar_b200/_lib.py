@@ -169,6 +169,9 @@ SIGNATURES = {
     "dyn_virtual_views": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "dyn_image_scores_workspace_bytes": (_sz, [_i, _i, _i]),
     "dyn_image_scores": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "dyn_lpips_param_count": (_sz, []),
+    "dyn_lpips_workspace_bytes": (_sz, [_i, _i, _i]),
+    "dyn_lpips": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "dyn_scene_masks_workspace_bytes": (_sz, [_i, _i, _i]),
     "dyn_scene_masks": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dyn_scene_views": (_i, [C.POINTER(Scene), _vp, _i, _vp, _i, _vp, _i, _vp, _i] + [_vp] * 7),

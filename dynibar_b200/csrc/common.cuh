@@ -137,6 +137,35 @@ __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-
 // torch Softplus(beta=1, threshold=20)
 __device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }
 
+namespace dyn {
+// eval_nvidia.py:383-384: np.sum over the 3 channels in float32 ((r + g) + b), strict > float32(1e-3)
+__device__ __forceinline__ bool valid_pixel(float r, float g, float b) {
+  return __fadd_rn(__fadd_rn(r, g), b) > 1e-3f;
+}
+
+// fixed-order CTA sum of N doubles per thread over a CTA of WARPS full warps: butterfly in each warp, then thread 0
+// over the warps in order.  The result is in v[] of thread 0.
+template <int N, int WARPS>
+__device__ __forceinline__ void block_sum(double (&v)[N], double (*red)[N]) {
+#pragma unroll
+  for (int j = 0; j < N; ++j)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0)
+#pragma unroll
+    for (int j = 0; j < N; ++j) red[warp][j] = v[j];
+  __syncthreads();
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+      double s = red[0][j];
+      for (int w = 1; w < WARPS; ++w) s += red[w][j];
+      v[j] = s;
+    }
+}
+}  // namespace dyn
+
 // F.normalize(v, dim=-1): v / max(||v||, 1e-12)
 __device__ __forceinline__ void normalize3(float& x, float& y, float& z) {
   float n = sqrtf(x * x + y * y + z * z);

@@ -23,7 +23,6 @@ constexpr int kMaxRows = 3, kSums = 3 * kMaxRows;  // per mask row m: sum S w_m,
 constexpr float kCov = (float)(49.0 / 48.0);
 constexpr float kC1 = (float)((0.01 * 2.0) * (0.01 * 2.0));
 constexpr float kC2 = (float)((0.03 * 2.0) * (0.03 * 2.0));
-constexpr float kValidEps = 1e-3f;  // eval_nvidia.py:384: sum(rgb) > 1e-3 on a float32 array
 constexpr double kCountEps = 1e-8;  // np.sum(mask) + 1e-8
 
 // scipy.ndimage mode 'reflect' (d c b a | a b c d); the clamp only keeps the unused rows / columns of a partial tile in
@@ -32,32 +31,6 @@ __device__ __forceinline__ int reflect(int i, int n) {
   if (i < 0) i = -i - 1;
   if (i >= n) i = 2 * n - 1 - i;
   return min(max(i, 0), n - 1);
-}
-
-// eval_nvidia.py:383-384: np.sum over the 3 channels in float32 ((r + g) + b), strict > float32(1e-3)
-__device__ __forceinline__ bool valid_pixel(float r, float g, float b) {
-  return __fadd_rn(__fadd_rn(r, g), b) > kValidEps;
-}
-
-// fixed-order CTA sum of kSums doubles per thread: butterfly in each warp, then warp 0 over the warps in order.
-// The result is in v[] of thread 0.
-__device__ __forceinline__ void block_sum(double (&v)[kSums], double (*red)[kSums]) {
-#pragma unroll
-  for (int j = 0; j < kSums; ++j)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0)
-#pragma unroll
-    for (int j = 0; j < kSums; ++j) red[warp][j] = v[j];
-  __syncthreads();
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int j = 0; j < kSums; ++j) {
-      double s = red[0][j];
-      for (int w = 1; w < kWarps; ++w) s += red[w][j];
-      v[j] = s;
-    }
 }
 
 // One CTA per kTileW x kTileH output tile of image blockIdx.z, all 3 channels.  The tile plus a 3-pixel reflected halo
@@ -161,7 +134,7 @@ __global__ void __launch_bounds__(kThreads) ssim_tile_kernel(const float* __rest
     __syncthreads();
   }
 
-  block_sum(acc, red);
+  block_sum<kSums, kWarps>(acc, red);
   if (threadIdx.x == 0) {
     const size_t tile = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
 #pragma unroll
@@ -182,7 +155,7 @@ __global__ void __launch_bounds__(kThreads) scores_finish_kernel(const double* _
   for (int t = threadIdx.x; t < tiles; t += kThreads)
 #pragma unroll
     for (int j = 0; j < kSums; ++j) acc[j] += p[(size_t)t * kSums + j];
-  block_sum(acc, red);
+  block_sum<kSums, kWarps>(acc, red);
   if (threadIdx.x != 0) return;
   double* out = scores + (size_t)blockIdx.x * M * 2;
 #pragma unroll

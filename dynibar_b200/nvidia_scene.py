@@ -5,6 +5,7 @@ __main__ block) without imageio or scikit-image, and without decoding any file a
   scene = NvidiaScene(scene_path, args, device)    # reads <scene_path> (the reference's `dense` folder) once
   step = scene.time_step(img_i)                     # one time step's batch, ground truth and masks, on the device
   result = scene.evaluate(model, projector, args)   # eval_nvidia.py:305-481: PSNR / SSIM of every camera
+  result = scene.evaluate(model, projector, args, lpips=LPIPSWeights(alexnet, lin))   # and LPIPS
 
 Frames, coarse static masks, ground truth and dynamic masks are uploaded once: the ground truth is resized to the
 render size on the device (csrc/nvi_scene.cu: cv2's INTER_AREA, byte for byte) and the masks with cv2's
@@ -322,28 +323,46 @@ class NvidiaScene(object):
         fine_featmaps=(ref_featmaps_fine, None, static_featmaps_fine), is_train=False)
     return torch.stack([r["outputs_fine_ref"]["rgb"] for r in rets]).to(self.device)
 
-  def evaluate(self, model, projector, args, on_step=None):
-    """eval_nvidia.py:305-481 without LPIPS: per time step the encoder passes, one render_multi_image_nvi, one
-    score_views and one read-back of the scores.  on_step(img_i, scores so far [t+1, 11, 3, 2]) is called after each
-    time step (the script prints its MOVING lines there).
+  def evaluate(self, model, projector, args, on_step=None, lpips=None):
+    """eval_nvidia.py:305-481: per time step the encoder passes, one render_multi_image_nvi, one score_views and one
+    read-back of the scores.  on_step(img_i, scores so far [t+1, 11, 3, 2]) is called after each time step (the script
+    prints its MOVING lines there).
 
     Returns dict(scores float64 [T, 11, 3, 2] (full / dynamic / static x PSNR / SSIM, cameras in target_cameras
-    order), mean float64 [3, 2] (np.mean over every camera of every time step, as the AVG lines), steps)."""
-    from .metrics import score_views
-    out = []
+    order), mean float64 [3, 2] (np.mean over every camera of every time step, as the AVG lines), steps).
+
+    lpips: an LPIPSWeights (dynibar_b200.metrics) adds one lpips_views per time step, read back with the scores; the
+    result gains lpips float64 [T, 11, 3] and lpips_mean [3] (averaged as `mean`), and on_step receives the LPIPS
+    values so far [t+1, 11, 3] as a third argument.  Without it nothing of the above changes."""
+    from .metrics import lpips_views, score_views
+    out, lp = [], []
     for img_i in self.steps:
       step = self.time_step(img_i)
       with torch.no_grad():
         pred = self.render(step, model, projector, args)
         scores = score_views(pred, step["gt_rgb"], step["dynamic_mask"])
+        if lpips is not None:
+          lp.append(lpips_views(pred, step["gt_rgb"], step["dynamic_mask"], weights=lpips).cpu().numpy())
       out.append(scores.cpu().numpy())
       if on_step is not None:
-        on_step(img_i, np.stack(out))
+        if lpips is None:
+          on_step(img_i, np.stack(out))
+        else:
+          on_step(img_i, np.stack(out), np.stack(lp))
     scores = np.stack(out)
-    return dict(scores=scores, mean=mean_scores(scores), steps=list(self.steps))
+    res = dict(scores=scores, mean=mean_scores(scores), steps=list(self.steps))
+    if lpips is not None:
+      res.update(lpips=np.stack(lp), lpips_mean=mean_lpips(np.stack(lp)))
+    return res
 
 
 def mean_scores(scores):
   """The AVG / MOVING lines' np.mean over the flat per-camera lists (time-major, cameras in order) -> [3, 2]."""
   flat = scores.reshape(-1, 3, 2)
   return np.array([[np.mean(np.array(flat[:, r, c].tolist())) for c in range(2)] for r in range(3)])
+
+
+def mean_lpips(lpips):
+  """The LPIPS AVG / MOVING lines: lpips [T, 11, 3] -> [3], averaged as mean_scores averages."""
+  flat = lpips.reshape(-1, 3)
+  return np.array([np.mean(np.array(flat[:, r].tolist())) for r in range(3)])

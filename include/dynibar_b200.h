@@ -679,6 +679,28 @@ size_t dyn_image_scores_workspace_bytes(int K, int H, int W);
 int dyn_image_scores(const float* pred, const float* gt, const float* mask, int K, int H, int W, int mode,
                      double* scores, float* ssim_map, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- LPIPS v0.1 'alex' of rendered views (eval_nvidia.py:289-291, :402-452; DESIGN §3.6; csrc/lpips.cu) -----------
+ * weights: one fp32 blob of dyn_lpips_param_count() = 2 470 848 floats, in this order:
+ *   for l = 1..5: conv l weight [Cout, Cin, k, k] then its bias [Cout] (torchvision alexnet().features.{0,3,6,8,10};
+ *                 (Cin, Cout, k) = (3, 64, 11), (64, 192, 5), (192, 384, 3), (384, 256, 3), (256, 256, 3));
+ *   then for l = 0..4: lin l [Cout of conv l + 1] (LPIPS v0.1 alex.pth lin{l}.model.1.weight, non-negative).
+ * pred, gt [K,H,W,3] fp32 channels-last, contiguous; mask [K,H,W,3] fp32 or NULL; H, W >= 31.  Per camera: the
+ * ScalingLayer (x - shift) / scale, AlexNet's five ReLU taps in fp32 (FFMA, no TF32), per tap the unit-normalised
+ * channel vectors' squared difference dotted with lin -> d_l; per mask row m with weights w_m [H,W] (the sum of the
+ * row's 3 channels; the valid row and an absent mask count 3), m_l = adaptive_avg_pool2d(w_m, tap size) and
+ * score = sum over taps with sum m_l > 0 of sum(m_l d_l) / sum(m_l), in fp64.  scores [K,M] fp64.
+ *   DYN_SCORES_PLAIN  images already in [-1, 1] (PerceptualLoss's input); M = 1, row = mask (1 where mask is NULL).
+ *   DYN_SCORES_EVAL   images in [0, 1]: valid = ((r + g) + b) > 1e-3f on pred (float32), both images multiplied by
+ *                     valid and mapped to 2x - 1; rows valid, mask, 1 - mask (M = 3), or valid alone (M = 1) when mask
+ *                     is NULL.
+ * No float atomics: the same inputs give the same bits, and a camera's scores do not depend on K or the other
+ * cameras. */
+size_t dyn_lpips_param_count(void);
+/* workspace of dyn_lpips for K cameras of H x W (either mode); 0 for an unsupported shape */
+size_t dyn_lpips_workspace_bytes(int K, int H, int W);
+int dyn_lpips(const float* pred, const float* gt, const float* mask, int K, int H, int W, int mode,
+              const float* weights, double* scores, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- a monocular training scene resident on the device (DESIGN §3.7; csrc/scene.cu) --------------------------------
  * MonocularDataset.__getitem__ (ibrnet/data_loaders/monocular.py:146-426) and RaySamplerSingleImage.random_sample
  * (ibrnet/sample_ray.py:262-331) on a scene uploaded once.  Float values are the reference's float32 expressions,

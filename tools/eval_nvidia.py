@@ -3,11 +3,14 @@
 
   python tools/eval_nvidia.py --scene_path <folder_path>/<scene>/dense --coarse model_coarse.pth --fine model_fine.pth \\
       [--mask_static] [--N_samples 64] [--N_importance 64] [--chunk_size 8192] [--inv_uniform] [--white_bkgd] \\
-      [--anti_alias_pooling 1] [--mask_rgb 0] [--occ_weights_mode 0] [--num_basis 6]
+      [--anti_alias_pooling 1] [--mask_rgb 0] [--occ_weights_mode 0] [--num_basis 6] \\
+      [--lpips_alexnet alexnet.pth --lpips_lin alex.pth]
 
 The options are the keys the reference's configs_nvidia/*.txt set that the evaluation reads.  Checkpoints load
 through dynibar_b200.model.model_from_checkpoints.  Prints the reference's MOVING lines after every time step and the
-AVG lines at the end, in its order, without the LPIPS lines (LPIPS is not computed).
+AVG lines at the end, in its order.  With --lpips_alexnet (torchvision's AlexNet checkpoint) and --lpips_lin (LPIPS
+v0.1's alex.pth) it also computes LPIPS (dynibar_b200.metrics.lpips_views) and prints all nine lines of each block,
+as the reference does; without them the LPIPS lines are left out.
 """
 
 import argparse
@@ -20,6 +23,7 @@ if ROOT not in sys.path:
 
 LABELS = (("PSNR", 0, 0), ("SSIM", 0, 1), ("DYNAMIC PSNR", 1, 0), ("DYNAMIC SSIM", 1, 1), ("Static PSNR", 2, 0),
           ("Static SSIM", 2, 1))
+ROW_NAMES = ("", "DYNAMIC ", "Static ")  # eval_nvidia.py:459-481: per row PSNR, SSIM, LPIPS
 
 
 def parser():
@@ -42,16 +46,27 @@ def parser():
   ap.add_argument("--input_dir", type=int, default=1)
   ap.add_argument("--input_xyz", type=int, default=0)
   ap.add_argument("--device", default="cuda:0")
+  ap.add_argument("--lpips_alexnet", default=None, help="torchvision AlexNet checkpoint (with --lpips_lin)")
+  ap.add_argument("--lpips_lin", default=None, help="LPIPS v0.1 alex.pth (with --lpips_alexnet)")
   return ap
 
 
-def print_means(prefix, means):
-  for label, r, c in LABELS:
-    print("%s %s " % (prefix, label), means[r, c])
+def print_means(prefix, means, lpips=None):
+  if lpips is None:
+    for label, r, c in LABELS:
+      print("%s %s " % (prefix, label), means[r, c])
+    return
+  for r, name in enumerate(ROW_NAMES):
+    print("%s %sPSNR " % (prefix, name), means[r, 0])
+    print("%s %sSSIM " % (prefix, name), means[r, 1])
+    print("%s %sLPIPS " % (prefix, name), lpips[r])
 
 
 def main(argv=None):
-  args = parser().parse_args(argv)
+  ap = parser()
+  args = ap.parse_args(argv)
+  if (args.lpips_alexnet is None) != (args.lpips_lin is None):
+    ap.error("--lpips_alexnet and --lpips_lin go together")
   args.input_dir, args.input_xyz = bool(args.input_dir), bool(args.input_xyz)
   import torch
   from dynibar_b200 import model as dm
@@ -67,8 +82,16 @@ def main(argv=None):
     enc = ResNet().to(dev)
     enc.load_state_dict(dm._strip(info["encoders"][k]))
     setattr(model, k, enc.eval().requires_grad_(False))
-  res = scene.evaluate(model, Projector(dev), args, on_step=lambda i, s: print_means("MOVING", mean_scores(s)))
-  print_means("AVG", res["mean"])
+  if args.lpips_alexnet is None:
+    res = scene.evaluate(model, Projector(dev), args, on_step=lambda i, s: print_means("MOVING", mean_scores(s)))
+    print_means("AVG", res["mean"])
+    return res
+  from dynibar_b200.metrics import LPIPSWeights
+  from dynibar_b200.nvidia_scene import mean_lpips
+  w = LPIPSWeights(args.lpips_alexnet, args.lpips_lin, device=dev)
+  res = scene.evaluate(model, Projector(dev), args, lpips=w,
+                       on_step=lambda i, s, lp: print_means("MOVING", mean_scores(s), mean_lpips(lp)))
+  print_means("AVG", res["mean"], res["lpips_mean"])
   return res
 
 
