@@ -7,12 +7,13 @@ output frames) without imageio, and without decoding any file after the scene is
     ...                                                  # frames: uint8 [k, H', W', 3] on the host, RGB
 
 The 50 target cameras of the wander path around frame args.render_idx are split into groups of at most 16 cameras
-whose source views fit two pools of at most 32 views (bullet_time.group_cameras).  Per group the host writes one
-small pinned staging buffer (view table, cameras, depth range) and copies it with one asynchronous copy; two kernels
-assemble what sample_ray.stack_pooled_ray_batches would return for the group's get_all() batches; the encoder runs
-once per pool, render_image.render_multi_image_mono renders the group, and csrc/bt_scene.cu turns the rendered rgb
-into the script's cropped uint8 frames, which reach the host in one copy (the renderer itself still hands its
-outputs back on the host).  DESIGN §3.9 gives the semantics.
+whose source views fit two pools of at most 32 views (bullet_time.group_cameras).  A negative args.render_idx renders
+the stabilised video instead: camera i of bullet_time.stabilization_path at frame i's time, for i = 3 .. n-4, one
+camera per group.  Per group the host writes one small pinned staging buffer (view table, cameras, depth range) and
+copies it with one asynchronous copy; two kernels assemble what sample_ray.stack_pooled_ray_batches would return for
+the group's get_all() batches; the encoder runs once per pool, render_image.render_multi_image_mono renders the
+group, and csrc/bt_scene.cu turns the rendered rgb into the script's cropped uint8 frames, which reach the host in
+one copy (the renderer itself still hands its outputs back on the host).  DESIGN §3.9 gives the semantics.
 """
 
 import os
@@ -47,38 +48,51 @@ def camera_row(H, W, K, c2w):
 
 
 def plan_sweep(cams, render_idx, num_source_views, max_range, num_vv):
-  """The sweep of render_idx on a scene's cameras (mono_scene.load_cameras) -> dict:
-    cameras   float32 [50, 34]: the target cameras of the wander path (render intrinsics and poses)
-    render_K  float64 [50, 4, 4]
-    selections  per camera (temporal ids, virtual-view ids, static ids), bullet_time.select_source_views
-    groups    bullet_time.group_cameras's (start, stop) ranges."""
+  """The sweep of render_idx on a scene's cameras (mono_scene.load_cameras) -> dict over the path's m cameras (50 on
+  the wander path around render_idx; for render_idx < 0 the stabilised path's n, one per frame):
+    cameras   float32 [m, 34]: the target cameras (render intrinsics and poses)
+    render_K  float64 [m, 4, 4]
+    frames    int [m]: the frame whose time each camera is rendered at (render_idx, or camera i at frame i)
+    selections  per camera (temporal ids, virtual-view ids, static ids), bullet_time.select_source_views with
+              render_idx = frames[i]; None for a stabilised camera outside [3, n-4], which is not rendered
+    groups    bullet_time.group_cameras's (start, stop) ranges, each of one frame."""
   H, W = cams["hw"]
-  path = np.array(bt.wander_path(cams["poses"][render_idx])).astype(np.float32)
+  n = len(cams["c2w"])
+  if render_idx < 0:
+    path = bt.stabilization_path(cams["poses"])
+    frames = list(range(n))
+  else:
+    path = np.array(bt.wander_path(cams["poses"][render_idx])).astype(np.float32)
+    frames = [int(render_idx)] * len(path)
   parsed = [_opencv_camera(p) for p in path]
   render_K = np.stack([p[0] for p in parsed])
   render_c2w = np.stack([p[1] for p in parsed])
-  sel = [bt.select_source_views(c, cams["c2w"], cams["vv_c2w"], render_idx, num_source_views, max_range, num_vv)
-         for c in render_c2w]
+  sel = [bt.select_source_views(c, cams["c2w"], cams["vv_c2w"], f, num_source_views, max_range, num_vv)
+         if render_idx >= 0 or 3 <= f <= n - 4 else None for c, f in zip(render_c2w, frames)]
   return dict(cameras=np.stack([camera_row(H, W, k, c) for k, c in zip(render_K, render_c2w)]), render_K=render_K,
-              render_c2w=render_c2w, selections=sel, groups=bt.group_cameras(sel))
+              render_c2w=render_c2w, frames=frames, selections=sel, groups=bt.group_cameras(sel, frames=frames))
 
 
 def plan_group(cams, plan, render_idx, lo, hi, mask_src_view):
   """The pools of cameras lo..hi-1, as sample_ray.stack_pooled_ray_batches forms them from the cameras' batches:
   each pool holds the union of the cameras' views by identity in the order first met (camera lo's slots first), so
   the dynamic pool starts with the 7 temporal frames.  Returns dict with
-    dy_ids, st_ids        per camera, the identities of its slots (frame id, or ("vv", j) for a virtual view)
+    dy_ids, st_ids        per camera, the identities of its slots (frame id, or for virtual view j of the camera's
+                          frame f ("vv", j) on the wander path and ("vv", f, j) on the stabilised path)
     dy_pool, st_pool      the pools' identities in pool order
     src_views, static_src_views   int32 [k, 7 + num_vv] / [k, 2 num_source_views + 1]: pool entry of every slot
     src_cameras, static_src_cameras  float32 [P, 34]: a frame's row holds its own intrinsics; a virtual view's row
                           holds the render camera's intrinsics (:195-199), those of the first camera that names it
     table                 int32 [Pd + Ps, 4]: dyn_scene_pools rows (frame, virtual view or -1, masked,
-                          stack << 8 | slot); a virtual view's frame is 0, the scene's one set of virtual views."""
+                          stack << 8 | slot); a virtual view's frame is 0 on the wander path (the scene holds the
+                          virtual views of render_idx only) and f on the stabilised path (it holds every frame's)."""
   H, W = cams["hw"]
+  stabilized = render_idx < 0
   dy_ids, st_ids = [], []
   for k in range(lo, hi):
     t, vv, st = plan["selections"][k]
-    dy_ids.append(list(t) + [("vv", j) for j in vv])
+    f = plan["frames"][k]
+    dy_ids.append(list(t) + [("vv", f, j) if stabilized else ("vv", j) for j in vv])
     st_ids.append(list(st))
 
   def pool(ids_per_cam, row_of):
@@ -95,7 +109,7 @@ def plan_group(cams, plan, render_idx, lo, hi, mask_src_view):
 
   def dy_row(ident, k):
     if isinstance(ident, tuple):
-      return camera_row(H, W, plan["render_K"][k], cams["vv_c2w"][render_idx, ident[1]])
+      return camera_row(H, W, plan["render_K"][k], cams["vv_c2w"][plan["frames"][k], ident[-1]])
     return camera_row(H, W, cams["K"][ident], cams["c2w"][ident])
 
   st_row = lambda ident, k: camera_row(H, W, cams["K"][ident], cams["c2w"][ident])
@@ -103,7 +117,10 @@ def plan_group(cams, plan, render_idx, lo, hi, mask_src_view):
   st_pool, st_cameras, st_views = pool(st_ids, st_row)
   table = []
   for slot, ident in enumerate(dy_pool):
-    table.append((0, ident[1], 0, slot) if isinstance(ident, tuple) else (ident, -1, 0, slot))
+    if isinstance(ident, tuple):
+      table.append((ident[1] if stabilized else 0, ident[-1], 0, slot))
+    else:
+      table.append((ident, -1, 0, slot))
   for slot, ident in enumerate(st_pool):
     table.append((ident, -1, int(bool(mask_src_view)), 2 << 8 | slot))
   return dict(dy_ids=dy_ids, st_ids=st_ids, dy_pool=dy_pool, st_pool=st_pool, src_views=src_views,
@@ -119,9 +136,10 @@ def crop_of(H, W):
 # ---- the scene ---------------------------------------------------------------------------------------------------
 
 class BulletTimeScene(object):
-  """A monocular scene (the reference's `dense` folder) on one device, for the bullet-time sweep of one frame.
-  args: training_height, num_source_views, max_range, num_vv, mask_src_view, render_idx (the reference's rendering
-  options; sweep also reads N_samples, chunk_size, inv_uniform and, when present, N_importance and white_bkgd)."""
+  """A monocular scene (the reference's `dense` folder) on one device, for the bullet-time sweep of one frame or,
+  when render_idx < 0, the stabilised video.  args: training_height, num_source_views, max_range, num_vv,
+  mask_src_view, render_idx (the reference's rendering options; sweep also reads N_samples, chunk_size, inv_uniform
+  and, when present, N_importance and white_bkgd)."""
 
   def __init__(self, scene_path, args, device):
     self.device = torch.device(device)
@@ -141,9 +159,14 @@ class BulletTimeScene(object):
                        % (2 * self.num_source_views + 1, 7 + self.num_vv, bt.MAX_POOL))
     cams = self.cams = load_cameras(scene_path, args.training_height)
     n = self.num_frames = len(cams["rgb_files"])
-    if not 3 <= self.render_idx <= n - 4:
+    self.stabilized = self.render_idx < 0
+    if self.stabilized and n < 7:
+      raise ValueError("BulletTimeScene: the stabilised video renders cameras 3 .. n-4, each with the temporal views "
+                       "i - 3 .. i + 3, so it needs at least 7 frames; the scene has %d" % n)
+    if not self.stabilized and not 3 <= self.render_idx <= n - 4:
       raise ValueError("BulletTimeScene: render_idx %d; the temporal views are render_idx - 3 .. render_idx + 3, so "
-                       "render_idx must lie in [3, %d] for %d frames" % (self.render_idx, n - 4, n))
+                       "render_idx must lie in [3, %d] for %d frames (or be negative: the stabilised video)"
+                       % (self.render_idx, n - 4, n))
     H, W = self.H, self.W = cams["hw"]
     self.depth_range = depth_range(*cams["bounds"])
     self.plan = plan_sweep(cams, self.render_idx, self.num_source_views, self.max_range, self.num_vv)
@@ -172,11 +195,15 @@ class BulletTimeScene(object):
       return a
 
     frames = np.stack([image(f, "frame") for f in self.cams["rgb_files"]])
-    vdir = os.path.join(p, "source_virtual_views_%dx%d" % (W, H), "%05d" % self.render_idx)
-    if not os.path.isdir(vdir):
-      raise ValueError("BulletTimeScene: missing directory %s (the virtual views of render_idx %d)"
-                       % (vdir, self.render_idx))
-    vviews = np.stack([image(os.path.join(vdir, "%02d.png" % j), "virtual view") for j in range(N_VIRTUAL)])
+
+    def virtual_views(f):
+      vdir = os.path.join(p, "source_virtual_views_%dx%d" % (W, H), "%05d" % f)
+      if not os.path.isdir(vdir):
+        raise ValueError("BulletTimeScene: missing directory %s (the virtual views of frame %d)" % (vdir, f))
+      return np.stack([image(os.path.join(vdir, "%02d.png" % j), "virtual view") for j in range(N_VIRTUAL)])
+
+    # [8, H, W, 3] of render_idx, or [n, 8, H, W, 3] of every frame for the stabilised video
+    vviews = np.stack([virtual_views(f) for f in range(n)]) if self.stabilized else virtual_views(self.render_idx)
     masks = None
     if self.mask_src_view:
       mdir = os.path.join(p, "dynamic_masks")
@@ -229,17 +256,18 @@ class BulletTimeScene(object):
     return slot
 
   def group_batch(self, g):
-    """Group g of the sweep (cameras groups[g][0] .. groups[g][1] - 1), assembled on the device without a host
-    synchronisation:
+    """Group g of the sweep (cameras groups[g][0] .. groups[g][1] - 1, all rendered at one frame's time), assembled
+    on the device without a host synchronisation:
 
       ray_batch     what sample_ray.stack_pooled_ray_batches returns for the cameras' RaySamplerSingleImage(item)
                     .get_all() batches: camera [k,34], camera_index, depth_range float64 [1,2], the pools src_rgbs /
                     src_cameras and static_src_rgbs / static_src_cameras, src_views / static_src_views (host int32),
                     src_view_ids / static_src_view_ids; rgb is None (the script's ground truth is never used)
       ray_samplers  k objects with H and W (what render_multi_image_mono reads)
-      frame_idx, time_embedding, time_offset   as the script's loop builds them (:300-305)
+      frame_idx, time_embedding, time_offset   as the script's loop builds them (:300-305) for the group's frame
       cameras       the cameras' indices in the sweep."""
     lo, hi = self.groups[g]
+    frame = int(self.plan["frames"][lo])
     grp = plan_group(self.cams, self.plan, self.render_idx, lo, hi, self.mask_src_view)
     K, H, W = hi - lo, self.H, self.W
     nd, ns = len(grp["dy_pool"]), len(grp["st_pool"])
@@ -260,7 +288,7 @@ class BulletTimeScene(object):
     view["src_cameras"][0] = grp["src_cameras"]
     view["static_src_cameras"][0] = grp["static_src_cameras"]
     view["depth_range"][0] = self.depth_range
-    view["ref_time"][0] = float(self.render_idx / float(self.num_frames))
+    view["ref_time"][0] = float(frame / float(self.num_frames))
     d = torch.empty(L.nbytes, dtype=torch.uint8, device=self.device)
     d.copy_(pinned[:L.nbytes], non_blocking=True)
     event.record()
@@ -284,7 +312,7 @@ class BulletTimeScene(object):
       _lib.check(_lib.lib.dyn_nvi_rays(p(d["rays"]), K, H, W, p(rb["ray_o"]), p(rb["ray_d"]), p(rb["uv_grid"]),
                                        p(rb["camera_index"]), st_))
     return dict(ray_batch=rb, ray_samplers=[types.SimpleNamespace(H=H, W=W) for _ in range(K)],
-                frame_idx=(self.render_idx, None), time_embedding=(d["ref_time"], None),
+                frame_idx=(frame, None), time_embedding=(d["ref_time"], None),
                 time_offset=([int(o) for o in OFFSETS], None), cameras=list(range(lo, hi)))
 
   @staticmethod

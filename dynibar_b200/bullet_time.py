@@ -1,8 +1,9 @@
 """Host-side planning of a monocular bullet-time sweep (render_monocular_bt.py): the wander path of target
-cameras around one time step, each camera's source views, and the grouping of the sweep into batched calls of
-render_image.render_multi_image_mono.
+cameras around one time step or the stabilised path of the whole video, each camera's source views, and the grouping
+of the sweep into batched calls of render_image.render_multi_image_mono.
 
-numpy only, like the reference's data loader: this is per-sweep set-up, not the hot path.
+numpy (and cv2's Gaussian filter for the stabilised path), like the reference's data loader: this is per-sweep
+set-up, not the hot path.
 """
 
 import numpy as np
@@ -28,6 +29,29 @@ def wander_path(c2w, num_frames=50, max_disp=48.0):
     render_pose = np.dot(ref_pose, i_pose)
     out.append(np.concatenate([render_pose[:3, :], hwf], 1))
   return out
+
+
+def stabilization_path(poses, k_size=45):
+  """The stabilised camera path (llff_data_utils.py:453-497, render_idx < 0): poses float32 [N,3,5] (the recentred
+  llff poses, mono_scene.load_cameras) -> float32 [N,3,5], one pose per frame.  The first two rotation columns and
+  the centre are smoothed over the frames with cv2's k_size-tap Gaussian (its default sigma and reflected border),
+  the two columns are renormalised and the third is their cross product; every pose carries frame 0's hwf column.
+  The same cv2 and float32 numpy calls as the reference, so the poses are its render_poses bit for bit."""
+  import cv2
+  hwf = poses[0, :, 4:5]
+  inp = np.array([np.concatenate([p[:3, 0:1], p[:3, 1:2], p[:3, 3:4]], axis=-1) for p in poses])
+  kernel = cv2.getGaussianKernel(ksize=k_size, sigma=-1)
+  r1 = cv2.filter2D(inp[:, :, 0], -1, kernel)
+  r2 = cv2.filter2D(inp[:, :, 1], -1, kernel)
+  r1 = r1 / np.linalg.norm(r1, axis=-1, keepdims=True)
+  r2 = r2 / np.linalg.norm(r2, axis=-1, keepdims=True)
+  t = cv2.filter2D(inp[:, :, 2], -1, kernel)
+  out = []
+  for i in range(len(poses)):
+    r3 = np.cross(r1[i], r2[i])
+    pose = np.concatenate([r1[i, :, None], r2[i, :, None], r3[:, None], t[i, :, None]], axis=-1)
+    out.append(np.concatenate([pose[:3, :], hwf], 1))
+  return np.array(out).astype(np.float32)
 
 
 def _nearest_by_dist(tar_pose, ref_poses):
@@ -75,19 +99,25 @@ def select_source_views(render_pose, train_poses, src_vv_c2w, render_idx, num_so
   return ([int(i) for i in temporal], [int(i) for i in vv], [int(i) for i in static])
 
 
-def group_cameras(selections, max_cameras=MAX_CAMERAS, max_pool=MAX_POOL):
+def group_cameras(selections, max_cameras=MAX_CAMERAS, max_pool=MAX_POOL, frames=None):
   """Split a sweep into consecutive groups of cameras that one render_multi_image_mono call can take.
 
-  selections: per camera, (temporal_ids, vv_ids, static_ids) as select_source_views returns them.  Returns a list
-  of (start, stop) ranges, in order, covering every camera: each group holds at most max_cameras cameras, and its
-  dynamic pool (the temporal views and the union of the virtual views) and its static pool (the union of the
-  static views) hold at most max_pool views each."""
+  selections: per camera, (temporal_ids, vv_ids, static_ids) as select_source_views returns them, or None for a
+  camera that is not rendered; frames: per camera, the frame whose time it is rendered at (None: one frame for all).
+  Returns a list of (start, stop) ranges, in order, covering every rendered camera: each group holds at most
+  max_cameras cameras of one frame, and its dynamic pool (the temporal views and the union of the virtual views) and
+  its static pool (the union of the static views) hold at most max_pool views each."""
   groups, start = [], 0
   n = len(selections)
   while start < n:
+    if selections[start] is None:
+      start += 1
+      continue
     dy, st = set(), set()
     stop = start
-    while stop < n and stop - start < max_cameras:
+    while stop < n and stop - start < max_cameras and selections[stop] is not None:
+      if frames is not None and frames[stop] != frames[start]:
+        break
       t, vv, s = selections[stop]
       dy2 = dy | {("t", i) for i in t} | {("vv", j) for j in vv}
       st2 = st | set(s)

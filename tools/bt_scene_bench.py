@@ -1,16 +1,18 @@
-"""A monocular bullet-time sweep from files, two ways, on one GPU.
+"""A monocular bullet-time sweep or stabilised video from files, two ways, on one GPU.
 
-  python tools/bt_scene_bench.py [--cameras 50] [--frames 30] [--render-idx 15] [--reps 1]
+  python tools/bt_scene_bench.py [--cameras 50] [--frames 30] [--render-idx 15] [--reps 1] [--stabilized]
 
 A synthetic scene is written to a temporary `dense` folder (288x512 frames and virtual views as PNG, 1-channel
 dynamic masks) and swept with render_monocular_bt.py's configuration (configs/test_kid-running.txt: 7 source views,
 max_range 10, 3 virtual views, mask_src_view) at 64 samples, chunks of 8192 rays, with a randomly initialised
-model.
+model.  --stabilized renders the stabilised video instead (render_idx -1): cameras 3 .. n-4 of the smoothed input
+path, each at its own frame's time with that frame's virtual views, one camera per group.
 
   scene      BulletTimeScene: the scene is read once (timed on its own), then the sweep from the device-resident
              scene: per group of up to 16 cameras the pools and rays on the device, one encoder pass per pool, one
              render_multi_image_mono, the frame kernel and one copy of the uint8 frames.
-  reference  the script's flow, camera by camera: a cv2 restatement of DynamicVideoDataset.__getitem__ (its ground
+  reference  the script's flow, camera by camera: a cv2 restatement of DynamicVideoDataset.__getitem__ (with
+             render_idx set to the camera's frame for the stabilised video; its ground
              truth, 7 temporal frames, 3 virtual views, 15 static frames and their masks, read from the PNGs),
              RaySamplerSingleImage.get_all, the encoder over the camera's 10 + 15 views, render_single_image_mono and
              the numpy uint8 conversion.
@@ -39,7 +41,8 @@ if ROOT not in sys.path:
 
 def parse():
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-  ap.add_argument("--cameras", type=int, default=50, help="cameras of the reference arm (the scene arm sweeps 50)")
+  ap.add_argument("--cameras", type=int, default=50,
+                  help="at most this many cameras in the reference arm (the scene arm renders them all)")
   ap.add_argument("--frames", type=int, default=30)
   ap.add_argument("--render-idx", type=int, default=15)
   ap.add_argument("--H", type=int, default=288)
@@ -48,6 +51,7 @@ def parse():
   ap.add_argument("--chunk", type=int, default=8192)
   ap.add_argument("--reps", type=int, default=1, help="timed sweeps per arm (after one warm-up sweep each)")
   ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
+  ap.add_argument("--stabilized", action="store_true", help="the stabilised video (render_idx -1)")
   return ap.parse_args()
 
 
@@ -113,8 +117,8 @@ def main():
   model.feature_net_st = ResNet().to(dev).eval().requires_grad_(False)
   args.anti_alias_pooling, args.mask_rgb = 1, 1
   vars(args).update(training_height=a.H, num_source_views=7, max_range=10, num_vv=3, mask_src_view=True,
-                    render_idx=a.render_idx, N_samples=a.samples, N_importance=0, chunk_size=a.chunk,
-                    inv_uniform=True, white_bkgd=False)
+                    render_idx=-1 if a.stabilized else a.render_idx, N_samples=a.samples, N_importance=0,
+                    chunk_size=a.chunk, inv_uniform=True, white_bkgd=False)
   P = Projector(dev)
 
   def sync_time():
@@ -130,6 +134,8 @@ def main():
     plan, cams = scene.plan, scene.cams
     files = cams["rgb_files"]
     H, W = scene.H, scene.W
+    rendered = [c for lo, hi in scene.groups for c in range(lo, hi)]
+    ref_cams = rendered[:a.cameras]
 
     def scene_sweep():
       return np.concatenate([f for _, f in scene.sweep(model, P, args)])
@@ -140,36 +146,37 @@ def main():
     def item(k):
       """DynamicVideoDataset.__getitem__ restated with cv2 (render_monocular_bt.py:96-259)."""
       t, vv, st = plan["selections"][k]
+      frame = plan["frames"][k]
       read_rgb(files[min(k, len(files) - 1)])  # the unused ground truth
       src = [read_rgb(files[f]) for f in t]
       src_cams = [scene._cam_rows[f] for f in t]
-      vdir = os.path.join(root, "source_virtual_views_%dx%d" % (W, H), "%05d" % a.render_idx)
+      vdir = os.path.join(root, "source_virtual_views_%dx%d" % (W, H), "%05d" % frame)
       for j in vv:
         src.append(read_rgb(os.path.join(vdir, "%02d.png" % j)))
         src_cams.append(np.concatenate(([H, W], plan["render_K"][k].reshape(-1),
-                                        cams["vv_c2w"][a.render_idx, j].reshape(-1))).astype(np.float32))
+                                        cams["vv_c2w"][frame, j].reshape(-1))).astype(np.float32))
       static = []
-      for f in st:
-        m = cv2.imread(os.path.join(root, "dynamic_masks", "%d.png" % f), cv2.IMREAD_UNCHANGED)
+      for s in st:
+        m = cv2.imread(os.path.join(root, "dynamic_masks", "%d.png" % s), cv2.IMREAD_UNCHANGED)
         m = cv2.resize(m.astype(np.float32) / 255.0, (W, H), interpolation=cv2.INTER_NEAREST)
-        static.append(read_rgb(files[f]) * (m[..., None] if m.ndim == 2 else m))
+        static.append(read_rgb(files[s]) * (m[..., None] if m.ndim == 2 else m))
       return dict(camera=torch.from_numpy(plan["cameras"][k])[None],
                   depth_range=torch.from_numpy(scene.depth_range)[None],
                   src_rgbs=torch.from_numpy(np.stack(src))[None], src_cameras=torch.from_numpy(np.stack(src_cams))[None],
                   static_src_rgbs=torch.from_numpy(np.stack(static))[None],
                   static_src_cameras=torch.from_numpy(scene._cam_rows[st])[None])
 
-    ref_time = torch.tensor([a.render_idx / float(a.frames)], dtype=torch.float64, device=dev)
-
     def reference_sweep():
       out = []
-      for k in range(a.cameras):
+      for k in ref_cams:
+        frame = plan["frames"][k]
+        ref_time = torch.tensor([frame / float(a.frames)], dtype=torch.float64, device=dev)
         smp = sr.RaySamplerSingleImage(item(k), dev)
         rb = smp.get_all()
         with torch.no_grad():
           ref = model.feature_net(rb["src_rgbs"].squeeze(0).permute(0, 3, 1, 2))[0]
           st = model.feature_net_st(rb["static_src_rgbs"].squeeze(0).permute(0, 3, 1, 2))[0]
-          ret = render_single_image_mono((a.render_idx, None), (ref_time, None), (list(OFFSETS), None), smp, rb,
+          ret = render_single_image_mono((frame, None), (ref_time, None), (list(OFFSETS), None), smp, rb,
                                          model, P, a.chunk, a.samples, args, inv_uniform=True, det=True,
                                          featmaps=(ref, None, st), is_train=False, num_vv=3)
         x = ret["outputs_coarse_ref"]["rgb"].cpu().numpy()
@@ -178,7 +185,7 @@ def main():
       return np.stack(out)
 
     def loader_only():
-      for k in range(a.cameras):
+      for k in ref_cams:
         item(k)
 
     def timed(fn):
@@ -195,16 +202,18 @@ def main():
       dt, f_ref = timed(reference_sweep)
       t_ref.append(dt)
       t_load.append(timed(loader_only)[0])
-    same = np.array_equal(f_scene[:a.cameras], f_ref)
-    diff = int(np.abs(f_scene[:a.cameras].astype(np.int32) - f_ref.astype(np.int32)).max())
+    n_ref = len(ref_cams)
+    same = np.array_equal(f_scene[:n_ref], f_ref)
+    diff = int(np.abs(f_scene[:n_ref].astype(np.int32) - f_ref.astype(np.int32)).max())
     print(json.dumps({
-        "what": "bullet-time sweep from files: %d frames at %dx%d, 7+3 dynamic / 15 static views, mask_src_view, %d "
-                "samples, chunk %d, %s" % (a.frames, a.W, a.H, a.samples, a.chunk, a.precision),
+        "what": "%s from files: %d frames at %dx%d, 7+3 dynamic / 15 static views, mask_src_view, %d samples, "
+                "chunk %d, %s" % ("stabilised video" if a.stabilized else "bullet-time sweep", a.frames, a.W, a.H,
+                                  a.samples, a.chunk, a.precision),
         "groups": [hi - lo for lo, hi in scene.groups], "scene_load_s": load_s, "scene_mb": scene.nbytes / 1e6,
-        "scene_sweep_s_50_cameras": min(t_scene), "scene_all_reps_s": t_scene,
-        "reference_cameras": a.cameras, "reference_sweep_s": min(t_ref), "reference_all_reps_s": t_ref,
+        "scene_sweep_s_%d_cameras" % len(rendered): min(t_scene), "scene_all_reps_s": t_scene,
+        "reference_cameras": n_ref, "reference_sweep_s": min(t_ref), "reference_all_reps_s": t_ref,
         "reference_loader_s": min(t_load), "reference_loader_share": min(t_load) / min(t_ref),
-        "speedup_per_camera": (min(t_ref) / a.cameras) / (min(t_scene) / 50),
+        "speedup_per_camera": (min(t_ref) / n_ref) / (min(t_scene) / len(rendered)),
         "frames_equal": bool(same), "frames_max_abs_diff": diff,
         "timing": "host clock around device-synchronised work, best of the reps, after one warm-up of each arm",
         "gpu": gpu_info(dev.index),

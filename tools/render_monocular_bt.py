@@ -7,9 +7,11 @@
       [--anti_alias_pooling 1] [--mask_rgb 1] [--occ_weights_mode 0]
 
 The options are the keys of the reference's configs (configs/test_*.txt) that the script reads.  The checkpoint loads
-through dynibar_b200.model.model_from_checkpoints (mono=True).  Writes rgb_out/{i}.png, i = 0..49, under
+through dynibar_b200.model.model_from_checkpoints (mono=True).  Writes rgb_out/{i}.png under
 <out>/<eval_dataset>/<expname>/<render_idx>/<scene>_<step:06d>/videos/, as the script does (RGB PNGs, cropped by 3 %),
-and prints the sweep's wall time split into load, encoder, render and write.
+and prints the wall time split into load, encoder, render and write.  A render_idx >= 0 renders the bullet-time sweep
+of that frame, i = 0..49; a negative render_idx renders the stabilised video of the n frames, camera i at frame i's
+time, i = 3..n-4 (each camera needs the frames i-3 .. i+3).
 """
 
 import argparse
@@ -100,9 +102,11 @@ def main(argv=None):
     t["render"] += t3 - t2
     t["write"] += t4 - t3
   total = now() - t_sweep
-  print("bullet-time sweep of frame %d: %d cameras in %d groups; load %.3f s, sweep %.3f s (encoder %.3f s, render "
-        "%.3f s, write %.3f s)" % (args.render_idx, scene.plan["cameras"].shape[0], len(scene), t_load, total,
-                                   t["encoder"], t["render"], t["write"]))
+  what = ("stabilised video of %d frames" % scene.num_frames if scene.stabilized
+          else "bullet-time sweep of frame %d" % args.render_idx)
+  print("%s: %d cameras in %d groups; load %.3f s, sweep %.3f s (encoder %.3f s, render %.3f s, write %.3f s)"
+        % (what, sum(hi - lo for lo, hi in scene.groups), len(scene), t_load, total, t["encoder"], t["render"],
+           t["write"]))
   return out_dir
 
 
