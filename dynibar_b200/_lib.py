@@ -128,7 +128,9 @@ SIGNATURES = {
     "dyn_motion_mlp_train_forward": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _i, _vp]),
     "dyn_motion_mlp_backward": (_i, [_vp, _vp, _vp, _i, _vp, _sz, _vp, _vp, _i, _vp]),
     "dyn_composite_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
-    "dyn_project_gather_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "dyn_project_gather_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp,
+                                         _sz, _vp]),
+    "dyn_project_gather_backward_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "dyn_net_train_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "dyn_net_backward_scratch_bytes": (_sz, [_i, _i, _i, _i]),
     "dyn_net_dynamic_train_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp, _vp, _sz, _i, _vp]),

@@ -101,11 +101,13 @@ class _ProjectGather(torch.autograd.Function):
     g_xyz = torch.empty_like(xyz) if need_xyz else None
     gf = f32c(g_feat)
     with torch.cuda.device(fm.device):
+      nbytes = int(lib.dyn_project_gather_backward_workspace_bytes(V, R, S, h, w)) if need_maps else 0
+      ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=fm.device)
       check(lib.dyn_project_gather_backward(ptr(xyz_st), ptr(xyz) if ctx.has_xyz else None, ptr(imgs),
                                             ctx.cams.data_ptr(), ptr(fm), ptr(gf),
                                             V, R, S, H, W, Cc, h, w,
                                             ptr(g_maps) if need_maps else None,
-                                            ptr(g_xyz) if need_xyz else None, stream()))
+                                            ptr(g_xyz) if need_xyz else None, ws.data_ptr(), nbytes, stream()))
     return None, g_xyz, g_maps, None, None, None
 
 

@@ -11,8 +11,12 @@
 //   dyn_expected_scene_flow      exp_sf of the mv fine pass (render_ray.py:585-595), forward and backward
 //
 // fp32 throughout; one warp per ray for the compositing scan (reverse multiplicative scan for the
-// transmittance), atomicAdd scatter for the feature-map gradient.  The MLP / ray-transformer backward is not
-// built yet (DESIGN.md, "next").
+// transmittance).  No float atomics: the feature-map gradient is a gather -- each (view, point) pair gets the key
+// of its bilinear footprint's north-west cell, a stable radix sort groups the pairs by cell in pair order, and one
+// thread per (view, channel, texel) adds the four cells that reach its texel in a fixed order (the scheme of
+// splat.cu).  The same inputs give the same bits, however many samples land on one texel.
+#include <cub/device/device_radix_sort.cuh>
+
 #include "common.cuh"
 #include "geometry.cuh"
 
@@ -127,13 +131,15 @@ __global__ void composite_backward_kernel(const float* __restrict__ raw_a, const
   }
 }
 
-// one thread per (view, point): scatter into the feature-map gradient (reference layout [V,C,h,w]) and
-// accumulate d/d(u,v) -> d/d xyz of that view's displaced point.  g_feat [N,V,3+C] (rgb channels first).
+// one thread per (view, point) pair m = v N + point: d/d(u,v) -> d/d xyz of that view's displaced point, and (keys
+// non-null) the pair's feature-map cell key, its index and its bilinear weights (ax, ay, bx, by) for
+// map_grad_gather_kernel.  g_feat [N,V,3+C] (rgb channels first).
 __global__ void gather_backward_kernel(const float* __restrict__ xyz, const float* __restrict__ xyz_st,
                                        const float* __restrict__ featmaps, const float* __restrict__ rgbs,
                                        const float* __restrict__ g_feat, const __grid_constant__ ViewCams cams,
                                        int V, long long N, int H, int W, int C, int h, int w,
-                                       float* __restrict__ g_maps, float* __restrict__ g_xyz) {
+                                       unsigned* __restrict__ keys, unsigned* __restrict__ ids,
+                                       float4* __restrict__ wts, float* __restrict__ g_xyz) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * V) return;
   const int v = (int)(idx / N);
@@ -157,14 +163,22 @@ __global__ void gather_backward_kernel(const float* __restrict__ xyz, const floa
     const float ax = fx - x0f, ay = fy - y0f, bx = (x0f + 1.f) - fx, by = (y0f + 1.f) - fy;
     const bool in00 = x0 >= 0 && x0 < w && y0 >= 0 && y0 < h, in01 = x0 + 1 >= 0 && x0 + 1 < w && y0 >= 0 && y0 < h;
     const bool in10 = x0 >= 0 && x0 < w && y0 + 1 >= 0 && y0 + 1 < h, in11 = x0 + 1 >= 0 && x0 + 1 < w && y0 + 1 >= 0 && y0 + 1 < h;
+    if (keys != nullptr) {
+      const unsigned cells = (unsigned)(h + 1) * (w + 1);
+      // compared in float first: NaN, inf and far-off taps never reach the int conversion
+      const bool reach = fx >= -1.f && fx < (float)w && fy >= -1.f && fy < (float)h;
+      keys[idx] = reach ? (unsigned)v * cells + (unsigned)(y0 + 1) * (w + 1) + (unsigned)(x0 + 1) : cells * V;
+      ids[idx] = (unsigned)idx;
+      wts[idx] = make_float4(ax, ay, bx, by);
+    }
     for (int c = 0; c < C; ++c) {
       const float gc = g[3 + c];
       const long long base = ((long long)v * C + c) * h * w;
       float m00 = 0.f, m01 = 0.f, m10 = 0.f, m11 = 0.f;
-      if (in00) { m00 = featmaps[base + (long long)y0 * w + x0]; if (g_maps) atomicAdd(g_maps + base + (long long)y0 * w + x0, gc * bx * by); }
-      if (in01) { m01 = featmaps[base + (long long)y0 * w + x0 + 1]; if (g_maps) atomicAdd(g_maps + base + (long long)y0 * w + x0 + 1, gc * ax * by); }
-      if (in10) { m10 = featmaps[base + (long long)(y0 + 1) * w + x0]; if (g_maps) atomicAdd(g_maps + base + (long long)(y0 + 1) * w + x0, gc * bx * ay); }
-      if (in11) { m11 = featmaps[base + (long long)(y0 + 1) * w + x0 + 1]; if (g_maps) atomicAdd(g_maps + base + (long long)(y0 + 1) * w + x0 + 1, gc * ax * ay); }
+      if (in00) m00 = featmaps[base + (long long)y0 * w + x0];
+      if (in01) m01 = featmaps[base + (long long)y0 * w + x0 + 1];
+      if (in10) m10 = featmaps[base + (long long)(y0 + 1) * w + x0];
+      if (in11) m11 = featmaps[base + (long long)(y0 + 1) * w + x0 + 1];
       dfx += gc * ((m01 - m00) * by + (m11 - m10) * ay);
       dfy += gc * ((m10 - m00) * bx + (m11 - m01) * ax);
     }
@@ -199,6 +213,92 @@ __global__ void gather_backward_kernel(const float* __restrict__ xyz, const floa
     for (int k = 0; k < 3; ++k)
       o[k] = su * (P[k] - live * u0 * P[8 + k]) + sv * (P[4 + k] - live * v0 * P[8 + k]);
   }
+}
+
+// first / one-past-last sorted position of every occupied cell (both zeroed beforehand: empty cells are [0, 0))
+__global__ void map_cell_ranges_kernel(const unsigned* __restrict__ keys, long long n, unsigned invalid,
+                                       unsigned* __restrict__ start, unsigned* __restrict__ end) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned k = keys[i];
+  if (k >= invalid) return;
+  if (i == 0 || keys[i - 1] != k) start[k] = (unsigned)i;
+  if (i == n - 1 || keys[i + 1] != k) end[k] = (unsigned)(i + 1);
+}
+
+// g_maps [V,C,h,w], one thread per element: cells (x, y), (x-1, y), (x, y-1), (x-1, y-1) of view v reach texel (x, y)
+// through their pairs' NW, NE, SW, SE corner, in that order; within a cell the pairs come in pair order.
+__global__ void map_grad_gather_kernel(const float* __restrict__ g_feat, const float4* __restrict__ wts,
+                                       const unsigned* __restrict__ order, const unsigned* __restrict__ start,
+                                       const unsigned* __restrict__ end, int V, long long N, int C, int h, int w,
+                                       float* __restrict__ g_maps) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)V * C * h * w) return;
+  const int x = (int)(idx % w), y = (int)((idx / w) % h);
+  const long long vc = idx / ((long long)w * h);
+  const int c = (int)(vc % C), v = (int)(vc / C);
+  const unsigned cell0 = (unsigned)v * (h + 1) * (w + 1);
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int cy = y - (k >> 1), cx = x - (k & 1);  // the cell's north-west corner (-1 allowed)
+    const unsigned cell = cell0 + (unsigned)(cy + 1) * (w + 1) + (unsigned)(cx + 1);
+    const unsigned e = end[cell];
+    for (unsigned i = start[cell]; i < e; ++i) {
+      const unsigned m = order[i];
+      const long long pt = (long long)m - (long long)v * N;
+      const float gc = g_feat[(pt * V + v) * (long long)(3 + C) + 3 + c];
+      const float4 q = wts[m];  // ax, ay, bx, by
+      const float fx = (k & 1) ? q.x : q.z, fy = (k >> 1) ? q.y : q.w;
+      s += gc * fx * fy;
+    }
+  }
+  g_maps[idx] = s;
+}
+
+int map_key_bits(long long invalid) {
+  int bits = 1;
+  while ((1ll << bits) <= invalid) ++bits;
+  return bits;
+}
+
+size_t align256_b(size_t n) { return (n + 255) & ~(size_t)255; }
+
+// workspace of the feature-map gradient: per pair keys, indices, weights; cell ranges; the sort's temporary storage
+struct MapGradWs {
+  unsigned *keys, *keys_sorted, *ids, *order, *start, *end;
+  float4* wts;
+  void* sort_tmp;
+  size_t sort_bytes, total;
+};
+
+bool map_grad_shape_ok(long long V, long long N, long long h, long long w) {
+  // keys, pair indices and sorted positions are 32-bit; the sort takes an int count
+  return V >= 1 && N >= 1 && h >= 1 && w >= 1 && V * N < (1ll << 31) && V * (h + 1) * (w + 1) < (1ll << 31);
+}
+
+// NULL base: sizes only
+int map_grad_ws(int V, long long N, int h, int w, void* base, MapGradWs* ws) {
+  const size_t n = (size_t)V * N, cells = (size_t)V * (h + 1) * (w + 1);
+  size_t sort_bytes = 0;
+  cudaError_t err = cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned*)nullptr, (unsigned*)nullptr,
+                                                    (unsigned*)nullptr, (unsigned*)nullptr, (int)n, 0,
+                                                    map_key_bits((long long)cells));
+  if (err != cudaSuccess) return fail(DYN_E_CUDA, "gather backward: radix sort size query: %s", cudaGetErrorString(err));
+  char* p = (char*)base;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { void* r = p ? p + off : nullptr; off += align256_b(bytes); return r; };
+  ws->keys = (unsigned*)take(n * 4);
+  ws->keys_sorted = (unsigned*)take(n * 4);
+  ws->ids = (unsigned*)take(n * 4);
+  ws->order = (unsigned*)take(n * 4);
+  ws->wts = (float4*)take(n * 16);
+  ws->start = (unsigned*)take(cells * 4 * 2);
+  ws->end = ws->start ? ws->start + cells : nullptr;
+  ws->sort_tmp = take(sort_bytes);
+  ws->sort_bytes = sort_bytes;
+  ws->total = off;
+  return DYN_OK;
 }
 
 // Trajectory combination (compute_traj_pts + the displacements built from it, render_ray.py:361-369, :462-500,
@@ -388,19 +488,49 @@ int dyn_composite_vanilla_backward(const float* raw, const float* z_vals, const 
   return DYN_OK;
 }
 
+size_t dyn_project_gather_backward_workspace_bytes(int V, int R, int S, int h, int w) {
+  const long long N = (long long)R * S;
+  if (!map_grad_shape_ok(V, N, h, w)) return 0;
+  MapGradWs ws;
+  return map_grad_ws(V, N, h, w, nullptr, &ws) == DYN_OK ? ws.total : 0;
+}
+
 int dyn_project_gather_backward(const float* xyz_st, const float* xyz, const float* src_rgbs, const float* src_cams,
                                 const float* featmaps, const float* g_rgb_feat, int V, int R, int S, int H, int W, int C,
-                                int h, int w, float* g_featmaps, float* g_xyz, void* stream) {
+                                int h, int w, float* g_featmaps, float* g_xyz, void* workspace, size_t workspace_bytes,
+                                void* stream) {
   if (R == 0) return DYN_OK;
-  DYN_CHECK_ARG(xyz_st && src_rgbs && src_cams && featmaps && g_rgb_feat && (g_featmaps || g_xyz));
+  DYN_CHECK_ARG(xyz_st && src_rgbs && src_cams && featmaps && g_rgb_feat && (g_featmaps || g_xyz) && S >= 1 && V >= 1);
   cudaStream_t st = (cudaStream_t)stream;
+  const long long N = (long long)R * S;
+  MapGradWs ws{};
+  if (g_featmaps) {
+    if (!map_grad_shape_ok(V, N, h, w))
+      return fail(DYN_E_INVALID, "gather backward: %d views x %lld points on %d x %d maps exceed 32-bit indices", V, N,
+                  h, w);
+    int rc = map_grad_ws(V, N, h, w, nullptr, &ws);
+    if (rc) return rc;
+    if (workspace == nullptr || workspace_bytes < ws.total)
+      return fail(DYN_E_WORKSPACE, "gather backward: workspace of %zu bytes, %zu needed", workspace_bytes, ws.total);
+    map_grad_ws(V, N, h, w, workspace, &ws);
+  }
   ViewCams vc;
   int rc = build_view_cams(src_cams, V, nullptr, st, &vc);
   if (rc) return rc;
-  const long long N = (long long)R * S;
-  if (g_featmaps) DYN_CUDA(cudaMemsetAsync(g_featmaps, 0, (size_t)V * C * h * w * sizeof(float), st));
   gather_backward_kernel<<<cdiv(N * V, 256), 256, 0, st>>>(xyz, xyz_st, featmaps, src_rgbs, g_rgb_feat, vc, V, N, H, W,
-                                                           C, h, w, g_featmaps, g_xyz);
+                                                           C, h, w, ws.keys, ws.ids, ws.wts, g_xyz);
+  DYN_LAUNCH_CHECK();
+  if (g_featmaps == nullptr) return DYN_OK;
+  const long long n = (long long)V * N, cells = (long long)V * (h + 1) * (w + 1);
+  size_t tmp = ws.sort_bytes;
+  DYN_CUDA(cub::DeviceRadixSort::SortPairs(ws.sort_tmp, tmp, ws.keys, ws.keys_sorted, ws.ids, ws.order, (int)n, 0,
+                                           map_key_bits(cells), st));
+  ++g_launches;
+  DYN_CUDA(cudaMemsetAsync(ws.start, 0, (size_t)cells * 2 * sizeof(unsigned), st));
+  map_cell_ranges_kernel<<<cdiv(n, 256), 256, 0, st>>>(ws.keys_sorted, n, (unsigned)cells, ws.start, ws.end);
+  DYN_LAUNCH_CHECK();
+  map_grad_gather_kernel<<<cdiv((long long)V * C * h * w, 256), 256, 0, st>>>(g_rgb_feat, ws.wts, ws.order, ws.start,
+                                                                              ws.end, V, N, C, h, w, g_featmaps);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
 }

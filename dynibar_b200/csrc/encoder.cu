@@ -248,7 +248,8 @@ int in_norm(const float* x, const float* P, int gw, int gb, const float* residua
 //   dYt [rows, 64]       = dY (NCHW) with rows = (n, oy, ox)
 //   col [rows, Cin k k]  = im2col(X) with the forward's reflect padding / stride, column = ci k k + ky k + kx
 //                          (the layout of conv.weight [co][ci][ky][kx], so dW = dYt^T col is the weight gradient as is)
-//   dcol = dYt W  ->  col2im: scatter-add through the SAME index map (the adjoint of reflect padding for free)
+//   dcol = dYt W  ->  col2im in gather form: each input pixel adds the dcol entries that the SAME index map sends
+//                          to it (the adjoint of reflect padding), in a fixed order -- no float atomics
 // ---------------------------------------------------------------------------
 __global__ void enc_nchw_to_rows_kernel(const float* __restrict__ x, int C, int hw, long long rows,
                                         float* __restrict__ out) {
@@ -260,9 +261,9 @@ __global__ void enc_nchw_to_rows_kernel(const float* __restrict__ x, int C, int 
   out[idx] = x[(n * C + c) * hw + pix];
 }
 
-// mode 0: col[r, j] = X[...];  mode 1: atomicAdd(dX[...], col[r, j])
-__global__ void enc_im2col_kernel(float* __restrict__ x, int Cin, int H, int W, int Ho, int Wo, int k, int stride,
-                                  int pad, long long rows, float* __restrict__ col, int mode) {
+// col[r, j] = X[...]
+__global__ void enc_im2col_kernel(const float* __restrict__ x, int Cin, int H, int W, int Ho, int Wo, int k, int stride,
+                                  int pad, long long rows, float* __restrict__ col) {
   const int K = Cin * k * k;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= rows * K) return;
@@ -272,9 +273,47 @@ __global__ void enc_im2col_kernel(float* __restrict__ x, int Cin, int H, int W, 
   const int ox = (int)(r % Wo), oy = (int)((r / Wo) % Ho);
   const long long n = r / ((long long)Wo * Ho);
   const int iy = reflect_idx(oy * stride + ky - pad, H), ix = reflect_idx(ox * stride + kx - pad, W);
-  float* p = x + ((n * Cin + ci) * H + iy) * W + ix;
-  if (mode == 0) col[idx] = *p;
-  else atomicAdd(p, col[idx]);
+  col[idx] = x[((n * Cin + ci) * H + iy) * W + ix];
+}
+
+// The padded coordinates along one axis that reflect_idx sends to i (pads are < n): i itself, -i (top / left
+// reflection) and 2 (n - 1) - i (bottom / right reflection).  Returns how many there are (1 to 3).
+__device__ __forceinline__ int reflect_preimages(int i, int n, int p[3]) {
+  int c = 0;
+  p[c++] = i;
+  if (i > 0) p[c++] = -i;
+  if (i < n - 1) p[c++] = 2 * (n - 1) - i;
+  return c;
+}
+
+// col2im, the adjoint of enc_im2col_kernel: dX[n, ci, iy, ix] (+)= sum of dcol[r, j] over the (r, j) whose tap reads
+// (iy, ix).  One thread per input pixel; the sum runs over ky, the row preimages, kx, the column preimages, in that
+// order.
+__global__ void enc_col2im_kernel(const float* __restrict__ col, int Cin, int H, int W, int Ho, int Wo, int k,
+                                  int stride, int pad, long long total, float* __restrict__ dx, int acc) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int ix = (int)(idx % W), iy = (int)((idx / W) % H);
+  const long long nc = idx / ((long long)W * H);
+  const int ci = (int)(nc % Cin);
+  const long long n = nc / Cin;
+  const int K = Cin * k * k;
+  int py[3], px[3];
+  const int ny = reflect_preimages(iy, H, py), nx = reflect_preimages(ix, W, px);
+  float s = 0.f;
+  for (int ky = 0; ky < k; ++ky)
+    for (int a = 0; a < ny; ++a) {
+      const int ty = py[a] + pad - ky;
+      if (ty < 0 || ty % stride != 0 || ty / stride >= Ho) continue;
+      const long long rrow = (n * Ho + ty / stride) * Wo;
+      for (int kx = 0; kx < k; ++kx)
+        for (int b = 0; b < nx; ++b) {
+          const int tx = px[b] + pad - kx;
+          if (tx < 0 || tx % stride != 0 || tx / stride >= Wo) continue;
+          s += col[(rrow + tx / stride) * K + (ci * k + ky) * k + kx];
+        }
+    }
+  dx[idx] = acc ? dx[idx] + s : s;
 }
 
 __global__ void enc_relu_mask_kernel(float* __restrict__ g, const float* __restrict__ y, long long n) {
@@ -283,12 +322,13 @@ __global__ void enc_relu_mask_kernel(float* __restrict__ g, const float* __restr
 }
 
 // InstanceNorm2d backward, one block per (image, channel) plane: xh = (x - mean) rstd,
-// dx = rstd gamma (dy - mean(dy) - xh mean(dy xh)); dgamma += sum dy xh, dbeta += sum dy.  dx may alias dy.
+// dx = rstd gamma (dy - mean(dy) - xh mean(dy xh)); the plane's sum dy xh goes to part[n, c] and its sum dy to
+// part[n, C + c] (launch_red_add adds them over the images in order into dgamma, dbeta).  dx may alias dy.
 __global__ void __launch_bounds__(256) enc_in_bwd_kernel(const float* __restrict__ x, const float* dy,
                                                          const float* __restrict__ mean,
                                                          const float* __restrict__ rstd,
                                                          const float* __restrict__ gamma, int hw, int C, float* dx,
-                                                         float* __restrict__ dgamma, float* __restrict__ dbeta) {
+                                                         float* __restrict__ part) {
   const long long plane = blockIdx.x;
   const int c = (int)(plane % C);
   const float* xp = x + plane * hw;
@@ -315,8 +355,9 @@ __global__ void __launch_bounds__(256) enc_in_bwd_kernel(const float* __restrict
     op[i] = k * (gp[i] - mg - xh * mgx);
   }
   if (threadIdx.x == 0) {
-    atomicAdd(dgamma + c, (float)a2[0]);
-    atomicAdd(dbeta + c, (float)a1[0]);
+    const long long n = plane / C;
+    part[n * 2 * C + c] = (float)a2[0];
+    part[n * 2 * C + C + c] = (float)a1[0];
   }
 }
 
@@ -348,6 +389,7 @@ struct EncScratch {
   float *g2a, *g2b;        // half-resolution gradients
   float *g4a, *g4b, *g4c;  // quarter-resolution gradients
   float *dyt, *col, *img;
+  float* red;              // reduction scratch (train_gemm.cuh)
 };
 
 size_t enc_scratch_alloc(char* base, int N, int H, int W, int H2, int W2, int H4, int W4, EncScratch* q) {
@@ -367,6 +409,7 @@ size_t enc_scratch_alloc(char* base, int N, int H, int W, int H2, int W2, int H4
   const size_t c_stem = r2 * 147, c_33 = r4 * 576;
   q->col = take(c_stem > c_33 ? c_stem : c_33);
   q->img = take(tc_grad_in_scratch_bytes() / sizeof(float));
+  q->red = take(kRedFloats > 2LL * N * 64 ? (size_t)kRedFloats : (size_t)2 * N * 64);
   return off;
 }
 
@@ -382,15 +425,16 @@ struct ConvBwd {
     const int K = Cin * k * k;
     enc_nchw_to_rows_kernel<<<cdiv(rows * 64, 256), 256, 0, st>>>(dY, 64, Ho * Wo, rows, q.dyt);
     DYN_LAUNCH_CHECK();
-    enc_im2col_kernel<<<cdiv(rows * K, 256), 256, 0, st>>>(X, Cin, H, W, Ho, Wo, k, stride, pad, rows, q.col, 0);
+    enc_im2col_kernel<<<cdiv(rows * K, 256), 256, 0, st>>>(X, Cin, H, W, Ho, Wo, k, stride, pad, rows, q.col);
     DYN_LAUNCH_CHECK();
     for (int c0 = 0; c0 < K; c0 += 256) {  // dW[64, K] += dYt^T col
       const int wd = K - c0 < 256 ? K - c0 : 256;
       int rc;
       if (tc && tc_grad_w_ok(64, wd, rows)) {
-        rc = tc_grad_w(q.dyt, 64, 64, rows, q.col + c0, K, wd, nullptr, dW + c0, K, st);
+        rc = tc_grad_w(q.dyt, 64, 64, rows, q.col + c0, K, wd, nullptr, dW + c0, K, q.red, st);
       } else {
         GemmArgs g{q.dyt, q.col + c0, dW + c0, 64, wd, rows, 1, 64, K, 1, K, 1, 0};
+        g.red = q.red;
         rc = launch_gemm(g, true, st);
       }
       if (rc) return rc;
@@ -407,8 +451,9 @@ struct ConvBwd {
       }
       if (rc) return rc;
     }
-    if (zero_dx) DYN_CUDA(cudaMemsetAsync(dX, 0, (size_t)N * Cin * H * W * sizeof(float), st));
-    enc_im2col_kernel<<<cdiv(rows * K, 256), 256, 0, st>>>(dX, Cin, H, W, Ho, Wo, k, stride, pad, rows, q.col, 1);
+    const long long total = (long long)N * Cin * H * W;
+    enc_col2im_kernel<<<cdiv(total, 256), 256, 0, st>>>(q.col, Cin, H, W, Ho, Wo, k, stride, pad, total, dX,
+                                                        zero_dx ? 0 : 1);
     DYN_LAUNCH_CHECK();
     return DYN_OK;
   }
@@ -583,9 +628,10 @@ int dyn_encoder_backward(const float* params, size_t n_params, const float* imag
   const ConvBwd cb{st, precision == DYN_PREC_BF16, q, N};
   int rc;
   auto in_bwd = [&](const float* x, float* g, const float* stats, int gw, int gb, int hw) {
-    enc_in_bwd_kernel<<<N * 64, 256, 0, st>>>(x, g, stats, stats + N * 64, P + gw, hw, 64, g, dP + gw, dP + gb);
+    enc_in_bwd_kernel<<<N * 64, 256, 0, st>>>(x, g, stats, stats + N * 64, P + gw, hw, 64, g, q.red);
     DYN_LAUNCH_CHECK();
-    return DYN_OK;
+    const int rc2 = launch_red_add(q.red, N, 128, 1, 64, dP + gw, 64, true, st);
+    return rc2 ? rc2 : launch_red_add(q.red + 64, N, 128, 1, 64, dP + gb, 64, true, st);
   };
   auto relu_mask = [&](float* g, const float* y, long long n) {
     enc_relu_mask_kernel<<<cdiv(n, 256), 256, 0, st>>>(g, y, n);
@@ -601,7 +647,7 @@ int dyn_encoder_backward(const float* params, size_t n_params, const float* imag
   // out_conv (1x1, bias): db = sum over pixels; dW, d(o2)
   float* d_o = q.g4b;
   if ((rc = cb.run(g, H4, W4, P + L.outw, dP + L.outw, s.b[2].o, 64, H4, W4, 1, 1, 0, d_o, true))) return rc;
-  if ((rc = launch_colsum(q.dyt, 64, 64, (long long)N * hw4, dP + L.outb, st))) return rc;  // q.dyt = rows of g
+  if ((rc = launch_colsum(q.dyt, 64, 64, (long long)N * hw4, dP + L.outb, q.red, st))) return rc;  // q.dyt = rows of g
   // blocks 2, 1 (identity shortcuts), then block 0
   float* t = q.g4a;   // free again
   float* u = q.g4c;

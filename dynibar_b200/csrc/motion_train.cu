@@ -7,15 +7,15 @@
 //
 //   backward, fp32, one GEMM per product:
 //     dZ_i = dH_{i+1} * (out_i > 0)                    relu_mask_kernel
-//     dW_i += dZ_i^T in_i, db_i += colsum(dZ_i)        gemm_f32_kernel (split-K over the rows, atomicAdd)
+//     dW_i += dZ_i^T in_i, db_i += colsum(dZ_i)        gemm_f32_kernel (split-K over the rows: partials in order)
 //     dIn_i = dZ_i W_i                                  gemm_f32_kernel
 //     layer 5 reads cat([x0, out_4]): its dIn splits into a contribution to dx0 and dH
 //     d xyzt = PeriodicEmbed backward of dx0
 //
 // The gradients are ACCUMULATED into d_params (the caller zeroes it), in the same flat layout as the
-// parameter blob of the forward (motion_layout).  Split-K accumulation uses float atomics: results are
-// reproducible to rounding, not bit-exact between runs.  tests/test_backward_gpu.py checks them against
-// autograd through the oracle.
+// parameter blob of the forward (motion_layout).  Split-K partials are added in split order (train_gemm.cuh), no
+// float atomics: the same inputs give the same bits.  tests/test_backward_gpu.py checks them against autograd
+// through the oracle.
 #include "common.cuh"
 #include "linear_f32.cuh"
 #include "linear_tc.cuh"
@@ -68,36 +68,65 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(const GemmArgs a) {
     }
     __syncthreads();
   }
-  const bool atomic = a.accumulate || gridDim.z > 1;
+  // one split: every element has one owner (written, or added once); several: a dense [split, M, N] partial
+  const bool split = gridDim.z > 1;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const long long m = m0 + tm + i, n = n0 + tn + j;
       if (m < a.M && n < a.N) {
-        float* c = a.C + m * a.ldc + n;
-        if (atomic) atomicAdd(c, acc[i][j]);
-        else *c = acc[i][j];
+        if (split) {
+          a.red[((long long)blockIdx.z * a.M + m) * a.N + n] = acc[i][j];
+        } else {
+          float* c = a.C + m * a.ldc + n;
+          *c = a.accumulate ? *c + acc[i][j] : acc[i][j];
+        }
       }
     }
 }
 
+// C[m * ldc + n] (+)= sum_s part[s * sstride + m * N + n], s = 0, 1, ... in order
+__global__ void red_add_kernel(const float* __restrict__ part, int slabs, long long sstride, long long M, long long N,
+                               float* __restrict__ C, long long ldc, int accumulate) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= M * N) return;
+  const long long m = idx / N, n = idx - m * N;
+  float s = part[idx];
+  for (int k = 1; k < slabs; ++k) s += part[k * sstride + idx];
+  float* c = C + m * ldc + n;
+  *c = accumulate ? *c + s : s;
+}
+
 }  // namespace
+
+int launch_red_add(const float* part, int slabs, long long sstride, long long M, long long N, float* C, long long ldc,
+                   bool accumulate, cudaStream_t st) {
+  if (M == 0 || N == 0 || slabs == 0) return DYN_OK;
+  red_add_kernel<<<cdiv(M * N, 256), 256, 0, st>>>(part, slabs, sstride, M, N, C, ldc, accumulate ? 1 : 0);
+  DYN_LAUNCH_CHECK();
+  return DYN_OK;
+}
 
 int launch_gemm(GemmArgs a, bool split_k, cudaStream_t st) {
   if (a.M == 0 || a.N == 0) return DYN_OK;
   int splits = 1;
   if (split_k) {
+    // a split per 4096 rows, at most 128 and at most as many partials as the reduction scratch holds
     const long long want = (a.K + 4095) / 4096;
+    const long long fit = kRedFloats / (a.M * a.N);
     splits = (int)(want < 1 ? 1 : (want > 128 ? 128 : want));
+    if (splits > fit) splits = (int)(fit < 1 ? 1 : fit);
   }
   a.k_per_split = ((a.K + splits - 1) / splits + 15) / 16 * 16;
   if (a.k_per_split == 0) a.k_per_split = 16;
   splits = (int)((a.K + a.k_per_split - 1) / a.k_per_split);
   if (splits < 1) splits = 1;
+  if (splits > 1 && a.red == nullptr) return fail(DYN_E_INVALID, "launch_gemm: a split product needs reduction scratch");
   dim3 grid((unsigned)((a.M + 63) / 64), (unsigned)((a.N + 63) / 64), (unsigned)splits);
   gemm_f32_kernel<<<grid, 256, 0, st>>>(a);
   DYN_LAUNCH_CHECK();
+  if (splits > 1) return launch_red_add(a.red, splits, a.M * a.N, a.M, a.N, a.C, a.ldc, a.accumulate != 0, st);
   return DYN_OK;
 }
 
@@ -113,10 +142,12 @@ __global__ void relu_mask_kernel(float* __restrict__ g, long long ldg, const flo
   if (!(out[idx] > 0.f)) g[r * ldg + c] = 0.f;
 }
 
-// db[c] += sum_r g[r, c]: a block owns 32 columns x a slab of rows
+// sum_r g[r, c] over a slab of rows: a block owns 32 columns x one slab; one slab adds into db[c], several write
+// part[slab, c] for launch_red_add
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ g, long long ldg, int width,
-                                                     long long N, long long rows_per_block, float* __restrict__ db) {
-  __shared__ float part[8][32];
+                                                     long long N, long long rows_per_block, float* __restrict__ db,
+                                                     float* __restrict__ part) {
+  __shared__ float red[8][32];
   const int c = blockIdx.x * 32 + (threadIdx.x & 31);
   const int ry = threadIdx.x >> 5;
   const long long r0 = (long long)blockIdx.y * rows_per_block;
@@ -124,23 +155,30 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ g
   float s = 0.f;
   if (c < width)
     for (long long r = r0 + ry; r < r1; r += 8) s += g[r * ldg + c];
-  part[ry][threadIdx.x & 31] = s;
+  red[ry][threadIdx.x & 31] = s;
   __syncthreads();
   if (ry == 0 && c < width) {
 #pragma unroll
-    for (int i = 1; i < 8; ++i) s += part[i][threadIdx.x & 31];
-    atomicAdd(db + c, s);
+    for (int i = 1; i < 8; ++i) s += red[i][threadIdx.x & 31];
+    if (gridDim.y == 1) db[c] += s;
+    else part[(long long)blockIdx.y * width + c] = s;
   }
 }
 
 }  // namespace
 
-int launch_colsum(const float* g, long long ldg, int width, long long N, float* db, cudaStream_t st) {
+int launch_colsum(const float* g, long long ldg, int width, long long N, float* db, float* red, cudaStream_t st) {
   if (N == 0) return DYN_OK;
+  // slabs of 2048 rows: a call on rows [0, N) and calls on ray slices that start at multiples of 2048 rows form the
+  // same slab sums
   const long long rows_per_block = 2048;
-  dim3 grid((unsigned)((width + 31) / 32), (unsigned)((N + rows_per_block - 1) / rows_per_block));
-  colsum_kernel<<<grid, 256, 0, st>>>(g, ldg, width, N, rows_per_block, db);
+  const long long slabs = (N + rows_per_block - 1) / rows_per_block;
+  if (slabs > 1 && (red == nullptr || slabs * width > kRedFloats))
+    return fail(DYN_E_INVALID, "launch_colsum: %lld slabs of %d columns need reduction scratch", slabs, width);
+  dim3 grid((unsigned)((width + 31) / 32), (unsigned)slabs);
+  colsum_kernel<<<grid, 256, 0, st>>>(g, ldg, width, N, rows_per_block, db, red);
   DYN_LAUNCH_CHECK();
+  if (slabs > 1) return launch_red_add(red, (int)slabs, width, 1, width, db, width, true, st);
   return DYN_OK;
 }
 
@@ -180,6 +218,7 @@ struct TrainBufs {
   float* gw;       // [N,388] dIn of layer 5 (cat([x0, out_4])); reused for the [N,132] dIn of layer 0
   float* gx0;      // [N,132] gradient of x0 through the skip connection
   float* img;      // transposed weight image of the tensor-core dIn product
+  float* red;      // partials of the fixed-order reductions (train_gemm.cuh)
 };
 
 size_t train_alloc(char* base, long long N, TrainBufs* t) {
@@ -197,6 +236,7 @@ size_t train_alloc(char* base, long long N, TrainBufs* t) {
   t->gw = take((size_t)N * 388);
   t->gx0 = take((size_t)N * 132);
   t->img = take(tc_grad_in_scratch_bytes() / sizeof(float));
+  t->red = take((size_t)kRedFloats);
   return off;
 }
 
@@ -247,8 +287,10 @@ int motion_train_backward(const dyn_net* n, const float* xyzt, const float* d_co
   // product helpers on row-major operands
   auto grad_w = [&](const float* dz, long long lddz, int out, const float* in, long long ldin, int width,
                     float* dW, long long lddw) {  // dW[out, width] += dz^T in
-    if (tc && tc_grad_w_ok(out, width, N)) return tc_grad_w(dz, lddz, out, N, in, ldin, width, nullptr, dW, lddw, st);
+    if (tc && tc_grad_w_ok(out, width, N))
+      return tc_grad_w(dz, lddz, out, N, in, ldin, width, nullptr, dW, lddw, t.red, st);
     GemmArgs g{dz, in, dW, out, width, N, 1, lddz, ldin, 1, lddw, 1, 0};
+    g.red = t.red;
     return launch_gemm(g, true, st);
   };
   auto grad_in = [&](const float* dz, long long lddz, int out, const float* W, int in, float* din, long long ldd) {
@@ -263,14 +305,14 @@ int motion_train_backward(const dyn_net* n, const float* xyzt, const float* d_co
   };
   const LinearP& lc = L.coeff;
   MT_RUN(grad_w(d_coeff, lc.out, lc.out, t.out[7], 256, 256, d_params + lc.w, 256));
-  MT_RUN(launch_colsum(d_coeff, lc.out, lc.out, N, d_params + lc.b, st));
+  MT_RUN(launch_colsum(d_coeff, lc.out, lc.out, N, d_params + lc.b, t.red, st));
   float *g = t.ga, *g2 = t.gb;  // dense [N,256]
   MT_RUN(grad_in(d_coeff, lc.out, lc.out, n->params + lc.w, 256, g, 256));
   for (int i = 7; i >= 0; --i) {
     const LinearP& l = L.pts[i];
     relu_mask_kernel<<<(unsigned)((N * 256 + 255) / 256), 256, 0, st>>>(g, 256, t.out[i], 256, N);
     DYN_LAUNCH_CHECK();
-    MT_RUN(launch_colsum(g, 256, 256, N, d_params + l.b, st));
+    MT_RUN(launch_colsum(g, 256, 256, N, d_params + l.b, t.red, st));
     if (i == 5) {  // input cat([x0, out_4]): W is [256, 388]
       MT_RUN(grad_w(g, 256, 256, t.x0, 132, 132, d_params + l.w, 388));
       MT_RUN(grad_w(g, 256, 256, t.out[4], 256, 256, d_params + l.w + 132, 388));

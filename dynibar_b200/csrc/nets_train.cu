@@ -15,8 +15,9 @@
 //                       with the query-row mask quirk, positional encodings, both output heads
 //
 // Gradients of the parameters are ACCUMULATED into d_params (flat, the layout of the blob given to
-// dyn_net_create; the caller zeroes it).  Float atomics: reproducible to rounding, not bit-exact between runs.
-// tests/test_train_gpu.py checks everything against torch autograd through the oracle.
+// dyn_net_create; the caller zeroes it).  No float atomics: every reduction over rows adds per-slab partials in slab
+// order (train_gemm.cuh), so the same inputs give the same bits.  tests/test_train_gpu.py checks everything against
+// torch autograd through the oracle.
 #include <math.h>
 
 #include "common.cuh"
@@ -141,10 +142,15 @@ __global__ void pool2_w_bwd_kernel(const float* __restrict__ vis2, const float* 
 }
 
 // static first pooling weights with anti-aliasing (mlp_network.py:461-467): e_v = exp(|s| (cos_v - 1)),
-// u_v = (e_v - min_v e) mask_v, w = u / (sum u + 1e-8).  In: dw [M].  Out: d/ds accumulated into ds.
-__global__ void aa_w_bwd_kernel(const float* __restrict__ ray_diff, const float* __restrict__ meff,
-                                const float* __restrict__ s_param, const float* __restrict__ dw, long long P,
-                                int V, float* __restrict__ ds) {
+// u_v = (e_v - min_v e) mask_v, w = u / (sum u + 1e-8).  In: dw [M].  Out: this block's share of d/ds in
+// part[blockIdx.x] (its warps' sums in warp order); launch_red_add adds the blocks' shares in block order.
+constexpr int kAaThreads = 256;
+__global__ void __launch_bounds__(kAaThreads) aa_w_bwd_kernel(const float* __restrict__ ray_diff,
+                                                              const float* __restrict__ meff,
+                                                              const float* __restrict__ s_param,
+                                                              const float* __restrict__ dw, long long P, int V,
+                                                              float* __restrict__ part) {
+  __shared__ float wpart[kAaThreads / 32];
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   float contrib = 0.f;
   if (p < P) {
@@ -177,7 +183,14 @@ __global__ void aa_w_bwd_kernel(const float* __restrict__ ray_diff, const float*
     contrib = sv > 0.f ? acc : (sv < 0.f ? -acc : 0.f);  // d|s|/ds, 0 at s = 0 like torch.abs
   }
   contrib = wsum(contrib);
-  if ((threadIdx.x & 31) == 0 && contrib != 0.f) atomicAdd(ds, contrib);
+  if ((threadIdx.x & 31) == 0) wpart[threadIdx.x >> 5] = contrib;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < kAaThreads / 32; ++k) s += wpart[k];
+    part[blockIdx.x] = s;
+  }
 }
 
 // y = x * scale[row] fed a layer: dx[m, c] (+)= ds[m, c] scale[m];  dscale[m] (=) sum_c ds[m, c] x[m, c].  Warp per row.
@@ -222,11 +235,11 @@ __global__ void xv_bwd_kernel(const float* __restrict__ dx2, const float* __rest
 }
 
 // out = LayerNorm(a + resid) w + b (mlp_network.py:100-102), eps 1e-6: dv = d/d(a + resid); dw, db accumulated
-// per block and added once.  A warp walks rows r, r + nwarps, ...
+// per block into part[block] = [dw 128 | db 128] (launch_red_add adds the blocks in order).  A warp walks rows r,
+// r + nwarps, ...
 __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ a, const float* __restrict__ resid,
                                                       const float* __restrict__ w, const float* __restrict__ dy,
-                                                      long long P, float* __restrict__ dv, float* __restrict__ dw,
-                                                      float* __restrict__ db) {
+                                                      long long P, float* __restrict__ dv, float* __restrict__ part) {
   __shared__ float sw[8][128], sb[8][128];
   const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
   const long long nw = (long long)gridDim.x * 8;
@@ -270,8 +283,8 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ a
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) { s1 += sw[k][threadIdx.x]; s2 += sb[k][threadIdx.x]; }
-    atomicAdd(dw + threadIdx.x, s1);
-    atomicAdd(db + threadIdx.x, s2);
+    part[(long long)blockIdx.x * 256 + threadIdx.x] = s1;
+    part[(long long)blockIdx.x * 256 + 128 + threadIdx.x] = s2;
   }
 }
 
@@ -503,7 +516,8 @@ __global__ void st_out_bwd_kernel(const float* __restrict__ draw, const float* _
 }
 
 // dynamic time feature ray_dir_fc(PE(t)) (mlp_network.py:240-244; dyn_time_feat_kernel with keep = 1):
-// saved = [dfeat 35 .. | hidden 256 at 64 | PE(t) 21 at 320], ddfeat[35] = column sums of d feat.  One block.
+// saved = [dfeat 35 .. | hidden 256 at 64 | PE(t) 21 at 320], ddfeat[35] = column sums of d feat.  One block; each
+// gradient element has one owning thread and is added to once.
 __global__ void dyn_time_feat_bwd_kernel(const float* __restrict__ prm, DynamicLayout L,
                                          const float* __restrict__ saved, const float* __restrict__ ddfeat,
                                          float* __restrict__ dprm) {
@@ -520,14 +534,14 @@ __global__ void dyn_time_feat_bwd_kernel(const float* __restrict__ prm, DynamicL
     float dh = 0.f;
     for (int c = 0; c < kF; ++c) {
       dh = fmaf(dz2[c], prm[L.ray_dir2.w + c * 256 + tid], dh);
-      atomicAdd(dprm + L.ray_dir2.w + c * 256 + tid, dz2[c] * hk);
+      dprm[L.ray_dir2.w + c * 256 + tid] += dz2[c] * hk;
     }
     dz0[tid] = dh * (hk > 0.f ? 1.f : hk + 1.f);
-    if (tid < kF) atomicAdd(dprm + L.ray_dir2.b + tid, dz2[tid]);
+    if (tid < kF) dprm[L.ray_dir2.b + tid] += dz2[tid];
   }
   __syncthreads();
-  for (int j = 0; j < 21; ++j) atomicAdd(dprm + L.ray_dir0.w + tid * 21 + j, dz0[tid] * saved[320 + j]);
-  atomicAdd(dprm + L.ray_dir0.b + tid, dz0[tid]);
+  for (int j = 0; j < 21; ++j) dprm[L.ray_dir0.w + tid * 21 + j] += dz0[tid] * saved[320 + j];
+  dprm[L.ray_dir0.b + tid] += dz0[tid];
 }
 
 // static: feat70[:, 35:70] = src_feat * ref_feat[ray] (mlp_network.py:450-452): d src_feat [M,35] and
@@ -574,20 +588,22 @@ struct Prod {
   float* dprm;
   bool tc;      // large products on the tensor cores (train_tc.cu)
   void* img;    // scratch of tc_grad_in
+  float* red;   // reduction scratch (train_gemm.cuh)
   // dW[out, width] (leading dimension ldw, column offset applied by the caller) += dz^T in;
   // in[(row / bdiv) * ldin + c], optionally scaled per row
   int grad_w(const float* dz, long long lddz, int out, long long rows, const float* in, long long ldin, int width,
              float* dW, long long ldw, long long bdiv = 1, const float* kscale = nullptr) const {
     if (tc && bdiv == 1 && width > 256 && tc_grad_w_ok(out, 256, rows)) {  // 257 = 256 + 1: two passes over dz
-      int rc = tc_grad_w(dz, lddz, out, rows, in, ldin, 256, kscale, dW, ldw, st);
+      int rc = tc_grad_w(dz, lddz, out, rows, in, ldin, 256, kscale, dW, ldw, red, st);
       if (rc) return rc;
       return grad_w(dz, lddz, out, rows, in + 256, ldin, width - 256, dW + 256, ldw, 1, kscale);
     }
     if (tc && bdiv == 1 && tc_grad_w_ok(out, width, rows))
-      return tc_grad_w(dz, lddz, out, rows, in, ldin, width, kscale, dW, ldw, st);
+      return tc_grad_w(dz, lddz, out, rows, in, ldin, width, kscale, dW, ldw, red, st);
     GemmArgs g{dz, in, dW, out, width, rows, 1, lddz, ldin, 1, ldw, 1, 0};
     g.bdiv = bdiv;
     g.kscale = kscale;
+    g.red = red;
     return launch_gemm(g, true, st);
   }
   // din[rows, width] (+)= dz[rows, out] W[out, coloff : coloff + width]   (W row-major with ldw columns)
@@ -605,7 +621,7 @@ struct Prod {
   }
   int bias(const float* dz, long long lddz, int out, long long rows, int b_off) const {
     if (b_off < 0) return DYN_OK;
-    return launch_colsum(dz, lddz, out, rows, dprm + b_off, st);
+    return launch_colsum(dz, lddz, out, rows, dprm + b_off, red, st);
   }
   int elu(float* g, long long ldg, const float* out, long long ldo, int width, long long rows, int posenc_S = 0) const {
     if (rows == 0) return DYN_OK;
@@ -640,6 +656,7 @@ struct BwdBufs {
   float *rA, *rB;                                                  // per ray
   float* small;
   float* img;                                                      // tc_grad_in weight image
+  float* red;                                                      // reduction scratch (train_gemm.cuh)
 };
 
 size_t bwd_alloc(Bump& b, bool st_net, int R, int S, int V, BwdBufs* q) {
@@ -658,6 +675,7 @@ size_t bwd_alloc(Bump& b, bool st_net, int R, int S, int V, BwdBufs* q) {
   q->rA = b.f((long long)R * 128); q->rB = b.f((long long)R * 2 * kF);
   q->small = b.f(64);
   q->img = b.f(tc_grad_in_scratch_bytes() / sizeof(float));
+  q->red = b.f(kRedFloats);
   return b.off;
 }
 
@@ -673,10 +691,11 @@ int trunk_backward(const dyn_net* n, const Layout& L, const Prod& pr, const Trun
   const float* prm = pr.prm;
   // LayerNorm(fc(O) + G2) (mlp_network.py:99-102)
   int ln_blocks = cdiv(P, 64);
-  ln_blocks = ln_blocks < 1 ? 1 : (ln_blocks > 1184 ? 1184 : ln_blocks);
-  ln_bwd_kernel<<<ln_blocks, 256, 0, st>>>(
-      t.O2, t.G2, prm + L.ln_w, q.pA, P, q.pB, dprm + L.ln_w, dprm + L.ln_b);
+  ln_blocks = ln_blocks < 1 ? 1 : (ln_blocks > 1184 ? 1184 : ln_blocks);  // 1184 x 256 partials < kRedFloats
+  ln_bwd_kernel<<<ln_blocks, 256, 0, st>>>(t.O2, t.G2, prm + L.ln_w, q.pA, P, q.pB, pr.red);
   DYN_LAUNCH_CHECK();
+  TR(launch_red_add(pr.red, ln_blocks, 256, 1, 128, dprm + L.ln_w, 128, true, st));
+  TR(launch_red_add(pr.red + 128, ln_blocks, 256, 1, 128, dprm + L.ln_b, 128, true, st));
   // q.pB = d/d(O2 + G2): fc has no bias
   TR(pr.grad_w(q.pB, 128, 128, P, t.O, 128, 128, dprm + L.fc.w, 128));
   TR(pr.grad_in(q.pB, 128, 128, P, prm + L.fc.w, 128, 128, q.pA, 128));  // q.pA = dO
@@ -788,7 +807,7 @@ int net_dynamic_backward(const dyn_net* n, const float* pts, const float* rgb_fe
   Bump b2{(char*)scratch, 0};
   BwdBufs q;
   if (bwd_alloc(b2, false, R, S, V, &q) > scratch_bytes) return fail(DYN_E_WORKSPACE, "net backward: scratch too small");
-  const Prod pr{st, n->params, d_params, prec == DYN_PREC_BF16, q.img};
+  const Prod pr{st, n->params, d_params, prec == DYN_PREC_BF16, q.img, q.red};
   const float* prm = n->params;
   float* dprm = d_params;
   // heads (mlp_network.py:294-315)
@@ -831,7 +850,7 @@ int net_dynamic_backward(const dyn_net* n, const float* pts, const float* rgb_fe
     DYN_LAUNCH_CHECK();
   }
   DYN_CUDA(cudaMemsetAsync(q.small, 0, 64 * sizeof(float), st));
-  TR(launch_colsum(q.mF, kF, kF, M, q.small, st));
+  TR(launch_colsum(q.mF, kF, kF, M, q.small, q.red, st));
   dyn_time_feat_bwd_kernel<<<1, 256, 0, st>>>(prm, L, d.dfeat, q.small, dprm);
   DYN_LAUNCH_CHECK();
   return DYN_OK;
@@ -848,7 +867,7 @@ int net_static_backward(const dyn_net* n, const float* rgb_feat, const float* ra
   Bump b2{(char*)scratch, 0};
   BwdBufs q;
   if (bwd_alloc(b2, true, R, S, V, &q) > scratch_bytes) return fail(DYN_E_WORKSPACE, "net backward: scratch too small");
-  const Prod pr{st, n->params, d_params, prec == DYN_PREC_BF16, q.img};
+  const Prod pr{st, n->params, d_params, prec == DYN_PREC_BF16, q.img, q.red};
   const float* prm = n->params;
   float* dprm = d_params;
   // blending head (mlp_network.py:508-526)
@@ -879,9 +898,12 @@ int net_static_backward(const dyn_net* n, const float* rgb_feat, const float* ra
   pool_bwd_kernel<<<cdiv(P * 32, 256), 256, 0, st>>>(d.feat70, 2 * kF, 2 * kF, d.w1, d.mv, 4 * kF, q.pMV, 4 * kF, P, V,
                                                      q.mF, 2 * kF, 1, q.mS2, 1);
   DYN_LAUNCH_CHECK();
-  if (n->anti_alias) {
-    aa_w_bwd_kernel<<<cdiv(P, 256), 256, 0, st>>>(ray_diff, d.meff, prm + L.s, q.mS2, P, V, dprm + L.s);
+  if (n->anti_alias && P > 0) {
+    const long long blocks = cdiv(P, kAaThreads);
+    if (blocks > kRedFloats) return fail(DYN_E_INVALID, "net backward: %lld points exceed the reduction scratch", P);
+    aa_w_bwd_kernel<<<(unsigned)blocks, kAaThreads, 0, st>>>(ray_diff, d.meff, prm + L.s, q.mS2, P, V, q.red);
     DYN_LAUNCH_CHECK();
+    TR(launch_red_add(q.red, (int)blocks, 1, 1, 1, dprm + L.s, 1, true, st));
   }
   if (d_rgb_feat != nullptr) {
     feat_out_kernel<<<cdiv(M * kF, 256), 256, 0, st>>>(q.mF, 2 * kF, M, 3, d_rgb_feat);

@@ -11,8 +11,9 @@
 // 8 consecutive columns of one row per store; 8 consecutive rows form one 128-byte core matrix whose CONTIGUOUS
 // dimension is M / N, i.e. the canonical MN-major no-swizzle layout: LBO = 128 B between 8-row groups along K,
 // SBO = 64 * 16 B between 8-column groups along M / N); warpgroup g multiplies rows 64 g .. of the tile with wgmma (both
-// operands MN-major) over a 2-stage ring; its accumulators live in registers for the whole slab and
-// are added to dW with float atomics at the end.
+// operands MN-major) over a 2-stage ring; its accumulators live in registers for the whole slab and are stored as
+// that slab's partial dW tile.  A second pass (launch_red_add) adds the slabs' partials into dW in slab order.  The
+// slab count is a function of the shape alone: the same inputs give the same bits on every H100.
 #include "linear_tc.cuh"
 #include "tc.cuh"
 #include "train_gemm.cuh"
@@ -33,7 +34,7 @@ struct GradWArgs {
   const float* x; long long ldx; int width;
   const float* kscale;
   long long rows, rows_per_cta;
-  float* dW; long long ldw;
+  float* part;  // [slab, out, width] partials
   int mtiles, nblocks;
 };
 
@@ -137,7 +138,8 @@ __global__ void __launch_bounds__(256, 1) grad_w_tc_kernel(const __grid_constant
   }
   if (nstages == 0) return;
 
-  // ---------------- epilogue: fragment -> dW (float atomics) ----------------
+  // ---------------- epilogue: fragment -> this slab's partial ----------------
+  float* part = a.part + (long long)blockIdx.x * a.out * a.width;
   const int w = warp & 3;
 #pragma unroll
   for (int b = 0; b < 2; ++b) {
@@ -151,7 +153,7 @@ __global__ void __launch_bounds__(256, 1) grad_w_tc_kernel(const __grid_constant
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int c = n0 + 64 * b + 8 * j + 2 * (lane & 3) + e;
-          if (c < a.width) atomicAdd(a.dW + (long long)o * a.ldw + c, acc[b][4 * j + 2 * h + e]);
+          if (c < a.width) part[(long long)o * a.width + c] = acc[b][4 * j + 2 * h + e];
         }
       }
     }
@@ -181,21 +183,20 @@ bool tc_grad_in_ok(int out, int width, long long rows) { return width >= 16 && w
 size_t tc_grad_in_scratch_bytes() { return tc_packed_bytes(256, 320); }
 
 int tc_grad_w(const float* dz, long long lddz, int out, long long rows, const float* x, long long ldx, int width,
-              const float* kscale, float* dW, long long ldw, cudaStream_t st) {
+              const float* kscale, float* dW, long long ldw, float* red, cudaStream_t st) {
   if (rows == 0) return DYN_OK;
   if (!tc_grad_w_ok(out, width, rows)) return fail(DYN_E_INVALID, "tc_grad_w: unsupported shape %d x %d", out, width);
+  if (red == nullptr) return fail(DYN_E_INVALID, "tc_grad_w: no reduction scratch");
   GradWArgs a;
   a.dz = dz; a.lddz = lddz; a.out = out; a.x = x; a.ldx = ldx; a.width = width; a.kscale = kscale;
-  a.rows = rows; a.dW = dW; a.ldw = ldw;
+  a.rows = rows; a.part = red;
   a.mtiles = (out + kTileM - 1) / kTileM;
   a.nblocks = (width + kTileN - 1) / kTileN;
-  // slabs: one wave of CTAs over all dW tiles, at least 1024 rows each: the epilogue adds a dW tile per CTA with
-  // atomics
-  int dev = 0, sms = 0;
-  DYN_CUDA(cudaGetDevice(&dev));
-  DYN_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  // slabs: about one wave of kGwCtas CTAs (an H100 has 132 SMs) over all dW tiles, at least 1024 rows each.  tiles is
+  // 1, 2 or 4, so slabs * out * width <= kGwCtas * 128 * 128 = kRedFloats.
+  constexpr int kGwCtas = 128;
   const int tiles = a.mtiles * a.nblocks;
-  long long slabs = (sms + tiles - 1) / tiles;
+  long long slabs = kGwCtas / tiles;
   long long per = (rows + slabs - 1) / slabs;
   per = per < 1024 ? 1024 : per;
   per = (per + kRowsStage - 1) / kRowsStage * kRowsStage;
@@ -205,10 +206,12 @@ int tc_grad_w(const float* dz, long long lddz, int out, long long rows, const fl
     DYN_CUDA(cudaFuncSetAttribute(grad_w_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGwSmem));
     attr_set = true;
   }
-  const dim3 grid((unsigned)((rows + per - 1) / per), (unsigned)tiles);
+  const long long nslabs = (rows + per - 1) / per;
+  if (nslabs * out * width > kRedFloats) return fail(DYN_E_INVALID, "tc_grad_w: partials exceed the reduction scratch");
+  const dim3 grid((unsigned)nslabs, (unsigned)tiles);
   grad_w_tc_kernel<<<grid, 256, kGwSmem, st>>>(a);
   DYN_LAUNCH_CHECK();
-  return DYN_OK;
+  return launch_red_add(red, (int)nslabs, (long long)out * width, out, width, dW, ldw, true, st);
 }
 
 int tc_grad_in(const float* dz, long long lddz, int out, long long rows, const float* W, long long ldw, int width,
@@ -231,10 +234,17 @@ int tc_grad_in(const float* dz, long long lddz, int out, long long rows, const f
 using namespace dyn;
 
 // unit-test hooks (tests/test_train_gpu.py): plain fp32 matrices in and out
+// The slab partials live in a stream-ordered allocation of this hook's own (the library's entry points take them from
+// the caller's scratch).
 extern "C" int dyn_debug_tc_grad_w(const float* dz, int lddz, int out, int rows, const float* x, int ldx, int width,
                                    const float* kscale, float* dW, int ldw, void* stream) {
   DYN_CHECK_ARG(dz && x && dW);
-  return tc_grad_w(dz, lddz, out, rows, x, ldx, width, kscale, dW, ldw, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  void* red = nullptr;
+  DYN_CUDA(cudaMallocAsync(&red, red_scratch_bytes(), st));
+  const int rc = tc_grad_w(dz, lddz, out, rows, x, ldx, width, kscale, dW, ldw, (float*)red, st);
+  DYN_CUDA(cudaFreeAsync(red, st));
+  return rc;
 }
 
 extern "C" int dyn_debug_tc_grad_in(const float* dz, int lddz, int out, int rows, const float* W, int ldw, int width,

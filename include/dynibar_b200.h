@@ -33,6 +33,12 @@
  *     from a train forward to its backward and must be passed unchanged.
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it,
  *     nothing synchronises.
+ *   - determinism: no entry point adds floats with atomics.  Reductions over
+ *     rows write per-slab partials that a second pass adds in slab order,
+ *     and every slab partition is a function of the shapes alone (never of
+ *     the SM count), so the same inputs give the same bits, the training
+ *     backwards included.  An accumulating output receives one add per
+ *     element per call.
  *   - return 0 on success, a negative DYN_E_* otherwise; `dyn_last_error()`
  *     returns a thread-local message.  No C++ exceptions cross the ABI.
  *   - R rays, S samples per ray, V source views, C feature channels (32),
@@ -343,8 +349,11 @@ int dyn_flow_sceneflow(const float* weights, const float* pts_seq,
  * rgb_dy, depth, mask(ignored)), g_samples [5,R,S] = d/d(alpha_dy, weights_dy, weights_st, alpha,
  * weights) or NULL -> g_raw_dy, g_raw_st [R,S,4].  S <= 256.
  * dyn_project_gather_backward: compute_with_motions (projection.py:103-176).  g_rgb_feat [R,S,V,3+C]
- * -> g_featmaps [V,C,h,w] (reference layout; zeroed here, atomically accumulated) and / or g_xyz [V,R,S,3]
- * (either may be NULL).  xyz may be NULL (every view uses xyz_st). */
+ * -> g_featmaps [V,C,h,w] (reference layout; written whole) and / or g_xyz [V,R,S,3] (either may be NULL).
+ * xyz may be NULL (every view uses xyz_st).  The feature-map gradient is a gather: the (view, point) pairs are
+ * radix-sorted by the texel cell they sample, and each texel adds its pairs in pair order; `workspace`
+ * (dyn_project_gather_backward_workspace_bytes(V, R, S, h, w) bytes; computed with the device's sort, 0 for an
+ * unsupported shape) is needed only when g_featmaps is not NULL. */
 int dyn_composite_backward(const float* raw_dy, const float* raw_st, const float* z_vals,
                            const float* g_rays, const float* g_samples, int R, int S,
                            float* g_raw_dy, float* g_raw_st, void* stream);
@@ -352,14 +361,15 @@ int dyn_project_gather_backward(const float* xyz_st, const float* xyz, const flo
                                 const float* src_cams, const float* featmaps,
                                 const float* g_rgb_feat, int V, int R, int S, int H, int W,
                                 int C, int h, int w, float* g_featmaps, float* g_xyz,
-                                void* stream);
+                                void* workspace, size_t workspace_bytes, void* stream);
+size_t dyn_project_gather_backward_workspace_bytes(int V, int R, int S, int h, int w);
 
 /* MotionMLP training slice (ibrnet/mlp_network.py:605-618; gradients as torch.autograd would produce them
  * for MotionMLP.forward).  The forward keeps the embedding and the eight post-ReLU activations in `saved`
  * (dyn_motion_train_workspace_bytes(N) bytes, also scratch for the backward).  The backward ACCUMULATES
  * d(loss)/d(params) into d_params (flat, the n_params floats of dyn_net_create, same layout as the
  * blob given to dyn_net_create; the caller zeroes it) and writes d(loss)/d(xyzt) [N,4] unless d_xyzt is NULL.
- * fp32; split-K float atomics (not bit-reproducible between runs). */
+ * fp32 (bf16 tensor-core products with DYN_PREC_BF16); split-K partials added in split order: bit-reproducible. */
 size_t dyn_motion_train_workspace_bytes(int N);
 int dyn_motion_mlp_train_forward(dyn_net_t motion, const float* xyzt, int N, float* coeff, void* saved,
                                  size_t saved_bytes, int precision, void* stream);
@@ -377,7 +387,7 @@ int dyn_motion_mlp_backward(dyn_net_t motion, const float* xyzt, const float* d_
  * no gradient (the reference detaches them).  `precision`: DYN_PREC_FP32 = SIMT products; DYN_PREC_BF16 = the
  * products of the large layers on the tensor cores (bf16 operands, fp32 accumulation, fp32 master weights / gradients; the
  * net must have been created with layer images, dyn_net_create_ex pack_level >= 1); everything else stays fp32.
- * Float atomics (not bit-reproducible between runs). */
+ * No float atomics: bit-reproducible. */
 size_t dyn_net_train_workspace_bytes(int kind, int R, int S, int V);
 size_t dyn_net_backward_scratch_bytes(int kind, int R, int S, int V);
 int dyn_net_dynamic_train_forward(dyn_net_t net, const float* pts, const float* rgb_feat, const float* ray_dir,
@@ -528,7 +538,8 @@ int dyn_mono_loss_finish(const float* partial, int nblocks, const dyn_mono_loss_
                          int K, int n_sf, float* out, void* stream);
 
 /* Unit-test hooks of the tensor-core training products (csrc/train_tc.cu; bf16 operands, fp32 accumulation):
- * dyn_debug_tc_grad_w: dW[out,width] += dz[rows,out]^T (x[rows,width] * kscale[rows] or 1); out, width <= 256.
+ * dyn_debug_tc_grad_w: dW[out,width] += dz[rows,out]^T (x[rows,width] * kscale[rows] or 1); out, width <= 256
+ *   (its slab partials in a stream-ordered allocation of its own, cudaMallocAsync / cudaFreeAsync on `stream`).
  * dyn_debug_tc_grad_in: din[rows,width] = dz[rows,out] W[out, 0:width] (W row-major with ldw columns). */
 int dyn_debug_tc_grad_w(const float* dz, int lddz, int out, int rows, const float* x, int ldx, int width,
                         const float* kscale, float* dW, int ldw, void* stream);

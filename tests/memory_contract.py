@@ -150,17 +150,3 @@ def assert_bit_identical(runs, what):
         raise AssertionError("%s: %s of run %s differs from run %s in %d of %d elements (max |diff| %s, %d non-finite)"
                              % (what, k, label, base_label, int((bits(g) != bits(v)).sum()), v.numel(),
                                 d.max().item() if d.numel() else 0, int((~torch.isfinite(g.double())).sum())))
-
-
-def global_rel_l2(got, base):
-  """||got - base|| / ||base|| over all tensors of two flat dicts taken as one vector, and the key holding the largest
-  share of the difference."""
-  num = {k: (got[k].double() - v.double()).norm().item() ** 2 for k, v in base.items()}
-  den = sum(v.double().norm().item() ** 2 for v in base.values())
-  worst = max(num, key=num.get)
-  return (sum(num.values()) / max(den, 1e-300)) ** 0.5, worst
-
-
-# floor of the spread, relative L2: one fp32 unit in the last place (two 0x00 runs whose float atomics happened to add
-# in the same order show a spread of exactly 0)
-SPREAD_FLOOR = 2.0 ** -23

@@ -323,7 +323,8 @@ def test_training_ray_slices_match_one_call(monkeypatch):
     if not results:
       gens = {(o, k): torch.randn(got[o][k].shape, generator=g).to(dev) for o, ks in _TRAIN_KEYS.items() for k in ks}
     sum((got[o][k] * v).sum() for (o, k), v in gens.items()).backward()
-    # (`s`: ill-conditioned sum, see above -- its value depends on the summation order)
+    # (`s`: ill-conditioned sum, see above.  Slices add its terms in another order than one call does, so its value
+    # moves with the slicing; two identical calls agree bit for bit, tests/test_train_determinism_gpu.py)
     results.append((got, [p.grad.clone() for mod in mods for k, p in mod.named_parameters() if k != "s"],
                     [f.grad.clone() for f in fd]))
   (a, ga, fa), (bb, gb, fb) = results

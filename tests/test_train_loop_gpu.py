@@ -2,12 +2,11 @@
 (tests/mono_scene_ref.write_scene: 8 frames of 48 x 64, 512 rays in 256-ray slices, 32 samples, bf16).
 
   1. The loop against the same steps written out by hand from MonocularScene.sample, mono_step_backward and Adam,
-     across the warm-up / main boundary: batches, epochs and per-group learning rates bit for bit; parameters within
-     2x the spread of two identical hand runs (relative L2 per optimiser group, SPREAD_BARS; the network backward's
-     float atomics make runs differ in the last bits, and Adam carries that forward).
+     across the warm-up / main boundary: batches, epochs, per-group learning rates and every parameter bit for bit
+     (the training backward adds in a fixed order, so the same steps give the same bits).
   2. Resume: k steps, save, a new Trainer from the file, m more steps, against k + m uninterrupted steps (inside the
      warm-up, and in the main phase): the same data stream, epochs, learning rates, scheduler state and Adam step counts;
-     parameters within the same bar.
+     parameters and Adam moments bit for bit.
   3. save -> load -> save gives identical tensors.
   4. The checkpoint renders through tools/render_monocular_bt.py's loading path, as the trainer's own model does.
   5. Under torch.cuda.set_sync_debug_mode("warn"): a loop step that neither logs, saves nor renders synchronises no
@@ -154,20 +153,19 @@ def _same_stream(got, want):
     assert torch.equal(g["rays"], w["rays"]) and torch.equal(g["views"], w["views"]), k
 
 
-# relative L2 per optimiser group: 2x the largest spread of two identical runs measured over five calls of tests 1 and
-# 2 on an H100 80GB HBM3 (700 W power limit).  One pair's spread varies up to 10x from call to call (motion_mlp
-# 2.8e-5 .. 2.9e-4), so each test's own pair only widens the bar.
-SPREAD_BARS = {"net_coarse_st": 2.4e-4, "feature_net_st": 9e-4, "net_coarse_dy": 2.7e-4, "feature_net": 1.3e-3,
-               "motion_mlp": 6e-4, "trajectory_basis": 1.7e-4}
-
-
-def _within_spread(got, ref, ref2, what):
-  spread, err = _rel(ref2, ref), _rel(got, ref)
+def _bit_identical(got, want, what):
+  """Every optimiser group's parameters, and (optimizers given) every Adam moment, equal bit for bit."""
   names = [g[0] for g in tr.GROUPS]
-  for n, s, e in zip(names, spread, err):
-    print("  %s %-15s spread %.3e  difference %.3e" % (what, n, s, e))
-  bad = [(n, e, s) for n, s, e in zip(names, spread, err) if not e <= max(2.0 * s, SPREAD_BARS[n])]
-  assert not bad, bad
+  diff = _rel(_groups(got), _groups(want))
+  bad = [(n, d) for n, a, b, d in zip(names, _groups(got), _groups(want), diff) if not torch.equal(a, b)]
+  assert not bad, "%s: groups differ (relative L2): %s" % (what, bad)
+  for k, (g1, g2) in enumerate(zip(got.param_groups, want.param_groups)):
+    for p1, p2 in zip(g1["params"], g2["params"]):
+      s1, s2 = got.state.get(p1), want.state.get(p2)
+      assert (s1 is None) == (s2 is None), (what, names[k])
+      if s1 is not None:
+        for key in ("exp_avg", "exp_avg_sq"):
+          assert torch.equal(s1[key], s2[key]), (what, names[k], key)
 
 
 def test_loop_matches_the_hand_written_steps(scene):
@@ -179,19 +177,16 @@ def test_loop_matches_the_hand_written_steps(scene):
   schedule = [("warmup", 0, False)] * N + [("main", 0, True)] * 3
   assert [(r["bootstrap"], r["epoch"]) for r in t.record] == [(p == "warmup", e) for p, e, _ in schedule]
   _, opt1, sched1, rec1 = hand_run(scene, args, init, schedule)
-  _, opt2, _, _ = hand_run(scene, args, init, schedule)
   _same_stream(t.record, rec1)
   assert t.scheduler.state_dict() == sched1.state_dict() and t.global_step == N + 3
-  _within_spread(_groups(t.optimizer), _groups(opt1), _groups(opt2), "loop-vs-hand")
+  _bit_identical(t.optimizer, opt1, "loop-vs-hand")
 
 
 @pytest.mark.parametrize("ide,k,m", [(4, N, 4), (1, N, 3)], ids=["in_warmup", "main"])
 def test_resume_continues_the_run(scene, tmp_path, ide, k, m):
   args = _args(init_decay_epoch=ide)
-  whole = []
-  for _ in range(2):  # one after the other: each run starts from the seeded generators
-    whole.append(_fresh(scene, args))
-    whole[-1].run(k + m)
+  whole = [_fresh(scene, args)]
+  whole[0].run(k + m)
   first = _fresh(scene, args)
   first.run(k)
   path = str(tmp_path / "model_latest.pth")
@@ -212,8 +207,7 @@ def test_resume_continues_the_run(scene, tmp_path, ide, k, m):
         assert int(s1["step"]) == int(s2["step"])
         counts.add(int(s1["step"]))
   assert k + m in counts
-  _within_spread(_groups(second.optimizer), _groups(whole[0].optimizer), _groups(whole[1].optimizer),
-                 "resumed-vs-whole")
+  _bit_identical(second.optimizer, whole[0].optimizer, "resumed-vs-whole")
 
 
 def _tensors(x, prefix=""):
